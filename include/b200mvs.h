@@ -96,7 +96,7 @@ typedef struct {
 	                        per direction); 4 front kernel (fused directions, auto default for uniform ranges) */
 	int sgmCost;         /* 0 auto (tensor-core kernel for dense volumes with one range of 64 / 128 / 192 / 256 disparities, SIMT otherwise);
 	                        1 SIMT cost kernel; 2 tensor-core (wgmma) cost kernel or an error */
-	int sweepFourCtas;   /* 1: the 64-register instantiation of the sweep kernel (4 CTAs per SM instead of 3) */
+	int sweepFourCtas;   /* reserved, ignored: the sweep kernel has one instantiation (80 registers, 3 CTAs per SM, no spills) */
 	int frontLayout;     /* wave-front aggregation: 0 auto; 1 two tilted fronts +-(x+2y), four directions each; 2 four straight
 	                        fronts; 3 eight passes of one direction */
 	int frontSerial;     /* 1: one pass per launch into one sum volume (default: two passes share a launch, each with its own

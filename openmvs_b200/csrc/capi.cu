@@ -19,7 +19,7 @@
 
 cudaError_t pm_configure_device();
 cudaError_t pm_launch_score(const PMParams& P, bool geom, cudaStream_t s);
-cudaError_t pm_launch_sweep(const PMParams& P, const void* tmapRef, bool geom, bool fourCtas, cudaStream_t s);
+cudaError_t pm_launch_sweep(const PMParams& P, const void* tmapRef, bool geom, cudaStream_t s);
 void pm_tma_box(int* w, int* h);
 cudaError_t pm_launch_finalize(int n, float keep, const float4* plane, const float* cost, const uint32_t* bestViews,
 	float* depth, float* normal, float* conf, uint32_t* viewsMap, cudaStream_t s);
@@ -326,7 +326,7 @@ int launch_sweep_timed(b200mvs_ctx* ctx, const PMParams& P, bool geom, cudaStrea
 		}
 		CK(cudaEventRecord(ctx->sweepEv[2*ctx->nSweepEv], s));
 	}
-	CK(pm_launch_sweep(P, ctx->tmapValid ? &ctx->tmapRef : nullptr, geom, ctx->dbg.sweepFourCtas != 0, s)); ++ctx->launches;
+	CK(pm_launch_sweep(P, ctx->tmapValid ? &ctx->tmapRef : nullptr, geom, s)); ++ctx->launches;
 	if (ctx->timeSweeps) {
 		CK(cudaEventRecord(ctx->sweepEv[2*ctx->nSweepEv+1], s));
 		++ctx->nSweepEv;
@@ -893,7 +893,7 @@ int b200mvs_pm_sweep(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, fl
 	for (int colour = 0; colour < 2; ++colour) {
 		if (half >= 0 && half != colour) continue;
 		P.colour = colour;
-		CK(pm_launch_sweep(P, ctx->tmapValid ? &ctx->tmapRef : nullptr, geom, ctx->dbg.sweepFourCtas != 0, s));
+		CK(pm_launch_sweep(P, ctx->tmapValid ? &ctx->tmapRef : nullptr, geom, s));
 	}
 	return B200MVS_OK;
 }
