@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define B200MVS_ABI_VERSION 5 /* struct layouts of this header; b200mvs_abi_version() returns the library's */
+#define B200MVS_ABI_VERSION 6 /* struct layouts of this header; b200mvs_abi_version() returns the library's */
 #define B200MVS_MAX_VIEWS 32 /* neighbours per reference view (MAX_VIEWS, PatchMatchCUDA.inl:35) */
 
 typedef struct b200mvs_ctx b200mvs_ctx;
@@ -249,6 +249,70 @@ int b200mvs_sgm_cross_check_device(b200mvs_ctx* ctx, int16_t* l2r, const int16_t
  * accums = NULL uses the accumulated costs of the last match on this context. */
 int b200mvs_sgm_refine_device(b200mvs_ctx* ctx, const b200mvs_sgm_pixel* pixels, const uint16_t* accums,
 	int16_t* disparity, int nPixels, int subpixelSteps, void* stream);
+
+/* ---- hierarchical (tSGM) matching of a rectified pair: SemiGlobalMatcher::Match(scene, idxImage, numNeighbors, minResolution)
+ * (libs/MVS/SemiGlobalMatcher.cpp:583-718) from the rectified pair to the left disparity and cost maps it exports ----------------
+ * Levels: minResolution > 0 gives level = Image8U::computeMaxResolution(width, height, 8, minResolution) (libs/Common/Types.inl:2459-2477)
+ * and the scales 1/max(2, 2^level), doubled until 1; the level sizes are round(width * scale) x round(height * scale) (computeResize,
+ * Types.inl:2440-2445).  minResolution = 0: one full-resolution level with one global range (the non-tSGM branch).
+ * b200mvs_sgm_levels is host code: *numLevels, the level sizes coarsest first (arrays of B200MVS_SGM_MAX_LEVELS entries, nullable) and
+ * the size of the initial disparity map, the valid region (-6) of computeResize(coarsest size, 0.5). */
+#define B200MVS_SGM_MAX_LEVELS 9
+int b200mvs_sgm_levels(int width, int height, int minResolution, int* numLevels, int* levelWidths, int* levelHeights,
+	int* initWidth, int* initHeight);
+
+/* The level loop, DEVICE pointers, all on `stream` (NULL: the context's stream).  Inputs as b200mvs_sgm_match takes them, plus the right
+ * colour image: gray float, BGR uint8, width x height.  At every level both images are resized from the full-resolution ones with
+ * INTER_AREA (ViewData::GetImage, SemiGlobalMatcher.h:127-142); then, as the reference does:
+ *   first level: masks resized NEAREST to the level and cropped to the valid region; later levels: UpscaleMask;
+ *   tSGM: FlipDirection(left -> right), Disparity2RangeMap(right, rightMask, first ? 11 : 5, first ? 33 : 7), match right -> left,
+ *         Disparity2RangeMap(left, leftMask, ...), match left -> right;
+ *   minResolution = 0: the range [2 min - 16, 2 max + 16) of the initial map's valid values for the right -> left match and its mirror
+ *         for the left -> right match (SemiGlobalMatcher.cpp:643-683; at most 256 disparities);
+ *   first level: cross-check left, then right against the checked left, filterSpeckles(NO_DISP, nSpeckleSize, 5) and ExtractMask
+ *         (thValid 3) of both; later levels: cross-check of the left map;
+ *   end: RefineDisparityMap of the left map with the accumulated costs of the last left match.
+ * initDisparity (nullable: all NO_DISP = 32767): int16, initWidth x initHeight as b200mvs_sgm_levels gives them, left disparities in pixels
+ * of half the coarsest level (the reference triangulates it from the sparse points, :608-625).  With minResolution = 0 it must hold a
+ * valid value (B200MVS_ERR_ARG otherwise).  leftMask / rightMask (nullable: all valid): uint8, width x height, 0 = invalid.
+ * Outputs over the valid region (width-6) x (height-6): outDisparity = round(left disparity * subpixelSteps) (NO_DISP where invalid),
+ * outCost = the summed path cost of the last left match (uint16).  numCostsPerLevel (nullable, >= 2 x levels entries): the volume size
+ * of the right and of the left match of every level.
+ * Host reads: each match reads its pixel-map statistics back (b200mvs_sgm_match_device), and each Disparity2RangeMap its 8-byte
+ * numCosts, which sizes the cost volume; the call returns after the work is done.  The context's "last match" is cleared: a following
+ * b200mvs_sgm_refine_device(accums = NULL) fails until the next b200mvs_sgm_match_device. */
+int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
+	const float* leftGray, const uint8_t* leftBGR, const float* rightGray, const uint8_t* rightBGR, int width, int height,
+	const int16_t* initDisparity, int initWidth, int initHeight, const uint8_t* leftMask, const uint8_t* rightMask,
+	int minResolution, int nSpeckleSize, int thCross, int subpixelSteps, const b200mvs_sgm_params* prm,
+	int16_t* outDisparity, uint16_t* outCost, uint64_t* numCostsPerLevel, void* stream);
+
+/* Building blocks of the level loop (DEVICE pointers; stream NULL = the context's stream), exposed for parity tests.
+ * Disparity2RangeMap (SemiGlobalMatcher.cpp:1350-1444): the per-pixel ranges and idx offsets of the 2x grid maskWidth x maskHeight
+ * (the next level's valid region) from the width x height disparity map; the mask is read at (2r+3, 2c+3).  Synchronises `stream`
+ * once to return *numCosts (host). */
+int b200mvs_sgm_range_map_device(b200mvs_ctx* ctx, const int16_t* disparity, int width, int height, const uint8_t* mask,
+	int maskWidth, int maskHeight, int minNumDisp, int minNumDispInvalid, b200mvs_sgm_pixel* pixels, uint64_t* numCosts, void* stream);
+/* FlipDirection (SemiGlobalMatcher.cpp:1630-1657): r2l = NO_DISP, then -d at columns c+d-1 .. c+d+1 of every valid l2r pixel, the
+ * largest c winning a column like the reference's sequential loop; r2l must not alias l2r */
+int b200mvs_sgm_flip_direction_device(b200mvs_ctx* ctx, const int16_t* l2r, int16_t* r2l, int width, int height, void* stream);
+/* UpscaleMask (SemiGlobalMatcher.cpp:1662-1690): width x height -> width2x x height2x, pixel (r, c) to the 2x2 block at (2r+3, 2c+3) */
+int b200mvs_sgm_upscale_mask_device(b200mvs_ctx* ctx, const uint8_t* mask, int width, int height, uint8_t* mask2x,
+	int width2x, int height2x, void* stream);
+/* ExtractMask (SemiGlobalMatcher.cpp:1518-1576), mask in place (same size as the disparity map) */
+int b200mvs_sgm_extract_mask_device(b200mvs_ctx* ctx, const int16_t* disparity, uint8_t* mask, int width, int height, int thValid,
+	void* stream);
+/* cv::filterSpeckles(disparity, newVal, maxSpeckleSize, maxDiff) on an int16 map, in place: every 4-connected region of pixels
+ * != newVal whose neighbours differ by at most maxDiff and that has at most maxSpeckleSize pixels becomes newVal */
+int b200mvs_sgm_filter_speckles_device(b200mvs_ctx* ctx, int16_t* disparity, int width, int height, int newVal, int maxSpeckleSize,
+	int maxDiff, void* stream);
+/* The level inputs: cv::resize(src, Size(), 1/factor, 1/factor, INTER_AREA) of an 8-bit image with 1, 3 or 4 interleaved channels
+ * (dst: round(width/factor) x round(height/factor), packed), and the first level's mask: cv::resize(mask, levelWidth x levelHeight,
+ * INTER_NEAREST) cropped to the valid region at (3, 3) (SemiGlobalMatcher.cpp:627-631; validMask: (levelWidth-6) x (levelHeight-6)). */
+int b200mvs_resize_area_u8_device(b200mvs_ctx* ctx, const uint8_t* src, int width, int height, int channels, int factor, uint8_t* dst,
+	void* stream);
+int b200mvs_sgm_level_mask_device(b200mvs_ctx* ctx, const uint8_t* mask, int width, int height, int levelWidth, int levelHeight,
+	uint8_t* validMask, void* stream);
 
 /* ---- depth-map post-processing after the estimation (SURVEY.md §8(f) rank 2) -----------------
  * DepthMapsData::FilterDepthMap / RemoveSmallSegments / GapInterpolation

@@ -52,6 +52,18 @@ cudaError_t sgm_launch_wta_uniform(const SGMParams& P, const uint16_t* second, i
 int sgm_max_disparities();
 cudaError_t sgm_launch_cross_check(int16_t* l2r, const int16_t* r2l, int w, int h, int th, cudaStream_t s);
 cudaError_t sgm_launch_refine(const SGMPixel* px, const uint16_t* accums, int16_t* disparity, int n, int steps, cudaStream_t s);
+// hierarchical level loop (sgm_tsgm.cu)
+size_t tsgm_range_map_scratch(size_t n);
+cudaError_t tsgm_launch_range_map(const int16_t* D, int W, int H, const uint8_t* mask, int W2, int H2, int minNumDisp, int minNumDispInvalid,
+	short2* ranges, SGMPixel* px, void* scratch, unsigned long long* total, cudaStream_t s);
+cudaError_t tsgm_launch_flip(const int16_t* l2r, int16_t* r2l, int W, int H, unsigned* keys, cudaStream_t s);
+cudaError_t tsgm_launch_upscale_mask(const uint8_t* m, int W, int H, uint8_t* m2, int W2, int H2, cudaStream_t s);
+cudaError_t tsgm_launch_extract_mask(const int16_t* D, uint8_t* M, int W, int H, int thValid, cudaStream_t s);
+cudaError_t tsgm_launch_speckles(int16_t* D, int W, int H, int newVal, int maxSpeckleSize, int maxDiff, int* labels, int* sizes, cudaStream_t s);
+cudaError_t tsgm_launch_area_u8(const uint8_t* src, int sw, int sh, int cn, uint8_t* dst, int dw, int dh, int k, cudaStream_t s);
+cudaError_t tsgm_launch_fill(int16_t* d, size_t n, int16_t v, cudaStream_t s);
+cudaError_t tsgm_launch_minmax(const int16_t* d, size_t n, int* out2, cudaStream_t s);
+cudaError_t tsgm_launch_dense_map(SGMPixel* px, size_t n, int lo, int hi, cudaStream_t s);
 #define FLT_MAX_NBR 16
 struct FltView { const float* depth; const float* conf; int w, h; double fx, fy, cx, cy; double R[9], C[3]; };
 struct FltParams {
@@ -151,6 +163,10 @@ struct b200mvs_ctx {
 	cudaStream_t sgSide[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // side streams of the ragged aggregation
 	cudaEvent_t sgJoin[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}, sgFork = nullptr;
 	const void* sgLastPx = nullptr; uint64_t sgLastNum = 0; // pixel map / size of the volume in sgAccums (b200mvs_sgm_refine_device check)
+	// hierarchical matcher: level images, masks, disparity maps, pixel maps, Disparity2RangeMap / FlipDirection / speckle scratch
+	enum { TS_IMG, TS_MASKL, TS_MASKR, TS_MASKT, TS_DL, TS_DR, TS_DL0, TS_DR0, TS_PXL, TS_PXR, TS_RANGES, TS_SCAN, TS_KEYS, TS_LABELS,
+		TS_SIZES, TS_SMALL, TS_COUNT };
+	DevBuf ts[TS_COUNT];
 	DevBuf fltZ, fltIn, fltOutD, fltOutC;     // FilterDepthMap: z-buffer keys, staged maps (host API), outputs
 	DevBuf ppA, ppB, ppD, ppN, ppC;           // RemoveSmallSegments labels/sizes, GapInterpolation temporaries, staging
 	DevBuf ppK, ppArcs, ppPatch;              // RemoveSmallSegments: seed keys, one-way edges (+ counter), patched segment sizes
@@ -594,6 +610,7 @@ int b200mvs_destroy(b200mvs_ctx* c) {
 	for (auto e: c->sweepEv) cudaEventDestroy(e);
 	c->sgL.release(); c->sgC.release(); c->sgR.release(); c->sgPx.release(); c->sgCosts.release(); c->sgAccums.release(); c->sgAccums2.release();
 	c->sgDisp.release(); c->sgCost.release(); c->sgMax.release();
+	for (auto& b: c->ts) b.release();
 	for (auto& fp: c->sgFront) { fp.items.release(); fp.need.release(); }
 	c->sgFrontCtl.release(); c->sgFrontState.release(); c->sgFrontMeta.release();
 	for (int i = 0; i < 7; ++i) { if (c->sgSide[i]) cudaStreamDestroy(c->sgSide[i]); if (c->sgJoin[i]) cudaEventDestroy(c->sgJoin[i]); }
@@ -1092,6 +1109,280 @@ int b200mvs_sgm_refine_device(b200mvs_ctx* ctx, const b200mvs_sgm_pixel* pixels,
 	if (subpixelSteps <= 1) return B200MVS_OK;
 	CK(cudaSetDevice(ctx->device));
 	CK(sgm_launch_refine((const SGMPixel*)pixels, accums, disparity, nPixels, subpixelSteps, stream ? (cudaStream_t)stream : ctx->stream));
+	return B200MVS_OK;
+}
+
+// ---- hierarchical (tSGM) matching ----------------------------------------------------------------
+static int tsgm_levels(int width, int height, int minResolution, int& n, int* ws, int* hs, int& iw, int& ih) {
+	if (width <= 6 || height <= 6 || minResolution < 0) return B200MVS_ERR_ARG;
+	double scale = 1;
+	if (minResolution > 0) {
+		// Image8U::computeMaxResolution(w, h, level = 8, minResolution) (libs/Common/Types.inl:2459-2477)
+		const unsigned imageSize = (unsigned)std::max(width, height), minSize = (unsigned)minResolution;
+		unsigned level = 8;
+		if ((imageSize >> level) < minSize) {
+			level = 0;
+			while ((imageSize >> (level+1)) >= minSize) ++level;
+		}
+		scale = 1.0/std::max(2.0, std::pow(2.0, (double)level));
+	}
+	n = 0;
+	do {
+		// computeResize / cv::resize(..., Size(), scale, scale): saturate_cast<int>(size * scale) rounds to nearest even
+		ws[n] = (int)std::nearbyint(width*scale); hs[n] = (int)std::nearbyint(height*scale);
+		if (ws[n] <= 6 || hs[n] <= 6) return B200MVS_ERR_ARG;
+		++n;
+	} while ((scale *= 2) < 1+1e-9 && n < B200MVS_SGM_MAX_LEVELS);
+	iw = (int)std::nearbyint(ws[0]*0.5)-6; ih = (int)std::nearbyint(hs[0]*0.5)-6;
+	if (iw < 1 || ih < 1) return B200MVS_ERR_ARG;
+	// Disparity2RangeMap reads the mask of the 2x grid at (2r+3, 2c+3) and needs the grid to end beyond column 2w+3
+	for (int k = 0, pw = iw, ph = ih; minResolution > 0 && k < n; pw = ws[k]-6, ph = hs[k]-6, ++k)
+		if (2*pw+3 >= ws[k]-6 || 2*ph+1 >= hs[k]-6) return B200MVS_ERR_ARG;
+	return B200MVS_OK;
+}
+
+int b200mvs_sgm_levels(int width, int height, int minResolution, int* numLevels, int* levelWidths, int* levelHeights, int* initWidth, int* initHeight) {
+	int n = 0, ws[B200MVS_SGM_MAX_LEVELS], hs[B200MVS_SGM_MAX_LEVELS], iw = 0, ih = 0;
+	const int rc = tsgm_levels(width, height, minResolution, n, ws, hs, iw, ih);
+	if (rc) return rc;
+	if (numLevels) *numLevels = n;
+	for (int k = 0; k < n; ++k) { if (levelWidths) levelWidths[k] = ws[k]; if (levelHeights) levelHeights[k] = hs[k]; }
+	if (initWidth) *initWidth = iw;
+	if (initHeight) *initHeight = ih;
+	return B200MVS_OK;
+}
+
+static int tsgm_range_map(b200mvs_ctx* ctx, const int16_t* disparity, int width, int height, const uint8_t* mask, int mw, int mh,
+	int minNumDisp, int minNumDispInvalid, b200mvs_sgm_pixel* pixels, uint64_t* numCosts, cudaStream_t s)
+{
+	const size_t n2 = (size_t)mw*mh;
+	CK(ctx->ts[b200mvs_ctx::TS_RANGES].reserve((size_t)width*height*sizeof(short2)));
+	CK(ctx->ts[b200mvs_ctx::TS_SCAN].reserve(tsgm_range_map_scratch(n2)));
+	CK(ctx->ts[b200mvs_ctx::TS_SMALL].reserve(64));
+	unsigned long long* total = ctx->ts[b200mvs_ctx::TS_SMALL].as<unsigned long long>();
+	CK(tsgm_launch_range_map(disparity, width, height, mask, mw, mh, minNumDisp, minNumDispInvalid,
+		ctx->ts[b200mvs_ctx::TS_RANGES].as<short2>(), (SGMPixel*)pixels, ctx->ts[b200mvs_ctx::TS_SCAN].p, total, s));
+	// the size of the volume: one 8-byte read per pixel map (the match that follows sizes its scratch with it)
+	unsigned long long num = 0;
+	CK(cudaMemcpyAsync(&num, total, sizeof(num), cudaMemcpyDeviceToHost, s));
+	CK(cudaStreamSynchronize(s));
+	*numCosts = num;
+	return B200MVS_OK;
+}
+
+int b200mvs_sgm_range_map_device(b200mvs_ctx* ctx, const int16_t* disparity, int width, int height, const uint8_t* mask,
+	int maskWidth, int maskHeight, int minNumDisp, int minNumDispInvalid, b200mvs_sgm_pixel* pixels, uint64_t* numCosts, void* stream)
+{
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!disparity || !mask || !pixels || !numCosts || width <= 0 || height <= 0)
+		return fail(ctx, B200MVS_ERR_ARG, "range map: null pointer or empty map");
+	if (maskWidth <= 2*width+3 || maskHeight <= 2*height+1 || (size_t)maskWidth*maskHeight >= (1u<<31))
+		return fail(ctx, B200MVS_ERR_ARG, "range map: the 2x grid must extend beyond (2 width + 3, 2 height + 1)");
+	CK(cudaSetDevice(ctx->device));
+	return tsgm_range_map(ctx, disparity, width, height, mask, maskWidth, maskHeight, minNumDisp, minNumDispInvalid, pixels, numCosts,
+		stream ? (cudaStream_t)stream : ctx->stream);
+}
+
+int b200mvs_sgm_flip_direction_device(b200mvs_ctx* ctx, const int16_t* l2r, int16_t* r2l, int width, int height, void* stream) {
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!l2r || !r2l || l2r == r2l || width <= 0 || height <= 0 || width >= 65535)
+		return fail(ctx, B200MVS_ERR_ARG, "flip direction: null or aliased maps, or a width outside [1, 65534]");
+	CK(cudaSetDevice(ctx->device));
+	CK(ctx->ts[b200mvs_ctx::TS_KEYS].reserve((size_t)width*height*sizeof(unsigned)));
+	CK(tsgm_launch_flip(l2r, r2l, width, height, ctx->ts[b200mvs_ctx::TS_KEYS].as<unsigned>(), stream ? (cudaStream_t)stream : ctx->stream));
+	return B200MVS_OK;
+}
+
+int b200mvs_sgm_upscale_mask_device(b200mvs_ctx* ctx, const uint8_t* mask, int width, int height, uint8_t* mask2x, int width2x, int height2x, void* stream) {
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!mask || !mask2x || mask == mask2x || width <= 0 || height <= 0 || width2x <= 0 || height2x <= 0)
+		return fail(ctx, B200MVS_ERR_ARG, "upscale mask: null or aliased masks, or an empty size");
+	CK(cudaSetDevice(ctx->device));
+	CK(tsgm_launch_upscale_mask(mask, width, height, mask2x, width2x, height2x, stream ? (cudaStream_t)stream : ctx->stream));
+	return B200MVS_OK;
+}
+
+int b200mvs_sgm_extract_mask_device(b200mvs_ctx* ctx, const int16_t* disparity, uint8_t* mask, int width, int height, int thValid, void* stream) {
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!disparity || !mask || width <= 0 || height <= 0)
+		return fail(ctx, B200MVS_ERR_ARG, "extract mask: null pointer or empty map");
+	CK(cudaSetDevice(ctx->device));
+	CK(tsgm_launch_extract_mask(disparity, mask, width, height, thValid, stream ? (cudaStream_t)stream : ctx->stream));
+	return B200MVS_OK;
+}
+
+int b200mvs_sgm_filter_speckles_device(b200mvs_ctx* ctx, int16_t* disparity, int width, int height, int newVal, int maxSpeckleSize,
+	int maxDiff, void* stream)
+{
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!disparity || width <= 0 || height <= 0 || (size_t)width*height >= (1u<<31) || maxSpeckleSize < 0 || maxDiff < 0)
+		return fail(ctx, B200MVS_ERR_ARG, "filter speckles: null map, bad size or negative limits");
+	CK(cudaSetDevice(ctx->device));
+	const size_t n = (size_t)width*height;
+	CK(ctx->ts[b200mvs_ctx::TS_LABELS].reserve(n*sizeof(int))); CK(ctx->ts[b200mvs_ctx::TS_SIZES].reserve(n*sizeof(int)));
+	CK(tsgm_launch_speckles(disparity, width, height, newVal, maxSpeckleSize, maxDiff, ctx->ts[b200mvs_ctx::TS_LABELS].as<int>(),
+		ctx->ts[b200mvs_ctx::TS_SIZES].as<int>(), stream ? (cudaStream_t)stream : ctx->stream));
+	return B200MVS_OK;
+}
+
+int b200mvs_resize_area_u8_device(b200mvs_ctx* ctx, const uint8_t* src, int width, int height, int channels, int factor, uint8_t* dst, void* stream) {
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!src || !dst || width <= 0 || height <= 0 || factor < 1 || (channels != 1 && channels != 3 && channels != 4))
+		return fail(ctx, B200MVS_ERR_ARG, "resize area u8: null pointer, empty image, factor < 1 or channels not 1, 3 or 4");
+	const int dw = (int)std::nearbyint(width*(1.0/factor)), dh = (int)std::nearbyint(height*(1.0/factor));
+	if (dw <= 0 || dh <= 0) return fail(ctx, B200MVS_ERR_ARG, "resize area u8: empty result");
+	CK(cudaSetDevice(ctx->device));
+	CK(tsgm_launch_area_u8(src, width, height, channels, dst, dw, dh, factor, stream ? (cudaStream_t)stream : ctx->stream));
+	return B200MVS_OK;
+}
+
+static int tsgm_level_mask(b200mvs_ctx* ctx, const uint8_t* mask, int width, int height, int lw, int lh, uint8_t* valid, cudaStream_t s) {
+	DevBuf& t = ctx->ts[b200mvs_ctx::TS_MASKT];
+	CK(t.reserve((size_t)lw*lh));
+	CK(rs_launch_nearest_u8(mask, width, height, width, t.as<uint8_t>(), lw, lh, s));
+	CK(cudaMemcpy2DAsync(valid, lw-6, t.as<uint8_t>()+3*lw+3, lw, lw-6, lh-6, cudaMemcpyDeviceToDevice, s));
+	return B200MVS_OK;
+}
+
+int b200mvs_sgm_level_mask_device(b200mvs_ctx* ctx, const uint8_t* mask, int width, int height, int levelWidth, int levelHeight,
+	uint8_t* validMask, void* stream)
+{
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!mask || !validMask || width <= 0 || height <= 0 || levelWidth <= 6 || levelHeight <= 6)
+		return fail(ctx, B200MVS_ERR_ARG, "level mask: null pointer or a level of at most 6 pixels");
+	CK(cudaSetDevice(ctx->device));
+	return tsgm_level_mask(ctx, mask, width, height, levelWidth, levelHeight, validMask, stream ? (cudaStream_t)stream : ctx->stream);
+}
+
+int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
+	const float* leftGray, const uint8_t* leftBGR, const float* rightGray, const uint8_t* rightBGR, int width, int height,
+	const int16_t* initDisparity, int initWidth, int initHeight, const uint8_t* leftMask, const uint8_t* rightMask,
+	int minResolution, int nSpeckleSize, int thCross, int subpixelSteps, const b200mvs_sgm_params* prm,
+	int16_t* outDisparity, uint16_t* outCost, uint64_t* numCostsPerLevel, void* stream)
+{
+	typedef b200mvs_ctx X;
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!leftGray || !leftBGR || !rightGray || !rightBGR || !outDisparity || !outCost)
+		return fail(ctx, B200MVS_ERR_ARG, "hierarchical sgm: null image or output map");
+	if (nSpeckleSize < 0 || thCross < 0 || width >= 65535)
+		return fail(ctx, B200MVS_ERR_ARG, "hierarchical sgm: negative nSpeckleSize / thCross or a width above 65534");
+	int nl = 0, lw[B200MVS_SGM_MAX_LEVELS], lh[B200MVS_SGM_MAX_LEVELS], iw = 0, ih = 0;
+	if (tsgm_levels(width, height, minResolution, nl, lw, lh, iw, ih))
+		return fail(ctx, B200MVS_ERR_ARG, "hierarchical sgm: negative minResolution, or the image is too small for its levels");
+	if (initDisparity && (initWidth != iw || initHeight != ih))
+		return fail(ctx, B200MVS_ERR_ARG, "hierarchical sgm: the initial disparity map must have the size b200mvs_sgm_levels gives");
+	CK(cudaSetDevice(ctx->device));
+	cudaStream_t s = stream ? (cudaStream_t)stream : ctx->stream;
+	const bool tsgm = minResolution > 0;
+	const size_t n = (size_t)width*height, nv = (size_t)(width-6)*(height-6);
+	// grow-only scratch, sized for the full-resolution level up front (nothing is reallocated while kernels use it)
+	const size_t nImg = nl > 1 ? (size_t)lw[nl-2]*lh[nl-2] : 0;
+	CK(ctx->ts[X::TS_IMG].reserve(nImg*14+64));
+	CK(ctx->ts[X::TS_MASKL].reserve(nv)); CK(ctx->ts[X::TS_MASKR].reserve(nv)); CK(ctx->ts[X::TS_MASKT].reserve(n));
+	for (int b: {X::TS_DL, X::TS_DR, X::TS_DL0, X::TS_DR0}) CK(ctx->ts[b].reserve(nv*sizeof(int16_t)));
+	CK(ctx->ts[X::TS_PXL].reserve(nv*sizeof(SGMPixel))); CK(ctx->ts[X::TS_PXR].reserve(nv*sizeof(SGMPixel)));
+	CK(ctx->ts[X::TS_RANGES].reserve(nv*sizeof(short2))); CK(ctx->ts[X::TS_SCAN].reserve(tsgm_range_map_scratch(nv)));
+	CK(ctx->ts[X::TS_KEYS].reserve(nv*sizeof(unsigned))); CK(ctx->ts[X::TS_LABELS].reserve(nv*sizeof(int)));
+	CK(ctx->ts[X::TS_SIZES].reserve(nv*sizeof(int))); CK(ctx->ts[X::TS_SMALL].reserve(64));
+	uint8_t* maskL = ctx->ts[X::TS_MASKL].as<uint8_t>(); uint8_t* maskR = ctx->ts[X::TS_MASKR].as<uint8_t>();
+	uint8_t* maskT = ctx->ts[X::TS_MASKT].as<uint8_t>();
+	b200mvs_sgm_pixel* pxL = ctx->ts[X::TS_PXL].as<b200mvs_sgm_pixel>(); b200mvs_sgm_pixel* pxR = ctx->ts[X::TS_PXR].as<b200mvs_sgm_pixel>();
+	// dL / dR: the maps of the previous level (pw x ph; first level: the initial map), nL / nR: the maps of this level
+	int16_t *dL = ctx->ts[X::TS_DL0].as<int16_t>(), *dR = ctx->ts[X::TS_DR0].as<int16_t>();
+	int16_t *nL = ctx->ts[X::TS_DL].as<int16_t>(), *nR = ctx->ts[X::TS_DR].as<int16_t>();
+	int pw = iw, ph = ih;
+	if (initDisparity) CK(cudaMemcpyAsync(dL, initDisparity, (size_t)iw*ih*sizeof(int16_t), cudaMemcpyDeviceToDevice, s));
+	else CK(tsgm_launch_fill(dL, (size_t)iw*ih, (int16_t)32767, s));
+	int fixLo = 0, fixHi = 0;
+	if (!tsgm) {
+		// the global range of the initial map (SemiGlobalMatcher.cpp:643-668) over its valid values
+		int mm[2] = {0, 0};
+		int* dmm = (int*)(ctx->ts[X::TS_SMALL].as<unsigned long long>()+1);
+		CK(tsgm_launch_minmax(dL, (size_t)iw*ih, dmm, s));
+		CK(cudaMemcpyAsync(mm, dmm, sizeof(mm), cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		if (mm[0] > mm[1]) return fail(ctx, B200MVS_ERR_ARG, "hierarchical sgm: minResolution = 0 needs an initial map with a valid disparity");
+		const int16_t numDisp = (int16_t)((int16_t)(mm[1]-mm[0])+16), disp = (int16_t)(mm[0]+mm[1]);
+		fixLo = (int16_t)(disp-numDisp); fixHi = (int16_t)(disp+numDisp);
+		if (fixHi-fixLo > sgm_max_disparities())
+			return fail(ctx, B200MVS_ERR_ARG, "hierarchical sgm: the initial map spans more than 256 disparities with its margins");
+	}
+	// one match; an empty volume (every pixel masked) leaves NO_DISP / NO_ACCUMCOST like the winner-takes-all of invalid pixels
+	auto match = [&](const float* g0, const uint8_t* c0, const float* g1, int w, int h, const b200mvs_sgm_pixel* px, uint64_t num,
+			int16_t* disp, uint16_t* cost) -> int {
+		if (num == 0) {
+			CK(tsgm_launch_fill(disp, (size_t)(w-6)*(h-6), (int16_t)32767, s));
+			CK(cudaMemsetAsync(cost, 0xFF, (size_t)(w-6)*(h-6)*sizeof(uint16_t), s));
+			return B200MVS_OK;
+		}
+		return b200mvs_sgm_match_device(ctx, g0, c0, g1, w, h, px, num, prm, 7, nullptr, nullptr, disp, cost, s, nullptr);
+	};
+	int rc = 0;
+	for (int lev = 0; lev < nl; ++lev) {
+		const int w = lw[lev], h = lh[lev], vw = w-6, vh = h-6;
+		const bool first = lev == 0;
+		// ViewData::GetImage(scale): INTER_AREA from the full-resolution images
+		const float *lg = leftGray, *rg = rightGray; const uint8_t *lc = leftBGR, *rcol = rightBGR;
+		if (lev+1 < nl) {
+			const int f = 1 << (nl-1-lev);
+			const size_t m = (size_t)w*h;
+			float* g = (float*)ctx->ts[X::TS_IMG].p; uint8_t* c = (uint8_t*)(g+2*m);
+			CK(rs_launch_area(leftGray, width, height, width, g, w, h, f, f, s));
+			CK(rs_launch_area(rightGray, width, height, width, g+m, w, h, f, f, s));
+			CK(tsgm_launch_area_u8(leftBGR, width, height, 3, c, w, h, f, s));
+			CK(tsgm_launch_area_u8(rightBGR, width, height, 3, c+3*m, w, h, f, s));
+			lg = g; rg = g+m; lc = c; rcol = c+3*m;
+		}
+		if (first) {
+			// masks: NEAREST to the level size, cropped to the valid region (SemiGlobalMatcher.cpp:627-631)
+			if (leftMask) { if ((rc = tsgm_level_mask(ctx, leftMask, width, height, w, h, maskL, s))) return rc; }
+			else CK(cudaMemsetAsync(maskL, 0xFF, (size_t)vw*vh, s));
+			if (rightMask) { if ((rc = tsgm_level_mask(ctx, rightMask, width, height, w, h, maskR, s))) return rc; }
+			else CK(cudaMemsetAsync(maskR, 0xFF, (size_t)vw*vh, s));
+		} else {
+			for (uint8_t* m: {maskL, maskR}) {
+				CK(tsgm_launch_upscale_mask(m, pw, ph, maskT, vw, vh, s));
+				CK(cudaMemcpyAsync(m, maskT, (size_t)vw*vh, cudaMemcpyDeviceToDevice, s));
+			}
+		}
+		uint64_t numR = 0, numL = 0;
+		if (tsgm) {
+			CK(tsgm_launch_flip(dL, dR, pw, ph, ctx->ts[X::TS_KEYS].as<unsigned>(), s));
+			if ((rc = tsgm_range_map(ctx, dR, pw, ph, maskR, vw, vh, first ? 11 : 5, first ? 33 : 7, pxR, &numR, s))) return rc;
+		} else {
+			numR = (uint64_t)nv*(uint64_t)(fixHi-fixLo);
+			CK(tsgm_launch_dense_map((SGMPixel*)pxR, nv, fixLo, fixHi, s));
+		}
+		if ((rc = match(rg, rcol, lg, w, h, pxR, numR, nR, outCost))) return rc;
+		if (tsgm) {
+			if ((rc = tsgm_range_map(ctx, dL, pw, ph, maskL, vw, vh, first ? 11 : 5, first ? 33 : 7, pxL, &numL, s))) return rc;
+		} else {
+			numL = numR;
+			CK(tsgm_launch_dense_map((SGMPixel*)pxL, nv, -fixHi, -fixLo, s));
+		}
+		if ((rc = match(lg, lc, rg, w, h, pxL, numL, nL, outCost))) return rc;
+		if (numCostsPerLevel) { numCostsPerLevel[2*lev] = numR; numCostsPerLevel[2*lev+1] = numL; }
+		if (first) {
+			// SemiGlobalMatcher.cpp:698-706
+			CK(sgm_launch_cross_check(nL, nR, vw, vh, thCross, s));
+			CK(sgm_launch_cross_check(nR, nL, vw, vh, thCross, s));
+			for (int16_t* d: {nL, nR})
+				CK(tsgm_launch_speckles(d, vw, vh, 32767, nSpeckleSize, 5, ctx->ts[X::TS_LABELS].as<int>(), ctx->ts[X::TS_SIZES].as<int>(), s));
+			CK(tsgm_launch_extract_mask(nL, maskL, vw, vh, 3, s));
+			CK(tsgm_launch_extract_mask(nR, maskR, vw, vh, 3, s));
+		} else {
+			CK(sgm_launch_cross_check(nL, nR, vw, vh, thCross, s));
+		}
+		std::swap(dL, nL); std::swap(dR, nR);
+		pw = vw; ph = vh;
+	}
+	// RefineDisparityMap(left) with the accumulated costs of the last left match (SemiGlobalMatcher.cpp:718)
+	if (subpixelSteps > 1 && ctx->sgAccums.p)
+		CK(sgm_launch_refine((const SGMPixel*)pxL, ctx->sgAccums.as<uint16_t>(), dL, (int)nv, subpixelSteps, s));
+	CK(cudaMemcpyAsync(outDisparity, dL, nv*sizeof(int16_t), cudaMemcpyDeviceToDevice, s));
+	// the pixel maps of the hierarchy are internal: no later refine call may take sgAccums for its own map
+	ctx->sgLastPx = nullptr;
+	CK(cudaStreamSynchronize(s));
 	return B200MVS_OK;
 }
 

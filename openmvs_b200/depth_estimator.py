@@ -653,6 +653,116 @@ class SemiGlobalMatcher:
 		torch.cuda.current_stream(dev).synchronize()
 		return ldisp, rdisp
 
+	@staticmethod
+	def HierarchyLevels(width: int, height: int, minResolution: int = 320):
+		"""Level sizes of the hierarchical matcher, coarsest first, and the size of its initial disparity map (b200mvs_sgm_levels):
+		([(w, h), ...], (initWidth, initHeight)).  Host arithmetic, no GPU needed."""
+		lib = _lib.load()
+		n, iw, ih = C.c_int(), C.c_int(), C.c_int()
+		ws, hs = (C.c_int*9)(), (C.c_int*9)()
+		rc = lib.b200mvs_sgm_levels(int(width), int(height), int(minResolution), C.byref(n), ws, hs, C.byref(iw), C.byref(ih))
+		if rc != 0:
+			raise _lib.B200MVSError("b200mvs_sgm_levels(%d, %d, %d) failed with status %d" % (width, height, minResolution, rc))
+		return [(ws[k], hs[k]) for k in range(n.value)], (iw.value, ih.value)
+
+	def MatchPairHierarchicalDevice(self, leftGray, leftColor, rightGray, rightColor, initDisparity=None, leftMask=None, rightMask=None,
+			minResolution: int = 320, thCross: int = 1, subpixelSteps: int = 4, nSpeckleSize: Optional[int] = None):
+		"""SemiGlobalMatcher::Match(scene, ...) for one rectified pair (libs/MVS/SemiGlobalMatcher.cpp:583-718) on CUDA tensors:
+		the image pyramid, per level FlipDirection + Disparity2RangeMap + right->left and left->right matches, the first level's
+		cross-checks, speckle filter and mask extraction, the later levels' cross-check, and the final sub-pixel refinement.
+		initDisparity: int16 map of HierarchyLevels' init size in half-coarsest-level pixels (None: no estimate, NO_DISP);
+		leftMask / rightMask: uint8 full-resolution masks (0 = invalid).  minResolution = 0: one level with the initial map's range.
+		Returns (leftDisparity * subpixelSteps, cost, levels) with levels = [{"size": (w, h), "numCosts": (right, left)}, ...];
+		cost holds the uint16 bit pattern in an int16 tensor."""
+		import torch
+		h, w = leftGray.shape
+		dev = leftGray.device
+		sizes, (iw, ih) = self.HierarchyLevels(w, h, minResolution)
+		if initDisparity is not None and tuple(initDisparity.shape) != (ih, iw):
+			raise ValueError("initDisparity must be %d x %d (rows x columns)" % (ih, iw))
+		ptr = lambda t: t.data_ptr() if t is not None else None
+		disp = torch.empty((h-6, w-6), dtype=torch.int16, device=dev)
+		cost = torch.empty((h-6, w-6), dtype=torch.int16, device=dev)
+		nums = (C.c_uint64*(2*len(sizes)))()
+		speckle = OPTDENSE.nSpeckleSize if nSpeckleSize is None else nSpeckleSize
+		rc = self._lib.b200mvs_sgm_match_hierarchical_device(self._ctx, leftGray.data_ptr(), leftColor.data_ptr(), rightGray.data_ptr(),
+			rightColor.data_ptr(), w, h, ptr(initDisparity), iw, ih, ptr(leftMask), ptr(rightMask), int(minResolution), int(speckle),
+			int(thCross), int(subpixelSteps), C.byref(self.prm), disp.data_ptr(), cost.data_ptr(), nums, C.c_void_p(_stream_handle(dev)))
+		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_match_hierarchical_device")
+		levels = [{"size": sizes[k], "numCosts": (int(nums[2*k]), int(nums[2*k+1]))} for k in range(len(sizes))]
+		return disp, cost, levels
+
+	# building blocks of the level loop on CUDA tensors (names of the reference's members, SemiGlobalMatcher.h:171-179)
+	def Disparity2RangeMap(self, disparityMap, maskMap, minNumDisp: int = 3, minNumDispInvalid: int = 16):
+		"""-> (PixelMap as a (maskH*maskW, 16) uint8 tensor, numCosts) for the 2x grid of maskMap (int16 / uint8 tensors)"""
+		import torch
+		h, w = disparityMap.shape
+		mh, mw = maskMap.shape
+		px = torch.empty((mh*mw, 16), dtype=torch.uint8, device=disparityMap.device)
+		num = C.c_uint64()
+		rc = self._lib.b200mvs_sgm_range_map_device(self._ctx, disparityMap.data_ptr(), w, h, maskMap.data_ptr(), mw, mh, int(minNumDisp),
+			int(minNumDispInvalid), px.data_ptr(), C.byref(num), C.c_void_p(_stream_handle(disparityMap.device)))
+		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_range_map_device")
+		return px, int(num.value)
+
+	def FlipDirection(self, l2r):
+		"""-> the right->left int16 map of a left->right one"""
+		import torch
+		h, w = l2r.shape
+		r2l = torch.empty_like(l2r)
+		rc = self._lib.b200mvs_sgm_flip_direction_device(self._ctx, l2r.data_ptr(), r2l.data_ptr(), w, h, C.c_void_p(_stream_handle(l2r.device)))
+		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_flip_direction_device")
+		return r2l
+
+	def UpscaleMask(self, maskMap, size2x):
+		"""-> the uint8 mask of size2x = (width, height)"""
+		import torch
+		h, w = maskMap.shape
+		out = torch.empty((int(size2x[1]), int(size2x[0])), dtype=torch.uint8, device=maskMap.device)
+		rc = self._lib.b200mvs_sgm_upscale_mask_device(self._ctx, maskMap.data_ptr(), w, h, out.data_ptr(), int(size2x[0]), int(size2x[1]),
+			C.c_void_p(_stream_handle(maskMap.device)))
+		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_upscale_mask_device")
+		return out
+
+	def ExtractMask(self, disparityMap, maskMap, thValid: int = 3):
+		"""maskMap (uint8, same size) in place"""
+		h, w = disparityMap.shape
+		rc = self._lib.b200mvs_sgm_extract_mask_device(self._ctx, disparityMap.data_ptr(), maskMap.data_ptr(), w, h, int(thValid),
+			C.c_void_p(_stream_handle(disparityMap.device)))
+		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_extract_mask_device")
+		return maskMap
+
+	def FilterSpeckles(self, disparityMap, newVal: int = NO_DISP, maxSpeckleSize: Optional[int] = None, maxDiff: int = 5):
+		"""cv::filterSpeckles on an int16 tensor, in place; maxSpeckleSize defaults to OPTDENSE.nSpeckleSize"""
+		h, w = disparityMap.shape
+		size = OPTDENSE.nSpeckleSize if maxSpeckleSize is None else maxSpeckleSize
+		rc = self._lib.b200mvs_sgm_filter_speckles_device(self._ctx, disparityMap.data_ptr(), w, h, int(newVal), int(size), int(maxDiff),
+			C.c_void_p(_stream_handle(disparityMap.device)))
+		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_filter_speckles_device")
+		return disparityMap
+
+	def ResizeAreaU8(self, image, factor: int):
+		"""cv::resize(image, Size(), 1/factor, 1/factor, INTER_AREA) of a uint8 (H, W[, C]) tensor with 1, 3 or 4 channels"""
+		import torch
+		h, w = image.shape[:2]
+		cn = 1 if image.dim() == 2 else image.shape[2]
+		dh, dw = int(np.rint(h/float(factor))), int(np.rint(w/float(factor)))
+		out = torch.empty((dh, dw) + tuple(image.shape[2:]), dtype=torch.uint8, device=image.device)
+		rc = self._lib.b200mvs_resize_area_u8_device(self._ctx, image.data_ptr(), w, h, int(cn), int(factor), out.data_ptr(),
+			C.c_void_p(_stream_handle(image.device)))
+		_lib.check(self._lib, self._ctx, rc, "b200mvs_resize_area_u8_device")
+		return out
+
+	def LevelMask(self, mask, levelSize):
+		"""first level's mask: NEAREST resize of the uint8 mask to levelSize = (w, h), cropped to the valid region"""
+		import torch
+		h, w = mask.shape
+		lw, lh = int(levelSize[0]), int(levelSize[1])
+		out = torch.empty((lh-6, lw-6), dtype=torch.uint8, device=mask.device)
+		rc = self._lib.b200mvs_sgm_level_mask_device(self._ctx, mask.data_ptr(), w, h, lw, lh, out.data_ptr(), C.c_void_p(_stream_handle(mask.device)))
+		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_level_mask_device")
+		return out
+
 
 @dataclasses.dataclass
 class PointCloud:

@@ -8,7 +8,7 @@ import os
 from . import build as _build
 
 MAX_VIEWS = 32
-ABI_VERSION = 5  # B200MVS_ABI_VERSION of include/b200mvs.h these structs mirror
+ABI_VERSION = 6  # B200MVS_ABI_VERSION of include/b200mvs.h these structs mirror
 
 
 class View(C.Structure):
@@ -96,6 +96,9 @@ SYMBOLS = [
 	"b200mvs_pm_pack", "b200mvs_pm_unpack", "b200mvs_pm_score", "b200mvs_pm_sweep", "b200mvs_pm_finalize",
 	"b200mvs_sgm_default_params", "b200mvs_sgm_match", "b200mvs_sgm_match_device",
 	"b200mvs_sgm_cross_check_device", "b200mvs_sgm_refine_device",
+	"b200mvs_sgm_levels", "b200mvs_sgm_match_hierarchical_device", "b200mvs_sgm_range_map_device", "b200mvs_sgm_flip_direction_device",
+	"b200mvs_sgm_upscale_mask_device", "b200mvs_sgm_extract_mask_device", "b200mvs_sgm_filter_speckles_device",
+	"b200mvs_resize_area_u8_device", "b200mvs_sgm_level_mask_device",
 	"b200mvs_filter_default_params", "b200mvs_filter_depth_map", "b200mvs_filter_depth_map_device",
 	"b200mvs_remove_small_segments", "b200mvs_remove_small_segments_device",
 	"b200mvs_gap_interpolation", "b200mvs_gap_interpolation_device",
@@ -163,6 +166,17 @@ def load(build_if_missing: bool = True):
 	lib.b200mvs_pointcloud_free.restype = None
 	lib.b200mvs_sgm_cross_check_device.argtypes = [P, P, P, C.c_int, C.c_int, C.c_int, P]
 	lib.b200mvs_sgm_refine_device.argtypes = [P, P, P, P, C.c_int, C.c_int, P]
+	I = C.c_int
+	IP = C.POINTER(C.c_int)
+	lib.b200mvs_sgm_levels.argtypes = [I, I, I, IP, IP, IP, IP, IP]
+	lib.b200mvs_sgm_match_hierarchical_device.argtypes = [P, P, P, P, P, I, I, P, I, I, P, P, I, I, I, I, C.POINTER(SgmParams), P, P, P, P]
+	lib.b200mvs_sgm_range_map_device.argtypes = [P, P, I, I, P, I, I, I, I, P, C.POINTER(C.c_uint64), P]
+	lib.b200mvs_sgm_flip_direction_device.argtypes = [P, P, P, I, I, P]
+	lib.b200mvs_sgm_upscale_mask_device.argtypes = [P, P, I, I, P, I, I, P]
+	lib.b200mvs_sgm_extract_mask_device.argtypes = [P, P, P, I, I, I, P]
+	lib.b200mvs_sgm_filter_speckles_device.argtypes = [P, P, I, I, I, I, I, P]
+	lib.b200mvs_resize_area_u8_device.argtypes = [P, P, I, I, I, I, P, P]
+	lib.b200mvs_sgm_level_mask_device.argtypes = [P, P, I, I, I, I, P, P]
 	lib.b200mvs_filter_default_params.argtypes = [C.POINTER(FilterParams)]
 	lib.b200mvs_filter_depth_map.argtypes = [P, C.POINTER(DMap), C.POINTER(DMap), C.c_int, C.POINTER(FilterParams), F, F, P, P,
 		C.POINTER(C.c_int), C.POINTER(Stats)]
