@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 LIB_PATH = os.path.join(HERE, "libb200mvs.so")
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-	"-Xcompiler", "-fPIC", "-shared"]
+	"-Xcompiler", "-fPIC", "-shared", "-Xlinker", "--no-undefined"]
 
 
 def sources():
@@ -21,7 +21,8 @@ def is_stale() -> bool:
 	if not os.path.exists(LIB_PATH):
 		return True
 	t = os.path.getmtime(LIB_PATH)
-	deps = sources() + glob.glob(os.path.join(HERE, "csrc", "*.cuh")) + glob.glob(os.path.join(ROOT, "include", "*.h"))
+	deps = sources() + glob.glob(os.path.join(HERE, "csrc", "*.cuh")) + glob.glob(os.path.join(HERE, "csrc", "*.h")) + \
+		glob.glob(os.path.join(ROOT, "include", "*.h"))
 	return any(os.path.getmtime(d) > t for d in deps)
 
 

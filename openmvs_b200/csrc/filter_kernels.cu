@@ -14,25 +14,7 @@
 // evaluation order oracle/filter_oracle.cpp writes out, so results are bit-identical to it.
 // HBM-bound integer/float work: per reference pixel the vote reads 8 B x N keys + 8 B and
 // writes 8 B; the splat reads 4 B and issues <= 4 atomics per neighbour pixel.
-#include <cuda_runtime.h>
-#include <cstdint>
-
-#define FLT_MAX_NBR 16
-
-struct FltView {
-	const float* depth; const float* conf;
-	int w, h;
-	double fx, fy, cx, cy;
-	double R[9], C[3];
-};
-struct FltParams {
-	FltView ref;
-	FltView nbr[FLT_MAX_NBR];
-	int N, nMinViews, nMinViewsAdjust;
-	float thDepthDiff, thStrict, dMin, dMax;
-	unsigned long long* zbuf; // N x ref.h x ref.w keys
-	float* outDepth; float* outConf;
-};
+#include "filter_common.cuh"
 
 namespace {
 
@@ -263,8 +245,6 @@ __global__ void seg_count_kernel(int* L, int* size, int* minKey, int W, int H) {
 	const int kmin = __reduce_min_sync(peers, key);
 	if (r >= 0 && (threadIdx.x&31) == __ffs(peers)-1) { atomicAdd(size+r, __popc(peers)); atomicMin(minKey+r, kmin); }
 }
-// one-way edges between different two-way components: arcs[k] = {source label, target label, sizes, seed keys}
-struct SegArc { int src, dst, srcSize, dstSize, srcKey, dstKey; };
 __global__ void seg_arcs_kernel(const float* __restrict__ depth, const int* __restrict__ L, const int* __restrict__ size, const int* __restrict__ minKey,
 	int W, int H, float th, SegArc* arcs, int* count, int cap)
 {

@@ -1,4 +1,4 @@
-// pm_common.cuh — shared device-side definitions of the PatchMatch kernels (sm_90a).
+// pm_common.cuh — shared definitions of the PatchMatch kernels (sm_90a) and their launch functions.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -52,3 +52,13 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
 	return c;
 }
 __device__ __forceinline__ float u32_to_unit(uint32_t u) { return (float)u*(1.0f/4294967296.0f); }
+
+// launch functions (pm_kernels.cu)
+cudaError_t pm_configure_device();
+cudaError_t pm_launch_score(const PMParams& P, bool geom, cudaStream_t s);
+cudaError_t pm_launch_sweep(const PMParams& P, const void* tmapRef, bool geom, cudaStream_t s);
+void pm_tma_box(int* w, int* h);
+cudaError_t pm_launch_finalize(int n, float keep, const float4* plane, const float* cost, const uint32_t* bestViews,
+	float* depth, float* normal, float* conf, uint32_t* viewsMap, cudaStream_t s);
+cudaError_t pm_launch_pack(int n, const float* depth, const float* normal, float4* plane, cudaStream_t s);
+cudaError_t pm_launch_unpack(int n, const float4* plane, float* depth, float* normal, cudaStream_t s);

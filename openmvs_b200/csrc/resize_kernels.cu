@@ -5,8 +5,7 @@
 //   cv::resize(..., INTER_LINEAR)  low-res depth  -> next level libs/MVS/SceneDensify.cpp:661
 //   cv::resize(..., INTER_NEAREST) low-res normal -> next level libs/MVS/SceneDensify.cpp:662
 // One thread per destination pixel; HBM-bound, a few MB per level.
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "resize_common.cuh"
 
 namespace {
 

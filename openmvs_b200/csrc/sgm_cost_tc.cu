@@ -23,25 +23,12 @@
 //              the volume with coalesced 16-byte stores.  The B tiles live in a ring of four: a block re-uses the last
 //              nTiles - 2 tiles of the block before it.
 // SASS: HGMMA (wgmma.mma_async), WARPGROUP.ARRIVE / WARPGROUP.DEPBAR (fence, wait).
-#include <cuda_runtime.h>
+#include "sgm_common.cuh"
 #include <cuda_fp16.h>
-#include <stdint.h>
 #include <string.h>
-
-struct SGMPixel { unsigned long long idx; short dmin, dmax; int pad; };
-struct SGMParams {
-	const float* lgray; const uchar3* lbgr; const float* rgray;
-	int w, h, vw, vh;
-	const SGMPixel* px;
-	uint8_t* costs; uint16_t* accums;
-	int P1;
-	uint16_t P2s[256];
-	int maxNumDisp;
-};
 
 namespace {
 
-constexpr int HW = 3, NT = 49;
 constexpr int BM = 128;          // pixels per block (two wgmma M = 64 halves)
 constexpr int BN = 64;           // right-image columns per tile (two wgmma N = 32 halves)
 constexpr int KP = 64;           // taps padded to the MMA K granularity (4 x 16)
@@ -109,13 +96,13 @@ __device__ __forceinline__ void build_a_quarter(unsigned char* sA, const unsigne
 	float2* part = (float2*)(sStage + ST_PART);
 	float wv[NN], gv[NN];
 	float sumW = 0.f, acc = 0.f;
-	const uint32_t cc = lc[HW*SP + row+HW];
+	const uint32_t cc = lc[SGM_HW*SP + row+SGM_HW];
 	#pragma unroll
 	for (int k = 0; k < NN; ++k) {
 		const int n = N0+k, i = n/7, j = n-7*i;   // compile-time after unrolling
 		const uint32_t d = __vabsdiffu4(lc[i*SP + row+j], cc);
 		const int dist2 = (int)__dp4a(d, d, 0u);
-		const float spatial = float((j-HW)*(j-HW)+(i-HW)*(i-HW))*(SIGMA_SPATIAL*LOG2E);
+		const float spatial = float((j-SGM_HW)*(j-SGM_HW)+(i-SGM_HW)*(i-SGM_HW))*(SIGMA_SPATIAL*LOG2E);
 		float wgt = ex2_approx(fmaf((float)dist2, SIGMA_COLOR*LOG2E, spatial));
 		if (!valid) wgt = 0.f;
 		const float g = lg[i*SP + row+j];
@@ -169,7 +156,7 @@ __device__ __forceinline__ void build_b_quarter(unsigned char* slot, const unsig
 		for (int e = 0; e < 8; ++e) {
 			const int n = kc*8+e;
 			float f = 0.f;
-			if (n < NT) { const int i = n/7, j = n-7*i; f = rg[i*SP + cs+c+j]; }
+			if (n < SGM_NT) { const int i = n/7, j = n-7*i; f = rg[i*SP + cs+c+j]; }
 			split_h(f, fh[e], fl[e]);
 			split_h(f*f, qh[e], ql[e]);
 		}
@@ -319,7 +306,7 @@ sgm_cost_tc_kernel(const __grid_constant__ SGMParams P, int dmin, int num, int n
 				const int row = h ? rowB : rowA, col = x0+row;
 				normSq0[h] = (sNorm[row]+sNorm[BM+row])+(sNorm[2*BM+row]+sNorm[3*BM+row]);
 				invW[h] = sInv[row];
-				dlo[h] = max(0, -(col+dmin)); dhi[h] = min(num, w-2*HW-col-dmin);
+				dlo[h] = max(0, -(col+dmin)); dhi[h] = min(num, w-2*SGM_HW-col-dmin);
 			}
 			// sums -> costs, tile by tile, into the shared cost tile
 			#pragma unroll 1

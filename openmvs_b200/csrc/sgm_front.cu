@@ -28,25 +28,12 @@
 //     never splits (a split warp runs every shuffle through a collective re-synchronisation).
 // Bit-exact against the oracle (tests/test_sgm_parity_gpu.py); the per-direction kernels of sgm_kernels.cu remain for
 // ragged (tSGM) ranges and as debug variants (b200mvs_debug.sgmAggregation).
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "sgm_common.cuh"
+#include "sgm_front_sched.h"
 #include <string.h>
 #include <algorithm>
 #include <vector>
 #include <type_traits>
-
-struct SGMPixel { unsigned long long idx; short dmin, dmax; int pad; };
-struct SGMParams {
-	const float* lgray; const uchar3* lbgr; const float* rgray;
-	int w, h, vw, vh;
-	const SGMPixel* px;
-	uint8_t* costs; uint16_t* accums;
-	int P1;
-	uint16_t P2s[256];
-	int maxNumDisp;
-};
-
-#include "sgm_front_sched.h"
 
 namespace {
 

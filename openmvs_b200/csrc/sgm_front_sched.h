@@ -1,5 +1,5 @@
 // sgm_front_sched.h — work items and schedule of the wave-front SGM aggregation (sgm_front.cu), shared by the kernel, the host
-// driver (capi.cu) and the CPU simulation of the schedule (tests/cpp/front_sched_main.cpp, run by tests/test_sgm_front_schedule.py).
+// driver (sgm_host.cu) and the CPU simulation of the schedule (tests/cpp/front_sched_main.cpp, run by tests/test_sgm_front_schedule.py).
 #pragma once
 #include <stdint.h>
 #include <algorithm>

@@ -9,26 +9,12 @@
 //   sgm_wta_kernel        first arg-min of the summed path costs                            :1272-1301
 // The cost volume is ragged: pixel p owns costs[p.idx .. p.idx + (dmax-dmin)) (PixelData,
 // libs/MVS/SemiGlobalMatcher.h:78-81); it is uint8, the path sum uint16 — HBM-bound integer work.
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "sgm_common.cuh"
 #include <string.h>
 #include <stdlib.h>
 
-struct SGMPixel { unsigned long long idx; short dmin, dmax; int pad; };
-
-struct SGMParams {
-	const float* lgray; const uchar3* lbgr; const float* rgray;
-	int w, h, vw, vh;           // image size, valid-region size (w-6, h-6)
-	const SGMPixel* px;
-	uint8_t* costs; uint16_t* accums;
-	int P1;
-	uint16_t P2s[256];
-	int maxNumDisp;
-};
-
 namespace {
 
-constexpr int HW = 3, NT = 49;
 constexpr int COST_THREADS = 128;
 
 // ---- (1) cost ----------------------------------------------------------------------------
@@ -41,22 +27,22 @@ sgm_cost_kernel(const __grid_constant__ SGMParams P)
 	if (col >= P.vw) return;
 	const SGMPixel p = P.px[(size_t)r*P.vw + col];
 	if (!(p.dmin < p.dmax)) return;
-	const int ux = col+HW, uy = r+HW;
+	const int ux = col+SGM_HW, uy = r+SGM_HW;
 	const float sigmaColor = -1.f/(2.f*(0.3f*255)*(0.3f*255));
 	const float sigmaSpatial = -1.f/(2.f*(0.4f*7)*(0.4f*7));
 	float2* w = sw + threadIdx.x;
 	const uchar3 cc = P.lbgr[(size_t)uy*P.w + ux];
 	float acc = 0.f, sumW = 0.f;
 	#pragma unroll 1
-	for (int i = -HW; i <= HW; ++i) {
+	for (int i = -SGM_HW; i <= SGM_HW; ++i) {
 		#pragma unroll
-		for (int j = -HW; j <= HW; ++j) {
+		for (int j = -SGM_HW; j <= SGM_HW; ++j) {
 			const size_t o = (size_t)(uy+i)*P.w + (ux+j);
 			const uchar3 pc = P.lbgr[o];
 			const int d0 = abs((int)pc.x-(int)cc.x), d1 = abs((int)pc.y-(int)cc.y), d2 = abs((int)pc.z-(int)cc.z);
 			const float wgt = expf(float(d0*d0+d1*d1+d2*d2)*sigmaColor + float(j*j+i*i)*sigmaSpatial);
 			const float g = __ldg(P.lgray + o);
-			w[((i+HW)*7+(j+HW))*COST_THREADS] = make_float2(wgt, g);
+			w[((i+SGM_HW)*7+(j+SGM_HW))*COST_THREADS] = make_float2(wgt, g);
 			acc += g*wgt;
 			sumW += wgt;
 		}
@@ -64,7 +50,7 @@ sgm_cost_kernel(const __grid_constant__ SGMParams P)
 	const float tm = acc/sumW;
 	float normSq0 = 0.f;
 	#pragma unroll 7
-	for (int n = 0; n < NT; ++n) {
+	for (int n = 0; n < SGM_NT; ++n) {
 		float2 e = w[n*COST_THREADS];
 		const float t = e.y-tm;
 		e.y = e.x*t;
@@ -79,19 +65,19 @@ sgm_cost_kernel(const __grid_constant__ SGMParams P)
 	constexpr int DCH = 4;
 	#pragma unroll 1
 	for (int d = p.dmin; d < p.dmax; d += DCH) {
-		const int x0 = ux-HW+d;
+		const int x0 = ux-SGM_HW+d;
 		float sum[DCH], sumSq[DCH], nom[DCH];
 		#pragma unroll
 		for (int q = 0; q < DCH; ++q) { sum[q] = 0.f; sumSq[q] = 0.f; nom[q] = 0.f; }
-		int col[2*HW+DCH];
+		int col[2*SGM_HW+DCH];
 		#pragma unroll
-		for (int t = 0; t < 2*HW+DCH; ++t) col[t] = min(max(x0+t, 0), P.w-1);
+		for (int t = 0; t < 2*SGM_HW+DCH; ++t) col[t] = min(max(x0+t, 0), P.w-1);
 		#pragma unroll
 		for (int i = 0; i < 7; ++i) {
-			const float* rp = P.rgray + (size_t)(uy-HW+i)*P.w;
-			float f[2*HW+DCH];
+			const float* rp = P.rgray + (size_t)(uy-SGM_HW+i)*P.w;
+			float f[2*SGM_HW+DCH];
 			#pragma unroll
-			for (int t = 0; t < 2*HW+DCH; ++t) f[t] = __ldg(rp + col[t]);
+			for (int t = 0; t < 2*SGM_HW+DCH; ++t) f[t] = __ldg(rp + col[t]);
 			#pragma unroll
 			for (int j = 0; j < 7; ++j) {
 				const float2 e = w[(i*7+j)*COST_THREADS];
@@ -111,7 +97,7 @@ sgm_cost_kernel(const __grid_constant__ SGMParams P)
 				const float normSq1 = sumSq[q] - sum[q]*sum[q]/sumW;
 				const float ncc = nom[q]/sqrtf(normSq0*normSq1+eps);
 				uint8_t cst = ncc <= 0.f ? (uint8_t)255 : (uint8_t)(int)floorf((1.f-fminf(ncc, 1.f))*255.f+.5f);
-				if (x0+q < 0 || x0+q+2*HW >= P.w) cst = 255;
+				if (x0+q < 0 || x0+q+2*SGM_HW >= P.w) cst = 255;
 				costs[d-p.dmin+q] = cst;
 			}
 		}
@@ -647,13 +633,13 @@ __global__ void sgm_cross_check_kernel(int16_t* __restrict__ l2r, const int16_t*
 	const int c = blockIdx.x*blockDim.x + threadIdx.x, r = blockIdx.y;
 	if (c >= w) return;
 	const int16_t ld = l2r[(size_t)r*w+c];
-	if (ld == 32767) return;
+	if (ld == SGM_NO_DISP) return;
 	const int vx = c+ld;
 	int16_t out = ld;
-	if (vx < 0 || vx >= w) out = 32767;
+	if (vx < 0 || vx >= w) out = SGM_NO_DISP;
 	else {
 		const int16_t rd = r2l[(size_t)r*w+vx];
-		if (rd == 32767 || abs((int)ld+(int)rd) > th) out = 32767;
+		if (rd == SGM_NO_DISP || abs((int)ld+(int)rd) > th) out = SGM_NO_DISP;
 	}
 	l2r[(size_t)r*w+c] = out;
 }
@@ -665,7 +651,7 @@ __global__ void sgm_refine_kernel(const SGMPixel* __restrict__ px, const uint16_
 	const SGMPixel p = px[i];
 	if (p.dmax-p.dmin < 2) return;
 	const int16_t d = disparity[i];
-	if (d == 32767) return;
+	if (d == SGM_NO_DISP) return;
 	const uint16_t* a = accums + p.idx;
 	const int k = d-p.dmin;
 	float disp = (float)d;
@@ -735,7 +721,7 @@ cudaError_t sgm_configure_device() {
 	cudaError_t e;
 	if ((e = configure_ring<4, 16>()) != cudaSuccess) return e;
 	if ((e = configure_ring<8, 8>()) != cudaSuccess) return e;
-	return cudaFuncSetAttribute(sgm_cost_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)NT*COST_THREADS*sizeof(float2)));
+	return cudaFuncSetAttribute(sgm_cost_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)SGM_NT*COST_THREADS*sizeof(float2)));
 }
 cudaError_t sgm_launch_maxdisp(const SGMPixel* px, int n, unsigned long long numCosts, int* out8, cudaStream_t s) {
 	int dev = 0, sms = 0;
@@ -765,7 +751,7 @@ cudaError_t sgm_launch_aggregate_uniform(const SGMParams& P, int dir, int dmin, 
 	return cudaGetLastError();
 }
 cudaError_t sgm_launch_cost(const SGMParams& P, cudaStream_t s) {
-	const size_t smem = (size_t)NT*COST_THREADS*sizeof(float2);
+	const size_t smem = (size_t)SGM_NT*COST_THREADS*sizeof(float2);
 	dim3 grid((P.vw+COST_THREADS-1)/COST_THREADS, P.vh);
 	sgm_cost_kernel<<<grid, COST_THREADS, smem, s>>>(P);
 	return cudaGetLastError();

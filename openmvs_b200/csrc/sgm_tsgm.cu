@@ -10,15 +10,10 @@
 //   tsgm_area_u8_kernel                      cv::resize(INTER_AREA) of the 8-bit colour pyramid (ViewData::GetImage,
 //                                            SemiGlobalMatcher.h:127-142) at an integer factor
 // All integer work on a few MB; one thread per pixel (per row for ExtractMask).  Every result is bit-exact to the sequential code.
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "sgm_common.cuh"
 #include <cub/device/device_scan.cuh>
 
-struct SGMPixel { unsigned long long idx; short dmin, dmax; int pad; };
-
 namespace {
-
-constexpr int NO_DISP = 32767;
 
 inline dim3 grid2(int w, int h, dim3 b) { return dim3((w+b.x-1)/b.x, (h+b.y-1)/b.y); }
 
@@ -32,7 +27,7 @@ __device__ int window_kth(const int16_t* __restrict__ D, int W, int H, int r, in
 		for (int i = i0; i <= i1; ++i)
 			for (int j = j0; j <= j1; ++j) {
 				const int d = D[(size_t)i*W+j];
-				cnt += (d != NO_DISP && d <= mid) ? 1 : 0;
+				cnt += (d != SGM_NO_DISP && d <= mid) ? 1 : 0;
 			}
 		if (cnt > k) hi = mid; else lo = mid+1;
 	}
@@ -46,15 +41,15 @@ __global__ void tsgm_range_kernel(const int16_t* __restrict__ D, int W, int H, c
 {
 	const int c = blockIdx.x*blockDim.x+threadIdx.x, r = blockIdx.y*blockDim.y+threadIdx.y;
 	if (c >= W || r >= H) return;
-	short lo = NO_DISP, hi = NO_DISP;
+	short lo = SGM_NO_DISP, hi = SGM_NO_DISP;
 	if (mask[(size_t)(2*r+3)*mw + 2*c+3] != 0) {
-		const bool bInvalid = D[(size_t)r*W+c] == NO_DISP;
+		const bool bInvalid = D[(size_t)r*W+c] == SGM_NO_DISP;
 		const int hw = bInvalid ? 20 : 3;
 		int n = 0, mn = 0x7FFFFFFF, mx = -0x7FFFFFFF;
 		for (int i = max(r-hw, 0); i <= min(r+hw, H-1); ++i)
 			for (int j = max(c-hw, 0); j <= min(c+hw, W-1); ++j) {
 				const int d = D[(size_t)i*W+j];
-				if (d != NO_DISP) { ++n; mn = min(mn, d); mx = max(mx, d); }
+				if (d != SGM_NO_DISP) { ++n; mn = min(mn, d); mx = max(mx, d); }
 			}
 		if (n < 3) {
 			hi = (short)min((int)(short)(W*2/3), minNumDispInvalid);
@@ -114,7 +109,7 @@ __global__ void tsgm_flip_scatter_kernel(const int16_t* __restrict__ l2r, int W,
 	const int c = blockIdx.x*blockDim.x+threadIdx.x, r = blockIdx.y*blockDim.y+threadIdx.y;
 	if (c >= W || r >= H) return;
 	const int d = l2r[(size_t)r*W+c];
-	if (d == NO_DISP) return;
+	if (d == SGM_NO_DISP) return;
 	const unsigned key = ((unsigned)(c+1) << 16) | (unsigned)(uint16_t)(int16_t)(-d);
 	for (int x = max(c+d-1, 0), xe = min(c+d+2, W); x < xe; ++x)
 		atomicMax(keys+(size_t)r*W+x, key);
@@ -123,7 +118,7 @@ __global__ void tsgm_flip_resolve_kernel(const unsigned* __restrict__ keys, int1
 	const size_t i = (size_t)blockIdx.x*blockDim.x+threadIdx.x;
 	if (i >= n) return;
 	const unsigned k = keys[i];
-	r2l[i] = k ? (int16_t)(uint16_t)(k & 0xFFFFu) : (int16_t)NO_DISP;
+	r2l[i] = k ? (int16_t)(uint16_t)(k & 0xFFFFu) : (int16_t)SGM_NO_DISP;
 }
 
 // UpscaleMask: coarse (r, c) owns the 2x2 block at (2r+3, 2c+3); everything else is INVALID
@@ -149,14 +144,14 @@ __global__ void tsgm_extract_mask_kernel(const int16_t* __restrict__ D, uint8_t*
 	for (int c = 0; c < W; ++c) {
 		if (m[c] == 0) continue;
 		m[c] = 0;
-		if (d[c] == NO_DISP) continue;
+		if (d[c] == SGM_NO_DISP) continue;
 		if (++numValid >= thValid) break;
 	}
 	numValid = 0;
 	for (int c = W; --c >= 0; ) {
 		if (m[c] == 0) continue;
 		m[c] = 0;
-		if (d[c] == NO_DISP) continue;
+		if (d[c] == SGM_NO_DISP) continue;
 		if (++numValid >= thValid) break;
 	}
 }
@@ -251,12 +246,12 @@ __global__ void tsgm_fill_kernel(int16_t* __restrict__ d, size_t n, int16_t v) {
 }
 
 __global__ void tsgm_minmax_init_kernel(int* out) { out[0] = 0x7FFFFFFF; out[1] = -0x7FFFFFFF-1; }
-// out[0] = min, out[1] = max of the values != NO_DISP (initialised to INT_MAX / INT_MIN by tsgm_minmax_init_kernel)
+// out[0] = min, out[1] = max of the values != SGM_NO_DISP (initialised to INT_MAX / INT_MIN by tsgm_minmax_init_kernel)
 __global__ void tsgm_minmax_kernel(const int16_t* __restrict__ d, size_t n, int* out) {
 	int lo = 0x7FFFFFFF, hi = -0x7FFFFFFF-1;
 	for (size_t i = (size_t)blockIdx.x*blockDim.x+threadIdx.x; i < n; i += (size_t)gridDim.x*blockDim.x) {
 		const int v = d[i];
-		if (v != NO_DISP) { lo = min(lo, v); hi = max(hi, v); }
+		if (v != SGM_NO_DISP) { lo = min(lo, v); hi = max(hi, v); }
 	}
 	lo = __reduce_min_sync(0xFFFFFFFFu, lo); hi = __reduce_max_sync(0xFFFFFFFFu, hi);
 	if ((threadIdx.x&31) == 0) { atomicMin(out, lo); atomicMax(out+1, hi); }
