@@ -246,7 +246,8 @@ int b200mvs_sgm_cross_check_device(b200mvs_ctx* ctx, int16_t* l2r, const int16_t
 
 /* RefineDisparityMap (SemiGlobalMatcher.cpp:1693-1811) with SUBPIXEL_LC_BLEND: sub-pixel offset from the
  * accumulated costs around the winner, result stored as round(disparity * subpixelSteps).  DEVICE pointers;
- * accums = NULL uses the accumulated costs of the last match on this context. */
+ * accums = NULL uses the accumulated costs of the last match on this context.  Left unchanged: NO_DISP, pixels whose range is
+ * narrower than 2, and disparities outside the pixel's [dmin, dmax) (they would index another pixel's costs). */
 int b200mvs_sgm_refine_device(b200mvs_ctx* ctx, const b200mvs_sgm_pixel* pixels, const uint16_t* accums,
 	int16_t* disparity, int nPixels, int subpixelSteps, void* stream);
 

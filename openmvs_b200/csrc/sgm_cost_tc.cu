@@ -8,8 +8,12 @@
 // K = 49 taps padded to 64) and the Toeplitz matrix B[n, u] = right(y+i, u+j) (u = x + d, the right-image column), the wanted
 // entries are D[x, u] for u - x in [dmin, dmin+D).  The band is cut into 64-column tiles of u; a tile serves two pixel blocks, a
 // block needs (128+D)/64 tiles (band utilisation 50 % at D = 128).  Precision: the operands are split into fp16 high and low
-// parts (w = wh + wl, error 2^-22) and every sum is three f16 MMAs with fp32 accumulation (wh fh + wh fl + wl fh) — the dropped
-// wl fl term is 2^-22 relative — so the uint8 cost stays within the +-1 level of the SIMT kernel.
+// parts (w = wh + wl) and every sum is three f16 MMAs with fp32 accumulation (wh fh + wh fl + wl fh).  For operands of 2^-3 and
+// more the split keeps 22 bits (error 2^-22 relative, and the dropped wl fl term is 2^-22 relative too); below that the low part,
+// and below 2^-14 the high part, are fp16 subnormals with an absolute error of up to 2^-25 each.  Bilateral weights of saturated
+// colour contrast reach exp(-17.8) ~ 1.9e-8 and keep no relative precision, but their absolute error is what enters the sums:
+// tests/test_sgm_reference_gpu.py bounds it as 2^-25 per operand and product, and the kernel equals the float64 cost on every
+// entry that this bound (with 2^-20 relative per product) leaves decidable.
 //
 // Structure (one CTA of 16 warps = 4 warpgroups per SM, persistent over the rows of the valid region):
 //   all warps stage the seven image rows of the block in shared memory (left colour packed to a word, left and right gray) and
@@ -76,7 +80,8 @@ __device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t adesc, 
 		: "l"(adesc), "l"(bdesc), "r"(accumulate) : "memory");
 }
 __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) { return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b)<<16); }
-// x = hi + lo with hi = fp16(x): two fp16 numbers carrying 22 bits of x
+// x = hi + lo with hi = fp16(x): two fp16 numbers carrying 22 bits of x for |x| >= 2^-3 (an absolute error <= 2^-25 below, where
+// lo, and below 2^-14 hi, is subnormal)
 __device__ __forceinline__ void split_h(float x, __half& hi, __half& lo) { hi = __float2half_rn(x); lo = __float2half_rn(x-__half2float(hi)); }
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 

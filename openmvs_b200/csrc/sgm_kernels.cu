@@ -651,7 +651,9 @@ __global__ void sgm_refine_kernel(const SGMPixel* __restrict__ px, const uint16_
 	const SGMPixel p = px[i];
 	if (p.dmax-p.dmin < 2) return;
 	const int16_t d = disparity[i];
-	if (d == SGM_NO_DISP) return;
+	// NO_DISP, and a disparity outside the pixel's range (the caller's map need not come from this volume): left unchanged
+	// instead of reading another pixel's slice
+	if (d == SGM_NO_DISP || d < p.dmin || d >= p.dmax) return;
 	const uint16_t* a = accums + p.idx;
 	const int k = d-p.dmin;
 	float disp = (float)d;
