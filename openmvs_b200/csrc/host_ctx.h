@@ -50,7 +50,7 @@ struct b200mvs_ctx {
 	DevBuf sgFrontCtl, sgFrontState, sgFrontMeta;
 	cudaStream_t sgSide[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // side streams of the ragged aggregation
 	cudaEvent_t sgJoin[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}, sgFork = nullptr;
-	const void* sgLastPx = nullptr; uint64_t sgLastNum = 0; // pixel map / size of the volume in sgAccums (b200mvs_sgm_refine_device check)
+	const void* sgLastPx = nullptr;           // pixel map of the volume in sgAccums (b200mvs_sgm_refine_device check)
 	// hierarchical matcher: level images, masks, disparity maps, pixel maps, Disparity2RangeMap / FlipDirection / speckle scratch
 	enum { TS_IMG, TS_MASKL, TS_MASKR, TS_MASKT, TS_DL, TS_DR, TS_DL0, TS_DR0, TS_PXL, TS_PXR, TS_RANGES, TS_SCAN, TS_KEYS, TS_LABELS,
 		TS_SIZES, TS_SMALL, TS_COUNT };

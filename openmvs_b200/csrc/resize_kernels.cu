@@ -67,18 +67,6 @@ __device__ __forceinline__ void linear_tap(int d, int ssize, double scale, int& 
 	if (s >= ssize-1) { f = 0.f; s = ssize-1; }
 }
 
-__global__ void resize_linear_kernel(const float* __restrict__ src, int sw, int sh, float* __restrict__ dst, int dw, int dh, double scx, double scy) {
-	const int x = blockIdx.x*blockDim.x + threadIdx.x, y = blockIdx.y*blockDim.y + threadIdx.y;
-	if (x >= dw || y >= dh) return;
-	int x0, y0; float fx, fy;
-	linear_tap(x, sw, scx, x0, fx);
-	linear_tap(y, sh, scy, y0, fy);
-	const int x1 = min(x0+1, sw-1), y1 = min(y0+1, sh-1);
-	const float r0 = src[(size_t)y0*sw+x0]*(1.f-fx) + src[(size_t)y0*sw+x1]*fx;
-	const float r1 = src[(size_t)y1*sw+x0]*(1.f-fx) + src[(size_t)y1*sw+x1]*fx;
-	dst[(size_t)y*dw+x] = r0*(1.f-fy) + r1*fy;
-}
-
 __global__ void resize_nearest_kernel(const float* __restrict__ src, int sw, int sh, int ch, float* __restrict__ dst, int dw, int dh, double ifx, double ify) {
 	const int x = blockIdx.x*blockDim.x + threadIdx.x, y = blockIdx.y*blockDim.y + threadIdx.y;
 	if (x >= dw || y >= dh) return;
@@ -164,11 +152,6 @@ cudaError_t rs_launch_area(const float* src, int sw, int sh, int spitch, float* 
 cudaError_t rs_launch_cubic(const float* src, int sw, int sh, int spitch, float* dst, int dw, int dh, int dpitch, double scx, double scy, cudaStream_t s) {
 	dim3 b(32, 8);
 	resize_cubic_kernel<<<grid2(dw, dh, b), b, 0, s>>>(src, sw, sh, spitch, dst, dw, dh, dpitch, scx, scy);
-	return cudaGetLastError();
-}
-cudaError_t rs_launch_linear(const float* src, int sw, int sh, float* dst, int dw, int dh, cudaStream_t s) {
-	dim3 b(32, 8);
-	resize_linear_kernel<<<grid2(dw, dh, b), b, 0, s>>>(src, sw, sh, dst, dw, dh, (double)sw/dw, (double)sh/dh);
 	return cudaGetLastError();
 }
 // scx/scy: source/destination scale; 1/factor for the factor form cv::resize(..., Size(), fx, fy, INTER_NEAREST)

@@ -24,16 +24,27 @@ struct SGMParams {
 
 constexpr int SGM_HW = 3, SGM_NT = 49;   // half width and taps of the 7x7 WZNCC window
 constexpr int SGM_NO_DISP = 32767;       // invalid disparity (NO_DISP, libs/MVS/SemiGlobalMatcher.h:68)
+constexpr int SGM_MAX_DISP = 256;        // disparities per pixel: the warp-per-scanline kernel keeps one line of at most this many
+
+// statistics of a pixel map, over its valid pixels unless stated (sgm_launch_map_stats); the kernel writes the fields in this order
+struct SGMMapStats {
+	int maxNum;           // largest disparity count dmax-dmin
+	int dminLo, dminHi;   // min / max of dmin
+	int dmaxLo, dmaxHi;   // min / max of dmax
+	int idxLowBits;       // OR of (idx & 15)
+	int notDense;         // 1: an invalid pixel, or idx != pixel index x disparity count
+	int overflow;         // 1: a slice ends beyond numCosts
+};
+static_assert(sizeof(SGMMapStats) == 8*sizeof(int), "pixel-map statistics layout");
 
 // sgm_kernels.cu
 cudaError_t sgm_configure_device();
-cudaError_t sgm_launch_maxdisp(const SGMPixel* px, int n, unsigned long long numCosts, int* out8, cudaStream_t s);
+cudaError_t sgm_launch_map_stats(const SGMPixel* px, int n, unsigned long long numCosts, SGMMapStats* out, cudaStream_t s);
 cudaError_t sgm_launch_cost(const SGMParams& P, cudaStream_t s);
 cudaError_t sgm_launch_aggregate(const SGMParams& P, int dir, bool store, cudaStream_t s);
 cudaError_t sgm_launch_aggregate_uniform(const SGMParams& P, int dir, int dmin, int num, bool ring, cudaStream_t s);
 cudaError_t sgm_launch_wta(const SGMParams& P, int nVol, unsigned long long volStride, const uint16_t* more, int16_t* disparity, uint16_t* cost, cudaStream_t s);
 cudaError_t sgm_launch_wta_uniform(const SGMParams& P, const uint16_t* second, int dmin, int num, int16_t* disparity, uint16_t* cost, cudaStream_t s);
-int sgm_max_disparities();
 cudaError_t sgm_launch_cross_check(int16_t* l2r, const int16_t* r2l, int w, int h, int th, cudaStream_t s);
 cudaError_t sgm_launch_refine(const SGMPixel* px, const uint16_t* accums, int16_t* disparity, int n, int steps, cudaStream_t s);
 // sgm_cost_tc.cu

@@ -1,5 +1,6 @@
-// sgm_front_sched.h — work items and schedule of the wave-front SGM aggregation (sgm_front.cu), shared by the kernel, the host
-// driver (sgm_host.cu) and the CPU simulation of the schedule (tests/cpp/front_sched_main.cpp, run by tests/test_sgm_front_schedule.py).
+// sgm_front_sched.h — the scanline geometry of every SGM aggregation kernel (sgm_front.cu, sgm_kernels.cu), and the work items and
+// schedule of the wave-front aggregation, shared by its kernel, the host driver (sgm_host.cu) and the CPU simulation of the schedule
+// (tests/cpp/front_sched_main.cpp, run by tests/test_sgm_front_schedule.py).
 #pragma once
 #include <stdint.h>
 #include <algorithm>
@@ -42,6 +43,8 @@ struct FrontArgs {
 	uint16_t* sum[2];
 };
 
+// number of scanlines of direction `dir` in a W x H region
+FRONT_HD inline int front_path_count(int dir, int W, int H) { return dir == 0 || dir == 2 ? W : dir == 1 || dir == 3 ? H : W+H-1; }
 // start pixel and step of scanline `k` of direction `dir` (order of SemiGlobalMatcher.cpp:1084-1199); host and device
 FRONT_HD inline bool front_path_start(int dir, int k, int W, int H, int& x, int& y, int& dx, int& dy) {
 	switch (dir) {
@@ -59,6 +62,7 @@ FRONT_HD inline bool front_path_start(int dir, int k, int W, int H, int& x, int&
 		if (k < W) { x = k; y = H-1; return true; } k -= W; if (k >= H-1) return false; x = W-1; y = k; return true;
 	}
 }
+// steps until the scanline leaves the region
 FRONT_HD inline int front_path_len(int x0, int y0, int dx, int dy, int W, int H) {
 	int n = 0x7FFFFFFF;
 	if (dx > 0) n = min(n, W-x0); else if (dx < 0) n = min(n, x0+1);
@@ -101,7 +105,7 @@ inline void sgm_front_build(int vw, int vh, const FrontPassDesc& pd, int FB, int
 	cellCount.assign((size_t)pd.nDirs*nFB*nSX, 0);
 	for (int ph = 0; ph < pd.nDirs; ++ph) {
 		const int dir = pd.dirs[ph];
-		const int nPaths = dir == 0 || dir == 2 ? vw : dir == 1 || dir == 3 ? vh : vw+vh-1;
+		const int nPaths = front_path_count(dir, vw, vh);
 		for (int band = 0; band*4 < nPaths; ++band) {
 			int nv[4], f0v[4], dfv[4], xsv[4], dxv[4]; bool pv[4];
 			int blo = 0x7FFFFFFF, bhi = -1;

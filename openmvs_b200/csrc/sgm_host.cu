@@ -10,12 +10,12 @@ namespace {
 //   1 two tilted fronts f = +-(x + 2y): {right, right-down, down, left-down} and {left, left-up, up, right-up};
 //   2 four straight fronts: top-down {down, right-down, left-down}, bottom-up {up, right-up, left-up}, left-right, right-left;
 //   3 eight passes of one direction each (the traffic of the per-direction kernels with the new step).
-// Unless frontSerial is set, consecutive passes share a launch: pass 2j accumulates into the caller's volume, pass 2j+1 into a
-// second one (ctx->sgAccums2), and `twoVolumes` tells the caller to add them (the winner-takes-all kernel does).
-int sgm_aggregate_fronts(b200mvs_ctx* ctx, const SGMParams& P, int num, cudaStream_t s, bool& twoVolumes) {
+// With a `second` volume, consecutive passes share a launch: pass 2j accumulates into the caller's volume, pass 2j+1 into
+// `second`, and the caller adds the two (the winner-takes-all kernel does).  Without one, every pass has a launch of its own.
+int sgm_aggregate_fronts(b200mvs_ctx* ctx, const SGMParams& P, int num, uint16_t* second, cudaStream_t s) {
 	const b200mvs_debug& D = ctx->dbg;
 	const int layout = std::min(std::max(D.frontLayout-1, 0), 2);
-	const bool concurrent = !D.frontSerial;
+	const bool concurrent = second != nullptr;
 	const int FB = D.frontBlock > 0 ? D.frontBlock : 32;   // fronts per block: larger blocks widen the window of the sum volume kept in the L2
 	// frontLag = lag + 1.  The sub-cell dependencies make every lag legal.  A larger lag lets more blocks be in flight at once, but
 	// the window of blocks between a block's first and last phase then outgrows the L2 and the sums go to DRAM and back; lag 0
@@ -42,13 +42,6 @@ int sgm_aggregate_fronts(b200mvs_ctx* ctx, const SGMParams& P, int num, cudaStre
 		}
 		CK(cudaStreamSynchronize(s)); // the pageable source vectors die with `plan`
 		memcpy(ctx->sgFrontKey, key, sizeof(key));
-	}
-	twoVolumes = false;
-	for (auto& fp: ctx->sgFront) twoVolumes |= fp.launch.nPasses > 1;
-	uint16_t* second = nullptr;
-	if (twoVolumes) {
-		CK(ctx->sgAccums2.reserve((size_t)vw*vh*num*sizeof(uint16_t)));
-		second = ctx->sgAccums2.as<uint16_t>();
 	}
 	const int maxPaths = vw+vh+8;
 	int maxCtl = 0;
@@ -82,6 +75,41 @@ int sgm_aggregate_fronts(b200mvs_ctx* ctx, const SGMParams& P, int num, cudaStre
 		CK(sgm_front_launch(P, A, blocks, pd, s)); ++ctx->launches;
 	}
 	return B200MVS_OK;
+}
+
+// The kernels of one match (sgm_plan).
+struct SGMPlan {
+	enum Aggregation { FRONTS, UNIFORM_RING, UNIFORM, RAGGED_STREAMS, RAGGED } agg;
+	bool tcCost;     // the tensor-core cost kernel (sgm_cost_tc.cu), else sgm_cost_kernel
+	bool denseWta;   // sgm_wta_uniform_kernel, else sgm_wta_kernel
+	int volumes;     // sum volumes the aggregation leaves for the winner-takes-all to add: 1, 2 (paired wave-front passes) or 8
+};
+
+// Picks the kernels from the pixel map's statistics, the debug switches (b200mvs_debug.sgmAggregation / sgmCost / frontSerial),
+// the 16-byte alignment of the cost and sum volumes' base pointers and the largest P2.
+SGMPlan sgm_plan(const SGMMapStats& st, const b200mvs_debug& D, bool costsAligned, bool accumsAligned, int maxP2, uint64_t numCosts) {
+	const int mode = D.sgmAggregation;
+	// one global range (the non-tSGM branch): packed, shared-memory-free aggregation kernels
+	const bool uniform = st.maxNum >= 4 && st.dminLo == st.dminHi && st.dmaxLo == st.dmaxHi && (st.maxNum & 3) == 0 && (st.idxLowBits & 3) == 0
+		&& mode != 1;
+	// ... every pixel valid, pixel i's slice at i*num, num % 16 == 0
+	const bool dense = uniform && (st.maxNum & 15) == 0 && !st.notDense;
+	// every slice 16-byte aligned: bulk-copy ring kernel (one launch per direction)
+	const bool ring = uniform && (st.maxNum & 15) == 0 && st.idxLowBits == 0 && costsAligned && accumsAligned && mode != 2;
+	// dense volume of a supported width: wave-front kernel (fused directions) — the default
+	// (its step carries P2 + the previous line's minimum in 16 bits: P2 <= 16000; sums of eight paths overflow far earlier)
+	const bool front = ring && !st.notDense && sgm_front_supports(st.maxNum) && maxP2 <= 16000 && (mode == 0 || mode == 4);
+	SGMPlan p;
+	// ragged (tSGM) ranges: one volume per direction (RAGGED_STREAMS) while the seven extra volumes take at most 3.5 GiB, else
+	// the eight directions add into one volume in turn
+	p.agg = front ? SGMPlan::FRONTS : ring ? SGMPlan::UNIFORM_RING : uniform ? SGMPlan::UNIFORM
+		: numCosts <= (1ull<<28) ? SGMPlan::RAGGED_STREAMS : SGMPlan::RAGGED;
+	// dense volume with one range of 64 / 128 / 192 / 256 disparities: the banded-GEMM cost kernel on the tensor cores
+	p.tcCost = dense && costsAligned && sgm_cost_tc_supports(st.maxNum) && D.sgmCost != 1;
+	p.denseWta = dense && accumsAligned;
+	// every wave-front layout has at least two passes, so unless frontSerial is set two of them share a launch
+	p.volumes = front ? (D.frontSerial ? 1 : 2) : p.agg == SGMPlan::RAGGED_STREAMS ? 8 : 1;
+	return p;
 }
 
 } // namespace
@@ -121,52 +149,47 @@ int b200mvs_sgm_match_device(b200mvs_ctx* ctx, const float* leftGray, const uint
 	P.costs = costs; P.accums = accums;
 	const auto t0 = std::chrono::steady_clock::now();
 	ctx->launches = 0;
-	int st8[8] = {0, 0, 0, 0, 0, 0, 0, 0}; bool uniform = false, ring = false, front = false;
-	const int mode = ctx->dbg.sgmAggregation;
+	SGMMapStats st = {};
+	SGMPlan plan = {};
 	if (stats) CK(cudaEventRecord(ctx->ev0, s));
 	if (stages & 7) {
-		// the warp-per-scanline kernel keeps one line of at most sgm_max_disparities() values
-		CK(ctx->sgMax.reserve(8*sizeof(int)));
-		CK(sgm_launch_maxdisp(P.px, P.vw*P.vh, numCosts, ctx->sgMax.as<int>(), s)); ctx->launches += 2;
-		CK(cudaMemcpyAsync(st8, ctx->sgMax.p, 8*sizeof(int), cudaMemcpyDeviceToHost, s));
+		CK(ctx->sgMax.reserve(sizeof(SGMMapStats)));
+		CK(sgm_launch_map_stats(P.px, P.vw*P.vh, numCosts, ctx->sgMax.as<SGMMapStats>(), s)); ctx->launches += 2;
+		CK(cudaMemcpyAsync(&st, ctx->sgMax.p, sizeof(st), cudaMemcpyDeviceToHost, s));
 		CK(cudaStreamSynchronize(s));
-		if (st8[7])
+		if (st.overflow)
 			return fail(ctx, B200MVS_ERR_ARG, "sgm: a pixel's slice [idx, idx+dmax-dmin) ends beyond numCosts");
-		if (st8[0] > sgm_max_disparities())
+		// the warp-per-scanline kernel keeps one line of at most SGM_MAX_DISP values
+		if (st.maxNum > SGM_MAX_DISP)
 			return fail(ctx, B200MVS_ERR_ARG, "sgm: more than 256 disparities per pixel");
-		P.maxNumDisp = st8[0];
-		// one global range (the non-tSGM branch): packed, shared-memory-free aggregation kernels
-		uniform = st8[0] >= 4 && st8[1] == st8[2] && st8[3] == st8[4] && (st8[0] & 3) == 0 && (st8[5] & 3) == 0 && mode != 1;
-		// every slice 16-byte aligned: bulk-copy ring kernel (one launch per direction)
-		ring = uniform && (st8[0] & 15) == 0 && st8[5] == 0 && !((uintptr_t)P.costs & 15) && !((uintptr_t)P.accums & 15) && mode != 2;
-		// dense volume of a supported width: wave-front kernel (fused directions) — the default
-		// (its step carries P2 + the previous line's minimum in 16 bits: P2 <= 16000; sums of eight paths overflow far earlier)
-		front = ring && !st8[6] && sgm_front_supports(st8[0]) && maxP2 <= 16000 && (mode == 0 || mode == 4);
-		if (mode == 4 && !front)
+		P.maxNumDisp = st.maxNum;
+		plan = sgm_plan(st, ctx->dbg, !((uintptr_t)P.costs & 15), !((uintptr_t)P.accums & 15), maxP2, numCosts);
+		if (ctx->dbg.sgmAggregation == 4 && plan.agg != SGMPlan::FRONTS)
 			return fail(ctx, B200MVS_ERR_ARG, "sgm: the wave-front kernel needs a dense volume with one range of 64, 128 or 256 disparities");
 	}
 	if (stages & 1) {
-		// dense volume with one range of 64 / 128 disparities: the banded-GEMM cost kernel on the tensor cores (sgm_cost_tc.cu)
-		const bool dense = uniform && (st8[0] & 15) == 0 && !st8[6] && !((uintptr_t)P.costs & 15);
-		const bool tc = dense && sgm_cost_tc_supports(st8[0]) && ctx->dbg.sgmCost != 1;   // auto: the tensor-core kernel where it applies
-		if (ctx->dbg.sgmCost == 2 && !tc)
+		if (ctx->dbg.sgmCost == 2 && !plan.tcCost)
 			return fail(ctx, B200MVS_ERR_ARG, "sgm: the tensor-core cost kernel needs a dense volume with one range of 64, 128, 192 or 256 disparities");
-		if (tc) { CK(sgm_cost_tc_launch(P, st8[1], st8[0], s)); ctx->launches += (st8[0]+127)/128; }
+		if (plan.tcCost) { CK(sgm_cost_tc_launch(P, st.dminLo, st.maxNum, s)); ctx->launches += (st.maxNum+127)/128; }
 		else { CK(sgm_launch_cost(P, s)); ++ctx->launches; }
 	}
-	bool twoVolumes = false;   // the wave-front passes ran side by side: accums + ctx->sgAccums2 is the sum
-	bool eightVolumes = false; // ragged ranges: one volume per direction, accums + the seven of ctx->sgAccums2
-	if ((stages & 2) && front) {
-		const int rc = sgm_aggregate_fronts(ctx, P, st8[0], s, twoVolumes);
+	// the sum volumes the winner-takes-all adds: accums, then nVol-1 more at `more` (ctx->sgAccums2)
+	const int nVol = (stages & 2) ? plan.volumes : 1;
+	uint16_t* more = nullptr;
+	if ((stages & 2) && plan.agg == SGMPlan::FRONTS) {
+		if (nVol == 2) {
+			CK(ctx->sgAccums2.reserve((size_t)P.vw*P.vh*st.maxNum*sizeof(uint16_t)));
+			more = ctx->sgAccums2.as<uint16_t>();
+		}
+		const int rc = sgm_aggregate_fronts(ctx, P, st.maxNum, more, s);
 		if (rc) return rc;
-		if (twoVolumes && !(stages & 4)) { CK(sgm_launch_wta_uniform(P, ctx->sgAccums2.as<uint16_t>(), st8[1], st8[0], nullptr, nullptr, s)); ++ctx->launches; }
 	} else
-	if ((stages & 2) && !uniform && numCosts <= (1ull<<28)) {
+	if ((stages & 2) && plan.agg == SGMPlan::RAGGED_STREAMS) {
 		// ragged (tSGM) ranges: a direction has only 1000-3000 scanlines, one warp each — far too few to fill the GPU.  The eight
 		// directions run side by side on eight streams, each STORING its path costs into a volume of its own (no memset, no
 		// read-modify-write, no races); the winner-takes-all kernel adds the volumes.
-		eightVolumes = true;
 		CK(ctx->sgAccums2.reserve((size_t)7*numCosts*sizeof(uint16_t)));
+		more = ctx->sgAccums2.as<uint16_t>();
 		if (!ctx->sgSide[0]) {
 			for (int i = 0; i < 7; ++i) { CK(cudaStreamCreateWithFlags(&ctx->sgSide[i], cudaStreamNonBlocking)); CK(cudaEventCreateWithFlags(&ctx->sgJoin[i], cudaEventDisableTiming)); }
 			CK(cudaEventCreateWithFlags(&ctx->sgFork, cudaEventDisableTiming));
@@ -176,7 +199,7 @@ int b200mvs_sgm_match_device(b200mvs_ctx* ctx, const float* leftGray, const uint
 			SGMParams Pd = P;
 			cudaStream_t sd = s;
 			if (dir > 0) {
-				Pd.accums = ctx->sgAccums2.as<uint16_t>() + (size_t)(dir-1)*numCosts;
+				Pd.accums = more + (size_t)(dir-1)*numCosts;
 				sd = ctx->sgSide[dir-1];
 				CK(cudaStreamWaitEvent(sd, ctx->sgFork, 0));
 			}
@@ -184,21 +207,22 @@ int b200mvs_sgm_match_device(b200mvs_ctx* ctx, const float* leftGray, const uint
 			++ctx->launches;
 			if (dir > 0) { CK(cudaEventRecord(ctx->sgJoin[dir-1], sd)); CK(cudaStreamWaitEvent(s, ctx->sgJoin[dir-1], 0)); }
 		}
-		if (!(stages & 4)) { CK(sgm_launch_wta(P, 8, numCosts, ctx->sgAccums2.as<uint16_t>(), nullptr, nullptr, s)); ++ctx->launches; }
 	} else
 	if (stages & 2) {
 		CK(cudaMemsetAsync(accums, 0, numCosts*sizeof(uint16_t), s));
 		for (int dir = 0; dir < 8; ++dir) {
-			if (uniform) CK(sgm_launch_aggregate_uniform(P, dir, st8[1], st8[0], ring, s));
-			else CK(sgm_launch_aggregate(P, dir, false, s));
+			if (plan.agg == SGMPlan::RAGGED) CK(sgm_launch_aggregate(P, dir, false, s));
+			else CK(sgm_launch_aggregate_uniform(P, dir, st.dminLo, st.maxNum, plan.agg == SGMPlan::UNIFORM_RING, s));
 			++ctx->launches;
 		}
 	}
-	if (stages & 2) { ctx->sgLastPx = (accums == ctx->sgAccums.as<uint16_t>()) ? (const void*)pixels : nullptr; ctx->sgLastNum = numCosts; }
-	if (stages & 4) {
-		const bool denseWta = uniform && (st8[0] & 15) == 0 && !st8[6] && !((uintptr_t)P.accums & 15);
-		if (denseWta) CK(sgm_launch_wta_uniform(P, twoVolumes ? ctx->sgAccums2.as<uint16_t>() : nullptr, st8[1], st8[0], disparity, cost, s));
-		else CK(sgm_launch_wta(P, eightVolumes ? 8 : 1, numCosts, eightVolumes ? ctx->sgAccums2.as<uint16_t>() : nullptr, disparity, cost, s));
+	if (stages & 2) ctx->sgLastPx = (accums == ctx->sgAccums.as<uint16_t>()) ? (const void*)pixels : nullptr;
+	// the winner-takes-all; without stage 4, several volumes are still added into accums (no disparity / cost maps)
+	if ((stages & 4) || nVol > 1) {
+		int16_t* d = (stages & 4) ? disparity : nullptr;
+		uint16_t* c = (stages & 4) ? cost : nullptr;
+		if (plan.denseWta) CK(sgm_launch_wta_uniform(P, more, st.dminLo, st.maxNum, d, c, s));
+		else CK(sgm_launch_wta(P, nVol, numCosts, more, d, c, s));
 		++ctx->launches;
 	}
 	if (stats) {
@@ -206,7 +230,7 @@ int b200mvs_sgm_match_device(b200mvs_ctx* ctx, const float* leftGray, const uint
 		CK(cudaStreamSynchronize(s));
 		const int rc = fill_stats(ctx, stats, t0, 1);
 		if (rc) return rc;
-		if ((stages & 2) && front) {
+		if ((stages & 2) && plan.agg == SGMPlan::FRONTS) {
 			// the wave-front kernel flags a dependency wait that timed out (never in a correct schedule): the stream is idle here
 			int err = 0;
 			CK(cudaMemcpy(&err, ctx->sgFrontCtl.as<int>()+1, sizeof(int), cudaMemcpyDeviceToHost));
@@ -459,7 +483,7 @@ int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
 		if (mm[0] > mm[1]) return fail(ctx, B200MVS_ERR_ARG, "hierarchical sgm: minResolution = 0 needs an initial map with a valid disparity");
 		const int16_t numDisp = (int16_t)((int16_t)(mm[1]-mm[0])+16), disp = (int16_t)(mm[0]+mm[1]);
 		fixLo = (int16_t)(disp-numDisp); fixHi = (int16_t)(disp+numDisp);
-		if (fixHi-fixLo > sgm_max_disparities())
+		if (fixHi-fixLo > SGM_MAX_DISP)
 			return fail(ctx, B200MVS_ERR_ARG, "hierarchical sgm: the initial map spans more than 256 disparities with its margins");
 	}
 	// one match; an empty volume (every pixel masked) leaves NO_DISP / NO_ACCUMCOST like the winner-takes-all of invalid pixels
