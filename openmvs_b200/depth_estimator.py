@@ -141,83 +141,106 @@ def _is_torch(a) -> bool:
 	return type(a).__module__.startswith("torch")
 
 
+def _layout(a):
+	"""(address, shape, strides in bytes, dtype name) of a numpy array or a torch tensor"""
+	if _is_torch(a):
+		return a.data_ptr(), tuple(a.shape), tuple(s*a.element_size() for s in a.stride()), str(a.dtype)[len("torch."):]
+	return a.ctypes.data, a.shape, a.strides, str(a.dtype)
+
+
+def _put_camera(o, cam: Camera, suffix: str = ""):
+	for name in ("K", "R", "C"):
+		getattr(o, name+suffix)[:] = np.asarray(getattr(cam, name), np.float64).ravel()
+
+
 def _make_views(images: List[ViewData]):
 	"""-> (ctypes View array, keepalive list, on_device flag)"""
-	n = len(images)
-	arr = (_lib.View*n)()
+	arr = (_lib.View*len(images))()
 	keep = []
 	dev = _is_torch(images[0].image)
+	device = images[0].image.device if dev else None
 	for i, v in enumerate(images):
 		o = arr[i]
 		if dev != _is_torch(v.image):
 			raise ValueError("mixing host and device images in one DepthData")
-		if dev:
-			img = v.image
-			if not img.is_cuda or img.device != images[0].image.device:
-				raise ValueError("all views of a DepthData must live on the same CUDA device")
-			if img.dtype.__str__() == "torch.uint8":
-				# 8-bit colour image: toGray runs on the device inside the call
-				if img.dim() != 3 or img.shape[2] not in (3, 4) or img.stride(2) != 1 or img.stride(1) != img.shape[2]:
-					raise ValueError("device colour image must be a (H, W, 3|4) uint8 CUDA tensor with packed pixels")
-				keep.append(img)
-				o.image = None; o.image8 = img.data_ptr(); o.height, o.width, o.channels8 = (int(x) for x in img.shape)
-				o.stride8_bytes = img.stride(0); o.bgr8 = int(bool(v.bgr))
-			else:
-				if img.dtype.__str__() != "torch.float32" or img.dim() != 2 or img.stride(1) != 1:
-					raise ValueError("device image must be a 2-D float32 CUDA tensor with unit column stride")
-				keep.append(img)
-				o.image = img.data_ptr(); o.height, o.width = img.shape; o.stride_bytes = img.stride(0)*4
+		img = v.image if dev else np.asarray(v.image)
+		if dev and (not img.is_cuda or img.device != device):
+			raise ValueError("all views of a DepthData must live on the same CUDA device")
+		ptr, shape, strides, dtype = _layout(img)
+		keep.append(img)
+		if dtype == "uint8":
+			# 8-bit colour image: toGray runs on the device inside the call
+			if len(shape) != 3 or shape[2] not in (3, 4) or strides[2] != 1 or strides[1] != shape[2]:
+				raise ValueError("colour image must be a (H, W, 3|4) uint8 array or CUDA tensor with packed pixels (Image8U3)")
+			o.image8 = ptr; o.height, o.width, o.channels8 = shape; o.stride8_bytes = strides[0]; o.bgr8 = int(bool(v.bgr))
 		else:
-			img = np.asarray(v.image)
-			if img.dtype == np.uint8:
-				if img.ndim != 3 or img.shape[2] not in (3, 4) or img.strides[2] != 1 or img.strides[1] != img.shape[2]:
-					raise ValueError("colour image must be a (H, W, 3|4) uint8 array with packed pixels (Image8U3)")
-				keep.append(img)
-				o.image = None; o.image8 = img.ctypes.data; o.height, o.width, o.channels8 = img.shape
-				o.stride8_bytes = img.strides[0]; o.bgr8 = int(bool(v.bgr))
-			else:
-				if img.dtype != np.float32 or img.ndim != 2 or img.strides[1] != 4:
-					raise ValueError("image must be a 2-D float32 array with contiguous rows (Image32F)")
-				keep.append(img)
-				o.image = img.ctypes.data; o.height, o.width = img.shape; o.stride_bytes = img.strides[0]
-		o.K[:] = np.asarray(v.camera.K, np.float64).ravel()
-		o.R[:] = np.asarray(v.camera.R, np.float64).ravel()
-		o.C[:] = np.asarray(v.camera.C, np.float64).ravel()
-		o.depth = None
+			if dtype != "float32" or len(shape) != 2 or strides[1] != 4:
+				raise ValueError("image must be a 2-D float32 array or CUDA tensor with contiguous rows (Image32F)")
+			o.image = ptr; o.height, o.width = shape; o.stride_bytes = strides[0]
+		_put_camera(o, v.camera)
 		if v.depthMap is not None and i > 0:
-			cam = v.cameraDepthMap or v.camera
-			if dev:
-				dm = v.depthMap
-				if not _is_torch(dm) or dm.dtype.__str__() != "torch.float32" or not dm.is_cuda or dm.dim() != 2 or dm.stride(1) != 1 or dm.device != images[0].image.device:
-					raise ValueError("device depth-map must be a 2-D float32 CUDA tensor with unit column stride on the images' device")
-				keep.append(dm)
-				o.depth = dm.data_ptr(); o.dheight, o.dwidth = dm.shape; o.dstride_bytes = dm.stride(0)*4
-			else:
-				dm = np.ascontiguousarray(v.depthMap, np.float32)
-				keep.append(dm)
-				o.depth = dm.ctypes.data; o.dheight, o.dwidth = dm.shape; o.dstride_bytes = dm.strides[0]
-			o.Kd[:] = np.asarray(cam.K, np.float64).ravel()
-			o.Rd[:] = np.asarray(cam.R, np.float64).ravel()
-			o.Cd[:] = np.asarray(cam.C, np.float64).ravel()
+			dm = v.depthMap if dev else np.ascontiguousarray(v.depthMap, np.float32)
+			if dev and not (_is_torch(dm) and dm.is_cuda and dm.device == device):
+				raise ValueError("device depth-map must be a CUDA tensor on the images' device")
+			ptr, shape, strides, dtype = _layout(dm)
+			if dtype != "float32" or len(shape) != 2 or strides[1] != 4:
+				raise ValueError("depth-map must be a 2-D float32 array or CUDA tensor with unit column stride")
+			keep.append(dm)
+			o.depth = ptr; o.dheight, o.dwidth = shape; o.dstride_bytes = strides[0]
+			_put_camera(o, v.cameraDepthMap or v.camera, "d")
 	return arr, keep, dev
 
 
-class PatchMatchB200:
-	"""Drop-in for the reference's `PatchMatchCUDA` (libs/MVS/PatchMatchCUDA.inl:78-131)."""
+# the output maps of a DepthData: (name, channels, dtype)
+_MAPS = (("depthMap", (), "float32"), ("normalMap", (3,), "float32"), ("confMap", (), "float32"), ("viewsMap", (4,), "uint8"))
 
-	def __init__(self, device: int = 0):
+
+def _host_maps(dd: DepthData):
+	"""Allocate the missing output maps of dd as zeroed numpy arrays and check the given ones -> their addresses."""
+	h, w = dd.images[0].image.shape[:2]
+	for name, ch, dtype in _MAPS:
+		a = getattr(dd, name)
+		if a is None:
+			a = np.zeros((h, w)+ch, dtype)
+		else:
+			a = np.ascontiguousarray(a, dtype)
+			if a.shape != (h, w)+ch:
+				raise ValueError("map has the wrong shape")
+		setattr(dd, name, a)
+	return [getattr(dd, name).ctypes.data for name, _, _ in _MAPS]
+
+
+def _device_maps(dd: DepthData):
+	"""Allocate the missing output maps of dd as zeroed CUDA tensors on the images' device and check the given ones -> their
+	addresses."""
+	import torch
+	t0 = dd.images[0].image
+	h, w = t0.shape[:2]
+	for name, ch, dt in _MAPS:
+		a, shape, dtype = getattr(dd, name), (h, w)+ch, getattr(torch, dt)
+		if a is None:
+			a = torch.zeros(shape, dtype=dtype, device=t0.device)
+		elif not _is_torch(a) or tuple(a.shape) != shape or not a.is_contiguous() or a.dtype != dtype or a.device != t0.device:
+			raise ValueError("map must be a contiguous %s CUDA tensor of shape %s on the images' device" % (dtype, shape))
+		setattr(dd, name, a)
+	return [getattr(dd, name).data_ptr() for name, _, _ in _MAPS]
+
+
+class _Context:
+	"""One engine context (b200mvs_create ... b200mvs_destroy) and the calls made on it."""
+
+	def __init__(self, device: int):
 		self._lib = _lib.load()
 		self._ctx = C.c_void_p()
 		rc = self._lib.b200mvs_create(int(device), C.byref(self._ctx))
 		if rc != 0:
 			raise _lib.B200MVSError("b200mvs_create(device=%d) failed with status %d (no GPU => no fallback)" % (device, rc))
-		self.device = int(device)
-		self.bGeomConsistency = False
 		self.stats = _lib.Stats()
 
-	def Init(self, bGeomConsistency: bool = False):
-		"""PatchMatchCUDA::Init: select photometric (false) or geometric-consistency (true) passes."""
-		self.bGeomConsistency = bool(bGeomConsistency)
+	def _call(self, name: str, *args):
+		"""b200mvs_<name>(ctx, *args); a non-zero status raises B200MVSError with the context's last error."""
+		fn = "b200mvs_" + name
+		_lib.check(self._lib, self._ctx, getattr(self._lib, fn)(self._ctx, *args), fn)
 
 	def Release(self):
 		if self._ctx:
@@ -230,6 +253,30 @@ class PatchMatchB200:
 		except Exception:
 			pass
 
+	def SetDebug(self, **kw):
+		"""b200mvs_set_debug: diagnostic kernel switches, the fields of b200mvs_debug; no arguments = defaults.
+		PatchMatch: scalarTaps, noTMA, sweepFourCtas.  SGM: sgmAggregation (0 auto, 1 general, 2 register-pipelined uniform,
+		3 bulk-copy ring, 4 wave fronts), sgmCost, frontLayout / frontSerial / frontBlock / frontLag / frontCtas / frontDepth."""
+		d = _lib.Debug()
+		for k, v in kw.items():
+			if k == "reserved" or not hasattr(d, k):
+				raise AttributeError(k)
+			setattr(d, k, int(v))
+		self._call("set_debug", C.byref(d))
+
+
+class PatchMatchB200(_Context):
+	"""Drop-in for the reference's `PatchMatchCUDA` (libs/MVS/PatchMatchCUDA.inl:78-131)."""
+
+	def __init__(self, device: int = 0):
+		super().__init__(device)
+		self.device = int(device)
+		self.bGeomConsistency = False
+
+	def Init(self, bGeomConsistency: bool = False):
+		"""PatchMatchCUDA::Init: select photometric (false) or geometric-consistency (true) passes."""
+		self.bGeomConsistency = bool(bGeomConsistency)
+
 	def ToGray(self, image, bgr: bool = True):
 		"""TImage::toGray(out, COLOR_BGR2GRAY, bNormalize=true) (libs/Common/Types.inl:2377-2431) on the device: uint8 CUDA tensor
 		(H, W, 3|4), channel order B,G,R(,A) as cv::imread delivers (bgr=False: R,G,B) -> float32 gray (H, W) in [0, 1]."""
@@ -238,9 +285,7 @@ class PatchMatchB200:
 			raise ValueError("ToGray needs a contiguous uint8 CUDA tensor of shape (H, W, 3|4)")
 		h, w, ch = (int(v) for v in image.shape)
 		out = torch.empty((h, w), dtype=torch.float32, device=image.device)
-		rc = self._lib.b200mvs_to_gray_device(self._ctx, image.data_ptr(), w, h, w*ch, ch, int(bool(bgr)), out.data_ptr(), w*4,
-			C.c_void_p(_stream_handle(image.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_to_gray_device")
+		self._call("to_gray_device", image.data_ptr(), w, h, w*ch, ch, int(bool(bgr)), out.data_ptr(), w*4, _stream_handle(image.device))
 		return out
 
 	def ScaleImage(self, image, scale: float):
@@ -252,26 +297,14 @@ class PatchMatchB200:
 			raise ValueError("ScaleImage needs a 2-D float32 CUDA tensor with unit column stride")
 		h, w = (int(v) for v in image.shape)
 		dw, dh, ok = C.c_int(), C.c_int(), C.c_int()
-		self._lib.b200mvs_scaled_size(w, h, C.c_float(scale), C.byref(dw), C.byref(dh))
+		self._lib.b200mvs_scaled_size(w, h, scale, C.byref(dw), C.byref(dh))
 		out = torch.empty((max(dh.value, 1), max(dw.value, 1)), dtype=torch.float32, device=image.device)
-		rc = self._lib.b200mvs_scale_image_device(self._ctx, image.data_ptr(), w, h, image.stride(0)*4, C.c_float(scale), out.data_ptr(),
-			C.byref(ok), C.c_void_p(_stream_handle(image.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_scale_image_device")
+		self._call("scale_image_device", image.data_ptr(), w, h, image.stride(0)*4, scale, out.data_ptr(), C.byref(ok),
+			_stream_handle(image.device))
 		return out if ok.value else None
 
 	def _set_params(self):
-		p = OPTDENSE.snapshot()
-		_lib.check(self._lib, self._ctx, self._lib.b200mvs_set_params(self._ctx, C.byref(p)), "b200mvs_set_params")
-
-	def SetDebug(self, **kw):
-		"""b200mvs_set_debug: diagnostic kernel switches (the fields of b200mvs_debug: scalarTaps, noTMA, sweepFourCtas, ...);
-		no arguments = defaults."""
-		d = _lib.Debug()
-		for k, v in kw.items():
-			if k == "reserved" or not hasattr(d, k):
-				raise AttributeError(k)
-			setattr(d, k, int(v))
-		_lib.check(self._lib, self._ctx, self._lib.b200mvs_set_debug(self._ctx, C.byref(d)), "b200mvs_set_debug")
+		self._call("set_params", C.byref(OPTDENSE.snapshot()))
 
 	def SetIgnoreMask(self, mask=None):
 		"""Ignore-mask of the reference view for the following EstimateDepthMap calls (OPTDENSE::nIgnoreMaskLabel >= 0,
@@ -279,19 +312,18 @@ class PatchMatchB200:
 		(kept by reference until cleared); None clears it."""
 		self._mask_keep = None
 		if mask is None:
-			rc = self._lib.b200mvs_set_ignore_mask(self._ctx, None, 0, 0, 0, 0)
+			self._call("set_ignore_mask", None, 0, 0, 0, 0)
 		elif _is_torch(mask):
 			import torch
 			if mask.dtype != torch.uint8 or not mask.is_cuda or mask.dim() != 2 or mask.stride(1) != 1:
 				raise ValueError("device mask must be a 2-D uint8 CUDA tensor with unit column stride")
 			self._mask_keep = mask
-			rc = self._lib.b200mvs_set_ignore_mask(self._ctx, mask.data_ptr(), int(mask.shape[1]), int(mask.shape[0]), int(mask.stride(0)), 1)
+			self._call("set_ignore_mask", mask.data_ptr(), int(mask.shape[1]), int(mask.shape[0]), int(mask.stride(0)), 1)
 		else:
 			m = np.ascontiguousarray(mask, np.uint8)
 			if m.ndim != 2:
 				raise ValueError("mask must be 2-D")
-			rc = self._lib.b200mvs_set_ignore_mask(self._ctx, m.ctypes.data, m.shape[1], m.shape[0], m.strides[0], 0)
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_set_ignore_mask")
+			self._call("set_ignore_mask", m.ctypes.data, m.shape[1], m.shape[0], m.strides[0], 0)
 
 	def EstimateDepthMap(self, depthData: DepthData, nGeometricIter: Optional[int] = None, stream=None, sync: bool = True):
 		"""PatchMatchCUDA::EstimateDepthMap(DepthData&): estimate depthMap/normalMap/confMap/viewsMap
@@ -302,57 +334,23 @@ class PatchMatchB200:
 			nGeometricIter = 0 if self.bGeomConsistency else -1
 		self._set_params()
 		arr, keep, dev = _make_views(depthData.images)
-		h, w = depthData.images[0].image.shape[:2]
+		job = (arr, len(arr), depthData.dMin, depthData.dMax, int(nGeometricIter))
 		if dev:
-			import torch
-			t0 = depthData.images[0].image
-			def dmap(a, shape, dtype):
-				if a is None:
-					return torch.zeros(shape, dtype=dtype, device=t0.device)
-				if not _is_torch(a) or tuple(a.shape) != tuple(shape) or not a.is_contiguous() or a.dtype != dtype or a.device != t0.device:
-					raise ValueError("map must be a contiguous %s CUDA tensor of shape %s on the images' device" % (dtype, tuple(shape)))
-				return a
-			depthData.depthMap = dmap(depthData.depthMap, (h, w), torch.float32)
-			depthData.normalMap = dmap(depthData.normalMap, (h, w, 3), torch.float32)
-			depthData.confMap = dmap(depthData.confMap, (h, w), torch.float32)
-			depthData.viewsMap = dmap(depthData.viewsMap, (h, w, 4), torch.uint8)
+			maps = _device_maps(depthData)
 			if stream is None:
-				stream = _stream_handle(t0.device)
-			rc = self._lib.b200mvs_estimate_device(self._ctx, arr, len(arr), C.c_float(depthData.dMin), C.c_float(depthData.dMax),
-				int(nGeometricIter), depthData.depthMap.data_ptr(), depthData.normalMap.data_ptr(),
-				depthData.confMap.data_ptr(), depthData.viewsMap.data_ptr(), C.c_void_p(stream),
-				C.byref(self.stats) if sync else None)
-			_lib.check(self._lib, self._ctx, rc, "b200mvs_estimate_device")
+				stream = _stream_handle(depthData.images[0].image.device)
+			self._call("estimate_device", *job, *maps, stream, C.byref(self.stats) if sync else None)
+		elif sync:
+			self._call("estimate", *job, *_host_maps(depthData), C.byref(self.stats))
 		else:
-			def hmap(a, shape, dtype):
-				if a is None:
-					return np.zeros(shape, dtype)
-				a = np.ascontiguousarray(a, dtype)
-				if a.shape != tuple(shape):
-					raise ValueError("map has the wrong shape")
-				return a
-			depthData.depthMap = hmap(depthData.depthMap, (h, w), np.float32)
-			depthData.normalMap = hmap(depthData.normalMap, (h, w, 3), np.float32)
-			depthData.confMap = hmap(depthData.confMap, (h, w), np.float32)
-			depthData.viewsMap = hmap(depthData.viewsMap, (h, w, 4), np.uint8)
-			if sync:
-				rc = self._lib.b200mvs_estimate(self._ctx, arr, len(arr), C.c_float(depthData.dMin), C.c_float(depthData.dMax),
-					int(nGeometricIter), depthData.depthMap.ctypes.data, depthData.normalMap.ctypes.data,
-					depthData.confMap.ctypes.data, depthData.viewsMap.ctypes.data, C.byref(self.stats))
-				_lib.check(self._lib, self._ctx, rc, "b200mvs_estimate")
-			else:
-				# asynchronous host path: the caller keeps depthData alive and calls Wait() before reading the maps
-				rc = self._lib.b200mvs_estimate_async(self._ctx, arr, len(arr), C.c_float(depthData.dMin), C.c_float(depthData.dMax),
-					int(nGeometricIter), depthData.depthMap.ctypes.data, depthData.normalMap.ctypes.data,
-					depthData.confMap.ctypes.data, depthData.viewsMap.ctypes.data)
-				_lib.check(self._lib, self._ctx, rc, "b200mvs_estimate_async")
-				self._inflight = (depthData, keep)
+			# asynchronous host path: the caller keeps depthData alive and calls Wait() before reading the maps
+			self._call("estimate_async", *job, *_host_maps(depthData))
+			self._inflight = (depthData, keep)
 		return depthData
 
 	def Wait(self):
 		"""b200mvs_sync: wait for an EstimateDepthMap(..., sync=False) on host buffers and fetch its stats."""
-		rc = self._lib.b200mvs_sync(self._ctx, C.byref(self.stats))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sync")
+		self._call("sync", C.byref(self.stats))
 		self._inflight = None
 
 	# ---- building blocks on device tensors (used by the parity tests) -----------------------
@@ -364,26 +362,19 @@ class PatchMatchB200:
 
 	def ScoreDepthMap(self, images, dMin, dMax, plane4, cost, lowres=None):
 		"""pass A (ScoreDepthMapTmp) on a packed plane field (H, W, 4) = {nx,ny,nz,depth}."""
-		import torch
 		self._set_params()
 		arr, keep = self._dev_views(images)
-		s = _stream_handle(plane4.device)
-		rc = self._lib.b200mvs_pm_score(self._ctx, arr, len(arr), C.c_float(dMin), C.c_float(dMax),
-			lowres.data_ptr() if lowres is not None else None, plane4.data_ptr(), cost.data_ptr(), C.c_void_p(s))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_pm_score")
+		self._call("pm_score", arr, len(arr), dMin, dMax, lowres.data_ptr() if lowres is not None else None, plane4.data_ptr(),
+			cost.data_ptr(), _stream_handle(plane4.device))
 
 	def SweepDepthMap(self, images, dMin, dMax, plane4, cost, sweep, half=-1, nRandomIters=None, lowres=None):
 		"""pass B: one red-black sweep (both colours, or one if half in {0,1})."""
-		import torch
 		self._set_params()
 		arr, keep = self._dev_views(images)
 		if nRandomIters is None:
 			nRandomIters = OPTDENSE.schedule()[1]
-		s = _stream_handle(plane4.device)
-		rc = self._lib.b200mvs_pm_sweep(self._ctx, arr, len(arr), C.c_float(dMin), C.c_float(dMax),
-			lowres.data_ptr() if lowres is not None else None, int(sweep), int(half), int(nRandomIters),
-			plane4.data_ptr(), cost.data_ptr(), C.c_void_p(s))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_pm_sweep")
+		self._call("pm_sweep", arr, len(arr), dMin, dMax, lowres.data_ptr() if lowres is not None else None, int(sweep), int(half),
+			int(nRandomIters), plane4.data_ptr(), cost.data_ptr(), _stream_handle(plane4.device))
 
 
 def EstimateDepthMapsBatch(arrDepthData: List[DepthData], engines: List["PatchMatchB200"], nGeometricIter: int = -1):
@@ -398,14 +389,10 @@ def EstimateDepthMapsBatch(arrDepthData: List[DepthData], engines: List["PatchMa
 		arr, k, dev = _make_views(dd.images)
 		if dev:
 			raise ValueError("the batch call takes host buffers")
-		h, w = dd.images[0].image.shape[:2]
-		dd.depthMap = np.zeros((h, w), np.float32) if dd.depthMap is None else np.ascontiguousarray(dd.depthMap, np.float32)
-		dd.normalMap = np.zeros((h, w, 3), np.float32) if dd.normalMap is None else np.ascontiguousarray(dd.normalMap, np.float32)
-		dd.confMap = np.zeros((h, w), np.float32); dd.viewsMap = np.zeros((h, w, 4), np.uint8)
 		keep.append((arr, k))
 		J = jobs[j]
 		J.views = arr; J.nViews = len(arr); J.dMin = dd.dMin; J.dMax = dd.dMax; J.nGeometricIter = int(nGeometricIter)
-		J.depth = dd.depthMap.ctypes.data; J.normal = dd.normalMap.ctypes.data; J.conf = dd.confMap.ctypes.data; J.viewsMap = dd.viewsMap.ctypes.data
+		J.depth, J.normal, J.conf, J.viewsMap = _host_maps(dd)
 	ctxs = (C.c_void_p*len(engines))(*[e._ctx for e in engines])
 	rc = lib.b200mvs_estimate_batch(ctxs, len(engines), jobs, len(arrDepthData))
 	if rc != 0:
@@ -448,7 +435,7 @@ class DepthMapsData:
 		keep += [d, c]
 		o.depth = DepthMapsData._ptr(d); o.conf = DepthMapsData._ptr(c) if c is not None else None
 		o.height, o.width = int(d.shape[0]), int(d.shape[1])
-		o.K[:] = np.asarray(cam.K, np.float64).ravel(); o.R[:] = np.asarray(cam.R, np.float64).ravel(); o.C[:] = np.asarray(cam.C, np.float64).ravel()
+		_put_camera(o, cam)
 		return d
 
 	def FilterDepthMap(self, depthDataRef: DepthData, neighbors: List[DepthData], bAdjust: Optional[bool] = None, projected: bool = False):
@@ -456,7 +443,6 @@ class DepthMapsData:
 		`neighbors` are the DepthData of the (at most 8, SceneDensify.cpp:2152) neighbour views whose depth-maps are valid.
 		Returns (newDepthMap, newConfMap) — what the reference saves as filtered.dmap / filtered.cmap — or None when the map
 		can not be filtered; with projected=True also the N projected neighbour depth and confidence maps (device path)."""
-		lib, ctx = self.pmCUDA._lib, self.pmCUDA._ctx
 		bAdjust = OPTDENSE.bFilterAdjust if bAdjust is None else bool(bAdjust)
 		prm = _lib.FilterParams(min(OPTDENSE.nMinViewsFilter, self.nCalibratedImages-1),
 			min(OPTDENSE.nMinViewsFilterAdjust, self.nCalibratedImages-1), OPTDENSE.fDepthDiffThreshold, int(bAdjust))
@@ -474,48 +460,44 @@ class DepthMapsData:
 			if projected:
 				pd = torch.empty((max(len(neighbors), 1),)+tuple(dref.shape), dtype=torch.float32, device=dref.device)
 				pc = torch.zeros_like(pd)
-			rc = lib.b200mvs_filter_depth_map_device(ctx, C.byref(arr[0]), nbrs, len(neighbors), C.byref(prm), depthDataRef.dMin, depthDataRef.dMax,
-				od.data_ptr(), oc.data_ptr(), pd.data_ptr() if projected else None, pc.data_ptr() if projected and bAdjust else None,
-				C.byref(ok), C.c_void_p(_stream_handle(dref.device)))
-			_lib.check(lib, ctx, rc, "b200mvs_filter_depth_map_device")
+			self.pmCUDA._call("filter_depth_map_device", C.byref(arr[0]), nbrs, len(neighbors), C.byref(prm), depthDataRef.dMin,
+				depthDataRef.dMax, od.data_ptr(), oc.data_ptr(), pd.data_ptr() if projected else None,
+				pc.data_ptr() if projected and bAdjust else None, C.byref(ok), _stream_handle(dref.device))
 			if not ok.value:
 				return None
 			return (od, oc, pd, pc) if projected else (od, oc)
 		od = np.empty_like(dref); oc = np.empty_like(dref)
-		rc = lib.b200mvs_filter_depth_map(ctx, C.byref(arr[0]), nbrs, len(neighbors), C.byref(prm), depthDataRef.dMin, depthDataRef.dMax,
+		self.pmCUDA._call("filter_depth_map", C.byref(arr[0]), nbrs, len(neighbors), C.byref(prm), depthDataRef.dMin, depthDataRef.dMax,
 			od.ctypes.data, oc.ctypes.data, C.byref(ok), C.byref(self.stats))
-		_lib.check(lib, ctx, rc, "b200mvs_filter_depth_map")
 		return (od, oc) if ok.value else None
 
 	def _post(self, name: str, depthData: DepthData, arg: int) -> bool:
-		lib, ctx = self.pmCUDA._lib, self.pmCUDA._ctx
 		d, n, c = depthData.depthMap, depthData.normalMap, depthData.confMap
 		h, w = int(d.shape[0]), int(d.shape[1])
 		if _is_torch(d):
 			for a in (d, n, c):
 				if a is not None and not a.is_contiguous():
 					raise ValueError("maps must be contiguous")
-			rc = getattr(lib, name+"_device")(ctx, d.data_ptr(), n.data_ptr() if n is not None else None, c.data_ptr() if c is not None else None,
-				w, h, OPTDENSE.fDepthDiffThreshold, int(arg), C.c_void_p(_stream_handle(d.device)))
+			self.pmCUDA._call(name+"_device", d.data_ptr(), n.data_ptr() if n is not None else None, c.data_ptr() if c is not None else None,
+				w, h, OPTDENSE.fDepthDiffThreshold, int(arg), _stream_handle(d.device))
 		else:
 			for a in (d, n, c):
 				if a is not None and not (a.flags.c_contiguous and a.dtype == np.float32):
 					raise ValueError("maps must be contiguous float32 arrays (processed in place)")
-			rc = getattr(lib, name)(ctx, d.ctypes.data, n.ctypes.data if n is not None else None, c.ctypes.data if c is not None else None,
+			self.pmCUDA._call(name, d.ctypes.data, n.ctypes.data if n is not None else None, c.ctypes.data if c is not None else None,
 				w, h, OPTDENSE.fDepthDiffThreshold, int(arg), C.byref(self.stats))
-		_lib.check(lib, ctx, rc, name)
 		return True
 
 	def RemoveSmallSegments(self, depthData: DepthData) -> bool:
 		"""DepthMapsData::RemoveSmallSegments (SceneDensify.cpp:810-900), depthData's maps in place."""
-		return self._post("b200mvs_remove_small_segments", depthData, OPTDENSE.nSpeckleSize)
+		return self._post("remove_small_segments", depthData, OPTDENSE.nSpeckleSize)
 
 	def GapInterpolation(self, depthData: DepthData) -> bool:
 		"""DepthMapsData::GapInterpolation (SceneDensify.cpp:904-1045), depthData's maps in place."""
-		return self._post("b200mvs_gap_interpolation", depthData, OPTDENSE.nIpolGapSize)
+		return self._post("gap_interpolation", depthData, OPTDENSE.nIpolGapSize)
 
 
-class SemiGlobalMatcher:
+class SemiGlobalMatcher(_Context):
 	"""The pair matcher of the reference's STEREO::SemiGlobalMatcher
 	(libs/MVS/SemiGlobalMatcher.h:61-203): Match(left, right) -> (disparityMap, costMap) over the
 	valid region, with the ctor parameters P1, P2, P2alpha, P2beta (defaults 3, 4, 14, 38)."""
@@ -523,36 +505,13 @@ class SemiGlobalMatcher:
 	NO_ACCUMCOST = 65535
 
 	def __init__(self, P1: int = 3, P2: int = 4, P2alpha: float = 14.0, P2beta: float = 38.0, device: int = 0):
-		self._lib = _lib.load()
-		self._ctx = C.c_void_p()
-		rc = self._lib.b200mvs_create(int(device), C.byref(self._ctx))
-		if rc != 0:
-			raise _lib.B200MVSError("b200mvs_create(device=%d) failed with status %d (no GPU => no fallback)" % (device, rc))
+		super().__init__(device)
 		self.prm = _lib.SgmParams(int(P1), int(P2), float(P2alpha), float(P2beta))
-		self.stats = _lib.Stats()
 
 	def Release(self):
 		if getattr(self, "_peer", None) is not None:
 			self._peer.Release(); self._peer = None
-		if self._ctx:
-			self._lib.b200mvs_destroy(self._ctx)
-			self._ctx = C.c_void_p()
-
-	def __del__(self):
-		try:
-			self.Release()
-		except Exception:
-			pass
-
-	def SetDebug(self, **kw):
-		"""b200mvs_set_debug: sgmAggregation (0 auto, 1 general, 2 register-pipelined uniform, 3 bulk-copy ring, 4 wave fronts),
-		sgmCost, frontLayout / frontSerial / frontBlock / frontLag / frontCtas / frontDepth (b200mvs_debug); no arguments = defaults."""
-		d = _lib.Debug()
-		for k, v in kw.items():
-			if k == "reserved" or not hasattr(d, k):
-				raise AttributeError(k)
-			setattr(d, k, int(v))
-		_lib.check(self._lib, self._ctx, self._lib.b200mvs_set_debug(self._ctx, C.byref(d)), "b200mvs_set_debug")
+		super().Release()
 
 	def Match(self, leftGray, leftColor, rightGray, imagePixels, numCosts: int):
 		"""Host path: numpy images (gray float32 HxW, colour uint8 HxWx3 BGR) and the PixelMap
@@ -566,9 +525,8 @@ class SemiGlobalMatcher:
 		if px.itemsize != 16 or px.size != (w-6)*(h-6):
 			raise ValueError("PixelMap must hold (w-6)*(h-6) 16-byte records")
 		disp = np.zeros((h-6, w-6), np.int16); cost = np.zeros((h-6, w-6), np.uint16)
-		rc = self._lib.b200mvs_sgm_match(self._ctx, lg.ctypes.data, lc.ctypes.data, rg.ctypes.data, w, h, px.ctypes.data,
-			C.c_uint64(numCosts), C.byref(self.prm), disp.ctypes.data, cost.ctypes.data, C.byref(self.stats))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_match")
+		self._call("sgm_match", lg.ctypes.data, lc.ctypes.data, rg.ctypes.data, w, h, px.ctypes.data, numCosts, C.byref(self.prm),
+			disp.ctypes.data, cost.ctypes.data, C.byref(self.stats))
 		return disp, cost
 
 	def MatchDevice(self, leftGray, leftColor, rightGray, imagePixels, numCosts: int, stages: int = 7, costs=None, accums=None, sync: bool = True):
@@ -580,26 +538,22 @@ class SemiGlobalMatcher:
 		dev = leftGray.device
 		disp = torch.zeros((h-6, w-6), dtype=torch.int16, device=dev)
 		cost = torch.zeros((h-6, w-6), dtype=torch.int16, device=dev)
-		s = _stream_handle(dev)
-		rc = self._lib.b200mvs_sgm_match_device(self._ctx, leftGray.data_ptr(), leftColor.data_ptr(), rightGray.data_ptr(), w, h,
-			imagePixels.data_ptr(), C.c_uint64(numCosts), C.byref(self.prm), int(stages),
-			costs.data_ptr() if costs is not None else None, accums.data_ptr() if accums is not None else None,
-			disp.data_ptr(), cost.data_ptr(), C.c_void_p(s), C.byref(self.stats) if sync else None)
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_match_device")
+		self._call("sgm_match_device", leftGray.data_ptr(), leftColor.data_ptr(), rightGray.data_ptr(), w, h, imagePixels.data_ptr(),
+			numCosts, C.byref(self.prm), int(stages), costs.data_ptr() if costs is not None else None,
+			accums.data_ptr() if accums is not None else None, disp.data_ptr(), cost.data_ptr(), _stream_handle(dev),
+			C.byref(self.stats) if sync else None)
 		return disp, cost
 
 	def ConsistencyCrossCheck(self, l2r, r2l, thCross: int = 1):
 		"""SemiGlobalMatcher::ConsistencyCrossCheck on int16 CUDA tensors; l2r is modified in place."""
 		h, w = l2r.shape
-		rc = self._lib.b200mvs_sgm_cross_check_device(self._ctx, l2r.data_ptr(), r2l.data_ptr(), w, h, int(thCross), C.c_void_p(_stream_handle(l2r.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_cross_check_device")
+		self._call("sgm_cross_check_device", l2r.data_ptr(), r2l.data_ptr(), w, h, int(thCross), _stream_handle(l2r.device))
 		return l2r
 
 	def RefineDisparityMap(self, disparityMap, imagePixels, accums=None, subpixelSteps: int = 4):
 		"""SemiGlobalMatcher::RefineDisparityMap (LC-blend) on CUDA tensors; disparityMap in place."""
-		rc = self._lib.b200mvs_sgm_refine_device(self._ctx, imagePixels.data_ptr(), accums.data_ptr() if accums is not None else None,
-			disparityMap.data_ptr(), disparityMap.numel(), int(subpixelSteps), C.c_void_p(_stream_handle(disparityMap.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_refine_device")
+		self._call("sgm_refine_device", imagePixels.data_ptr(), accums.data_ptr() if accums is not None else None,
+			disparityMap.data_ptr(), disparityMap.numel(), int(subpixelSteps), _stream_handle(disparityMap.device))
 		return disparityMap
 
 	def MatchPairDevice(self, leftGray, leftColor, rightGray, rightColor, minDisp: int, maxDisp: int, thCross: int = 1, subpixelSteps: int = 4,
@@ -659,7 +613,7 @@ class SemiGlobalMatcher:
 		([(w, h), ...], (initWidth, initHeight)).  Host arithmetic, no GPU needed."""
 		lib = _lib.load()
 		n, iw, ih = C.c_int(), C.c_int(), C.c_int()
-		ws, hs = (C.c_int*9)(), (C.c_int*9)()
+		ws, hs = (C.c_int*_lib.SGM_MAX_LEVELS)(), (C.c_int*_lib.SGM_MAX_LEVELS)()
 		rc = lib.b200mvs_sgm_levels(int(width), int(height), int(minResolution), C.byref(n), ws, hs, C.byref(iw), C.byref(ih))
 		if rc != 0:
 			raise _lib.B200MVSError("b200mvs_sgm_levels(%d, %d, %d) failed with status %d" % (width, height, minResolution, rc))
@@ -685,10 +639,9 @@ class SemiGlobalMatcher:
 		cost = torch.empty((h-6, w-6), dtype=torch.int16, device=dev)
 		nums = (C.c_uint64*(2*len(sizes)))()
 		speckle = OPTDENSE.nSpeckleSize if nSpeckleSize is None else nSpeckleSize
-		rc = self._lib.b200mvs_sgm_match_hierarchical_device(self._ctx, leftGray.data_ptr(), leftColor.data_ptr(), rightGray.data_ptr(),
-			rightColor.data_ptr(), w, h, ptr(initDisparity), iw, ih, ptr(leftMask), ptr(rightMask), int(minResolution), int(speckle),
-			int(thCross), int(subpixelSteps), C.byref(self.prm), disp.data_ptr(), cost.data_ptr(), nums, C.c_void_p(_stream_handle(dev)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_match_hierarchical_device")
+		self._call("sgm_match_hierarchical_device", leftGray.data_ptr(), leftColor.data_ptr(), rightGray.data_ptr(), rightColor.data_ptr(),
+			w, h, ptr(initDisparity), iw, ih, ptr(leftMask), ptr(rightMask), int(minResolution), int(speckle), int(thCross),
+			int(subpixelSteps), C.byref(self.prm), disp.data_ptr(), cost.data_ptr(), nums, _stream_handle(dev))
 		levels = [{"size": sizes[k], "numCosts": (int(nums[2*k]), int(nums[2*k+1]))} for k in range(len(sizes))]
 		return disp, cost, levels
 
@@ -700,9 +653,8 @@ class SemiGlobalMatcher:
 		mh, mw = maskMap.shape
 		px = torch.empty((mh*mw, 16), dtype=torch.uint8, device=disparityMap.device)
 		num = C.c_uint64()
-		rc = self._lib.b200mvs_sgm_range_map_device(self._ctx, disparityMap.data_ptr(), w, h, maskMap.data_ptr(), mw, mh, int(minNumDisp),
-			int(minNumDispInvalid), px.data_ptr(), C.byref(num), C.c_void_p(_stream_handle(disparityMap.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_range_map_device")
+		self._call("sgm_range_map_device", disparityMap.data_ptr(), w, h, maskMap.data_ptr(), mw, mh, int(minNumDisp),
+			int(minNumDispInvalid), px.data_ptr(), C.byref(num), _stream_handle(disparityMap.device))
 		return px, int(num.value)
 
 	def FlipDirection(self, l2r):
@@ -710,8 +662,7 @@ class SemiGlobalMatcher:
 		import torch
 		h, w = l2r.shape
 		r2l = torch.empty_like(l2r)
-		rc = self._lib.b200mvs_sgm_flip_direction_device(self._ctx, l2r.data_ptr(), r2l.data_ptr(), w, h, C.c_void_p(_stream_handle(l2r.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_flip_direction_device")
+		self._call("sgm_flip_direction_device", l2r.data_ptr(), r2l.data_ptr(), w, h, _stream_handle(l2r.device))
 		return r2l
 
 	def UpscaleMask(self, maskMap, size2x):
@@ -719,26 +670,23 @@ class SemiGlobalMatcher:
 		import torch
 		h, w = maskMap.shape
 		out = torch.empty((int(size2x[1]), int(size2x[0])), dtype=torch.uint8, device=maskMap.device)
-		rc = self._lib.b200mvs_sgm_upscale_mask_device(self._ctx, maskMap.data_ptr(), w, h, out.data_ptr(), int(size2x[0]), int(size2x[1]),
-			C.c_void_p(_stream_handle(maskMap.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_upscale_mask_device")
+		self._call("sgm_upscale_mask_device", maskMap.data_ptr(), w, h, out.data_ptr(), int(size2x[0]), int(size2x[1]),
+			_stream_handle(maskMap.device))
 		return out
 
 	def ExtractMask(self, disparityMap, maskMap, thValid: int = 3):
 		"""maskMap (uint8, same size) in place"""
 		h, w = disparityMap.shape
-		rc = self._lib.b200mvs_sgm_extract_mask_device(self._ctx, disparityMap.data_ptr(), maskMap.data_ptr(), w, h, int(thValid),
-			C.c_void_p(_stream_handle(disparityMap.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_extract_mask_device")
+		self._call("sgm_extract_mask_device", disparityMap.data_ptr(), maskMap.data_ptr(), w, h, int(thValid),
+			_stream_handle(disparityMap.device))
 		return maskMap
 
 	def FilterSpeckles(self, disparityMap, newVal: int = NO_DISP, maxSpeckleSize: Optional[int] = None, maxDiff: int = 5):
 		"""cv::filterSpeckles on an int16 tensor, in place; maxSpeckleSize defaults to OPTDENSE.nSpeckleSize"""
 		h, w = disparityMap.shape
 		size = OPTDENSE.nSpeckleSize if maxSpeckleSize is None else maxSpeckleSize
-		rc = self._lib.b200mvs_sgm_filter_speckles_device(self._ctx, disparityMap.data_ptr(), w, h, int(newVal), int(size), int(maxDiff),
-			C.c_void_p(_stream_handle(disparityMap.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_filter_speckles_device")
+		self._call("sgm_filter_speckles_device", disparityMap.data_ptr(), w, h, int(newVal), int(size), int(maxDiff),
+			_stream_handle(disparityMap.device))
 		return disparityMap
 
 	def ResizeAreaU8(self, image, factor: int):
@@ -748,9 +696,7 @@ class SemiGlobalMatcher:
 		cn = 1 if image.dim() == 2 else image.shape[2]
 		dh, dw = int(np.rint(h/float(factor))), int(np.rint(w/float(factor)))
 		out = torch.empty((dh, dw) + tuple(image.shape[2:]), dtype=torch.uint8, device=image.device)
-		rc = self._lib.b200mvs_resize_area_u8_device(self._ctx, image.data_ptr(), w, h, int(cn), int(factor), out.data_ptr(),
-			C.c_void_p(_stream_handle(image.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_resize_area_u8_device")
+		self._call("resize_area_u8_device", image.data_ptr(), w, h, int(cn), int(factor), out.data_ptr(), _stream_handle(image.device))
 		return out
 
 	def LevelMask(self, mask, levelSize):
@@ -759,8 +705,7 @@ class SemiGlobalMatcher:
 		h, w = mask.shape
 		lw, lh = int(levelSize[0]), int(levelSize[1])
 		out = torch.empty((lh-6, lw-6), dtype=torch.uint8, device=mask.device)
-		rc = self._lib.b200mvs_sgm_level_mask_device(self._ctx, mask.data_ptr(), w, h, lw, lh, out.data_ptr(), C.c_void_p(_stream_handle(mask.device)))
-		_lib.check(self._lib, self._ctx, rc, "b200mvs_sgm_level_mask_device")
+		self._call("sgm_level_mask_device", mask.data_ptr(), w, h, lw, lh, out.data_ptr(), _stream_handle(mask.device))
 		return out
 
 

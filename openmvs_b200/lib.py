@@ -7,8 +7,8 @@ import os
 
 from . import build as _build
 
-MAX_VIEWS = 32
 ABI_VERSION = 6  # B200MVS_ABI_VERSION of include/b200mvs.h these structs mirror
+SGM_MAX_LEVELS = 9  # B200MVS_SGM_MAX_LEVELS: entries of the level-size arrays of b200mvs_sgm_levels
 
 
 class View(C.Structure):
@@ -86,27 +86,72 @@ class FuseParams(C.Structure):
 		("bEstimateColor", C.c_int), ("bEstimateNormal", C.c_int)]
 
 
-MAX_FILTER_VIEWS = 16
+I, U, F, P, U64 = C.c_int, C.c_uint, C.c_float, C.c_void_p, C.c_uint64
+IP, PP = C.POINTER(C.c_int), C.POINTER(C.c_void_p)
+PView, PStats, PSgmParams, PDMap = C.POINTER(View), C.POINTER(Stats), C.POINTER(SgmParams), C.POINTER(DMap)
 
-# every symbol include/b200mvs.h declares (checked by tests/test_capi_symbols.py)
-SYMBOLS = [
-	"b200mvs_create", "b200mvs_destroy", "b200mvs_default_params", "b200mvs_set_params", "b200mvs_last_error",
-	"b200mvs_set_debug", "b200mvs_get_schedule", "b200mvs_abi_version", "b200mvs_sizeof", "b200mvs_set_ignore_mask",
-	"b200mvs_device_count", "b200mvs_estimate", "b200mvs_estimate_device", "b200mvs_estimate_async", "b200mvs_sync", "b200mvs_estimate_batch",
-	"b200mvs_pm_pack", "b200mvs_pm_unpack", "b200mvs_pm_score", "b200mvs_pm_sweep", "b200mvs_pm_finalize",
-	"b200mvs_sgm_default_params", "b200mvs_sgm_match", "b200mvs_sgm_match_device",
-	"b200mvs_sgm_cross_check_device", "b200mvs_sgm_refine_device",
-	"b200mvs_sgm_levels", "b200mvs_sgm_match_hierarchical_device", "b200mvs_sgm_range_map_device", "b200mvs_sgm_flip_direction_device",
-	"b200mvs_sgm_upscale_mask_device", "b200mvs_sgm_extract_mask_device", "b200mvs_sgm_filter_speckles_device",
-	"b200mvs_resize_area_u8_device", "b200mvs_sgm_level_mask_device",
-	"b200mvs_filter_default_params", "b200mvs_filter_depth_map", "b200mvs_filter_depth_map_device",
-	"b200mvs_remove_small_segments", "b200mvs_remove_small_segments_device",
-	"b200mvs_gap_interpolation", "b200mvs_gap_interpolation_device",
-	"b200mvs_to_gray_device", "b200mvs_scaled_size", "b200mvs_scale_image_device",
-	"b200mvs_fuse_default_params", "b200mvs_fuse_depth_maps", "b200mvs_pointcloud_size", "b200mvs_pointcloud_depths",
-	"b200mvs_pointcloud_points", "b200mvs_pointcloud_normals", "b200mvs_pointcloud_colors", "b200mvs_pointcloud_view_offsets",
-	"b200mvs_pointcloud_views", "b200mvs_pointcloud_weights", "b200mvs_pointcloud_projs", "b200mvs_pointcloud_free",
-]
+# name -> (restype, argtypes) of every function include/b200mvs.h declares, in header order; contexts, device buffers and
+# streams are c_void_p (checked against the header's prototypes by tests/test_capi_symbols.py)
+PROTOTYPES = {
+	"b200mvs_create": (I, [I, PP]),
+	"b200mvs_destroy": (I, [P]),
+	"b200mvs_default_params": (None, [C.POINTER(Params)]),
+	"b200mvs_set_params": (I, [P, C.POINTER(Params)]),
+	"b200mvs_set_debug": (I, [P, C.POINTER(Debug)]),
+	"b200mvs_get_schedule": (I, [C.POINTER(Params), I, IP, IP]),
+	"b200mvs_abi_version": (I, []),
+	"b200mvs_sizeof": (C.c_size_t, [I]),
+	"b200mvs_set_ignore_mask": (I, [P, P, I, I, I, I]),
+	"b200mvs_last_error": (C.c_char_p, [P]),
+	"b200mvs_device_count": (I, []),
+	"b200mvs_estimate": (I, [P, PView, I, F, F, I, P, P, P, P, PStats]),
+	"b200mvs_estimate_async": (I, [P, PView, I, F, F, I, P, P, P, P]),
+	"b200mvs_sync": (I, [P, PStats]),
+	"b200mvs_estimate_batch": (I, [PP, I, C.POINTER(Job), I]),
+	"b200mvs_estimate_device": (I, [P, PView, I, F, F, I, P, P, P, P, P, PStats]),
+	"b200mvs_pm_pack": (I, [P, I, I, P, P, P, P]),
+	"b200mvs_pm_unpack": (I, [P, I, I, P, P, P, P]),
+	"b200mvs_pm_score": (I, [P, PView, I, F, F, P, P, P, P]),
+	"b200mvs_pm_sweep": (I, [P, PView, I, F, F, P, I, I, I, P, P, P]),
+	"b200mvs_pm_finalize": (I, [P, I, I, F, P, P, P, P, P, P]),
+	"b200mvs_sgm_default_params": (None, [PSgmParams]),
+	"b200mvs_sgm_match": (I, [P, P, P, P, I, I, P, U64, PSgmParams, P, P, PStats]),
+	"b200mvs_sgm_match_device": (I, [P, P, P, P, I, I, P, U64, PSgmParams, I, P, P, P, P, P, PStats]),
+	"b200mvs_sgm_cross_check_device": (I, [P, P, P, I, I, I, P]),
+	"b200mvs_sgm_refine_device": (I, [P, P, P, P, I, I, P]),
+	"b200mvs_sgm_levels": (I, [I, I, I, IP, IP, IP, IP, IP]),
+	"b200mvs_sgm_match_hierarchical_device": (I, [P, P, P, P, P, I, I, P, I, I, P, P, I, I, I, I, PSgmParams, P, P, P, P]),
+	"b200mvs_sgm_range_map_device": (I, [P, P, I, I, P, I, I, I, I, P, C.POINTER(U64), P]),
+	"b200mvs_sgm_flip_direction_device": (I, [P, P, P, I, I, P]),
+	"b200mvs_sgm_upscale_mask_device": (I, [P, P, I, I, P, I, I, P]),
+	"b200mvs_sgm_extract_mask_device": (I, [P, P, P, I, I, I, P]),
+	"b200mvs_sgm_filter_speckles_device": (I, [P, P, I, I, I, I, I, P]),
+	"b200mvs_resize_area_u8_device": (I, [P, P, I, I, I, I, P, P]),
+	"b200mvs_sgm_level_mask_device": (I, [P, P, I, I, I, I, P, P]),
+	"b200mvs_filter_default_params": (None, [C.POINTER(FilterParams)]),
+	"b200mvs_filter_depth_map": (I, [P, PDMap, PDMap, I, C.POINTER(FilterParams), F, F, P, P, IP, PStats]),
+	"b200mvs_filter_depth_map_device": (I, [P, PDMap, PDMap, I, C.POINTER(FilterParams), F, F, P, P, P, P, IP, P]),
+	"b200mvs_remove_small_segments": (I, [P, P, P, P, I, I, F, U, PStats]),
+	"b200mvs_remove_small_segments_device": (I, [P, P, P, P, I, I, F, U, P]),
+	"b200mvs_gap_interpolation": (I, [P, P, P, P, I, I, F, U, PStats]),
+	"b200mvs_gap_interpolation_device": (I, [P, P, P, P, I, I, F, U, P]),
+	"b200mvs_to_gray_device": (I, [P, P, I, I, I, I, I, P, I, P]),
+	"b200mvs_scaled_size": (I, [I, I, F, IP, IP]),
+	"b200mvs_scale_image_device": (I, [P, P, I, I, I, F, P, IP, P]),
+	"b200mvs_fuse_default_params": (None, [C.POINTER(FuseParams)]),
+	"b200mvs_fuse_depth_maps": (I, [C.POINTER(FuseView), I, C.POINTER(FuseParams), PP]),
+	"b200mvs_pointcloud_size": (U64, [P]),
+	"b200mvs_pointcloud_depths": (U64, [P]),
+	"b200mvs_pointcloud_points": (C.POINTER(F), [P]),
+	"b200mvs_pointcloud_normals": (C.POINTER(F), [P]),
+	"b200mvs_pointcloud_colors": (C.POINTER(C.c_uint8), [P]),
+	"b200mvs_pointcloud_view_offsets": (C.POINTER(C.c_uint32), [P]),
+	"b200mvs_pointcloud_views": (C.POINTER(C.c_uint32), [P]),
+	"b200mvs_pointcloud_weights": (C.POINTER(F), [P]),
+	"b200mvs_pointcloud_projs": (C.POINTER(C.c_uint16), [P]),
+	"b200mvs_pointcloud_free": (None, [P]),
+}
+SYMBOLS = list(PROTOTYPES)
 
 _LIB = None
 
@@ -126,69 +171,12 @@ def load(build_if_missing: bool = True):
 	if not hasattr(lib, "b200mvs_abi_version") or lib.b200mvs_abi_version() != ABI_VERSION:
 		raise RuntimeError("%s was built from another version of include/b200mvs.h (ABI %s, bindings %d): rebuild it" % (
 			path, lib.b200mvs_abi_version() if hasattr(lib, "b200mvs_abi_version") else "?", ABI_VERSION))
-	lib.b200mvs_sizeof.restype = C.c_size_t
-	lib.b200mvs_sizeof.argtypes = [C.c_int]
+	for name, (restype, argtypes) in PROTOTYPES.items():
+		f = getattr(lib, name)
+		f.restype, f.argtypes = restype, argtypes
 	for what, T in enumerate((View, Params, Stats, Job, SgmPixel, SgmParams, DMap, FilterParams, Debug)):
 		if lib.b200mvs_sizeof(what) != C.sizeof(T):
 			raise RuntimeError("struct %s: library %d bytes, bindings %d bytes" % (T.__name__, lib.b200mvs_sizeof(what), C.sizeof(T)))
-	lib.b200mvs_last_error.restype = C.c_char_p
-	lib.b200mvs_last_error.argtypes = [C.c_void_p]
-	lib.b200mvs_create.argtypes = [C.c_int, C.POINTER(C.c_void_p)]
-	lib.b200mvs_destroy.argtypes = [C.c_void_p]
-	lib.b200mvs_set_params.argtypes = [C.c_void_p, C.POINTER(Params)]
-	lib.b200mvs_default_params.argtypes = [C.POINTER(Params)]
-	lib.b200mvs_set_debug.argtypes = [C.c_void_p, C.POINTER(Debug)]
-	lib.b200mvs_get_schedule.argtypes = [C.POINTER(Params), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-	lib.b200mvs_set_ignore_mask.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
-	F = C.c_float
-	P = C.c_void_p
-	lib.b200mvs_estimate.argtypes = [P, C.POINTER(View), C.c_int, F, F, C.c_int, P, P, P, P, C.POINTER(Stats)]
-	lib.b200mvs_estimate_async.argtypes = [P, C.POINTER(View), C.c_int, F, F, C.c_int, P, P, P, P]
-	lib.b200mvs_sync.argtypes = [P, C.POINTER(Stats)]
-	lib.b200mvs_estimate_batch.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.POINTER(Job), C.c_int]
-	lib.b200mvs_estimate_device.argtypes = [P, C.POINTER(View), C.c_int, F, F, C.c_int, P, P, P, P, P, C.POINTER(Stats)]
-	lib.b200mvs_pm_pack.argtypes = [P, C.c_int, C.c_int, P, P, P, P]
-	lib.b200mvs_pm_unpack.argtypes = [P, C.c_int, C.c_int, P, P, P, P]
-	lib.b200mvs_pm_score.argtypes = [P, C.POINTER(View), C.c_int, F, F, P, P, P, P]
-	lib.b200mvs_pm_sweep.argtypes = [P, C.POINTER(View), C.c_int, F, F, P, C.c_int, C.c_int, C.c_int, P, P, P]
-	lib.b200mvs_pm_finalize.argtypes = [P, C.c_int, C.c_int, F, P, P, P, P, P, P]
-	lib.b200mvs_sgm_default_params.argtypes = [C.POINTER(SgmParams)]
-	lib.b200mvs_sgm_match.argtypes = [P, P, P, P, C.c_int, C.c_int, P, C.c_uint64, C.POINTER(SgmParams), P, P, C.POINTER(Stats)]
-	lib.b200mvs_sgm_match_device.argtypes = [P, P, P, P, C.c_int, C.c_int, P, C.c_uint64, C.POINTER(SgmParams), C.c_int, P, P, P, P, P, C.POINTER(Stats)]
-	lib.b200mvs_fuse_default_params.argtypes = [C.POINTER(FuseParams)]
-	lib.b200mvs_fuse_depth_maps.argtypes = [C.POINTER(FuseView), C.c_int, C.POINTER(FuseParams), C.POINTER(C.c_void_p)]
-	for name, rt in (("size", C.c_uint64), ("depths", C.c_uint64), ("points", C.POINTER(C.c_float)), ("normals", C.POINTER(C.c_float)),
-			("colors", C.POINTER(C.c_uint8)), ("view_offsets", C.POINTER(C.c_uint32)), ("views", C.POINTER(C.c_uint32)),
-			("weights", C.POINTER(C.c_float)), ("projs", C.POINTER(C.c_uint16))):
-		f = getattr(lib, "b200mvs_pointcloud_"+name)
-		f.restype = rt; f.argtypes = [C.c_void_p]
-	lib.b200mvs_pointcloud_free.argtypes = [C.c_void_p]
-	lib.b200mvs_pointcloud_free.restype = None
-	lib.b200mvs_sgm_cross_check_device.argtypes = [P, P, P, C.c_int, C.c_int, C.c_int, P]
-	lib.b200mvs_sgm_refine_device.argtypes = [P, P, P, P, C.c_int, C.c_int, P]
-	I = C.c_int
-	IP = C.POINTER(C.c_int)
-	lib.b200mvs_sgm_levels.argtypes = [I, I, I, IP, IP, IP, IP, IP]
-	lib.b200mvs_sgm_match_hierarchical_device.argtypes = [P, P, P, P, P, I, I, P, I, I, P, P, I, I, I, I, C.POINTER(SgmParams), P, P, P, P]
-	lib.b200mvs_sgm_range_map_device.argtypes = [P, P, I, I, P, I, I, I, I, P, C.POINTER(C.c_uint64), P]
-	lib.b200mvs_sgm_flip_direction_device.argtypes = [P, P, P, I, I, P]
-	lib.b200mvs_sgm_upscale_mask_device.argtypes = [P, P, I, I, P, I, I, P]
-	lib.b200mvs_sgm_extract_mask_device.argtypes = [P, P, P, I, I, I, P]
-	lib.b200mvs_sgm_filter_speckles_device.argtypes = [P, P, I, I, I, I, I, P]
-	lib.b200mvs_resize_area_u8_device.argtypes = [P, P, I, I, I, I, P, P]
-	lib.b200mvs_sgm_level_mask_device.argtypes = [P, P, I, I, I, I, P, P]
-	lib.b200mvs_filter_default_params.argtypes = [C.POINTER(FilterParams)]
-	lib.b200mvs_filter_depth_map.argtypes = [P, C.POINTER(DMap), C.POINTER(DMap), C.c_int, C.POINTER(FilterParams), F, F, P, P,
-		C.POINTER(C.c_int), C.POINTER(Stats)]
-	lib.b200mvs_filter_depth_map_device.argtypes = [P, C.POINTER(DMap), C.POINTER(DMap), C.c_int, C.POINTER(FilterParams), F, F, P, P, P, P,
-		C.POINTER(C.c_int), P]
-	lib.b200mvs_remove_small_segments.argtypes = [P, P, P, P, C.c_int, C.c_int, F, C.c_uint, C.POINTER(Stats)]
-	lib.b200mvs_remove_small_segments_device.argtypes = [P, P, P, P, C.c_int, C.c_int, F, C.c_uint, P]
-	lib.b200mvs_gap_interpolation.argtypes = [P, P, P, P, C.c_int, C.c_int, F, C.c_uint, C.POINTER(Stats)]
-	lib.b200mvs_gap_interpolation_device.argtypes = [P, P, P, P, C.c_int, C.c_int, F, C.c_uint, P]
-	lib.b200mvs_to_gray_device.argtypes = [P, P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, P, C.c_int, P]
-	lib.b200mvs_scaled_size.argtypes = [C.c_int, C.c_int, F, C.POINTER(C.c_int), C.POINTER(C.c_int)]
-	lib.b200mvs_scale_image_device.argtypes = [P, P, C.c_int, C.c_int, C.c_int, F, P, C.POINTER(C.c_int), P]
 	_LIB = lib
 	return lib
 

@@ -9,10 +9,21 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
+def _header():
+	"""include/b200mvs.h without comments"""
+	return re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "b200mvs.h")).read(), flags=re.S)
+
+
 def _declared():
-	src = open(os.path.join(ROOT, "include", "b200mvs.h")).read()
-	src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-	return sorted(set(re.findall(r"\b(b200mvs_[a-z_0-9]+)\s*\(", src)))
+	return sorted(set(re.findall(r"\b(b200mvs_[a-z_0-9]+)\s*\(", _header())))
+
+
+def _mirrors():
+	"""every struct of include/b200mvs.h -> its ctypes mirror in openmvs_b200/lib.py"""
+	from openmvs_b200 import lib
+	return {"b200mvs_view": lib.View, "b200mvs_params": lib.Params, "b200mvs_stats": lib.Stats, "b200mvs_job": lib.Job,
+		"b200mvs_sgm_params": lib.SgmParams, "b200mvs_dmap": lib.DMap, "b200mvs_filter_params": lib.FilterParams,
+		"b200mvs_debug": lib.Debug, "b200mvs_sgm_pixel": lib.SgmPixel, "b200mvs_fuse_view": lib.FuseView, "b200mvs_fuse_params": lib.FuseParams}
 
 
 def test_library_builds_and_exports_every_declared_symbol():
@@ -39,10 +50,7 @@ def test_struct_layouts_match_header_sizes():
 def test_struct_layouts_match_a_c_compiler(tmp_path):
 	"""sizeof / offsetof of every struct of include/b200mvs.h as gcc sees them == the ctypes mirrors in openmvs_b200/lib.py"""
 	import subprocess
-	from openmvs_b200 import lib
-	structs = {"b200mvs_view": lib.View, "b200mvs_params": lib.Params, "b200mvs_stats": lib.Stats, "b200mvs_job": lib.Job,
-		"b200mvs_sgm_params": lib.SgmParams, "b200mvs_dmap": lib.DMap, "b200mvs_filter_params": lib.FilterParams,
-		"b200mvs_debug": lib.Debug, "b200mvs_sgm_pixel": lib.SgmPixel, "b200mvs_fuse_view": lib.FuseView, "b200mvs_fuse_params": lib.FuseParams}
+	structs = _mirrors()
 	lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "b200mvs.h"', 'int main(void) {']
 	for cname, ct in structs.items():
 		lines.append('printf("%s %%zu\\n", sizeof(%s));' % (cname, cname))
@@ -59,6 +67,51 @@ def test_struct_layouts_match_a_c_compiler(tmp_path):
 		for fname, _ in ct._fields_:
 			assert int(got["%s.%s" % (cname, fname)]) == getattr(ct, fname).offset, (cname, fname)
 	assert int(got["b200mvs_sgm_pixel"]) == 16  # SemiGlobalMatcher::PixelData
+
+
+def test_binding_prototypes_match_the_header():
+	"""Every entry of lib.PROTOTYPES has the arity, argument types and return type of its prototype in include/b200mvs.h:
+	ctypes passes a wrongly declared argument as garbage without any error."""
+	from openmvs_b200 import lib
+	src = re.sub(r"^\s*#.*$", "", _header(), flags=re.M)
+	protos = re.findall(r"([\w\s*]+?)\b(b200mvs_\w+)\s*\(([^()]*)\)\s*;", src)
+	assert [name for _, name, _ in protos] == lib.SYMBOLS  # one entry per prototype, in header order
+	mirrors = _mirrors()
+	assert set(re.findall(r"}\s*(b200mvs_\w+)\s*;", src)) == set(mirrors)
+	scalars = {"int": C.c_int, "unsigned": C.c_uint, "float": C.c_float, "uint64_t": C.c_uint64, "size_t": C.c_size_t,
+		"uint8_t": C.c_uint8, "int16_t": C.c_int16, "uint16_t": C.c_uint16, "uint32_t": C.c_uint32}
+
+	def allowed(words):
+		"""ctypes types that pass the C type `words` (tokens without const and the parameter name) correctly"""
+		stars = words.count("*")
+		base, = [w for w in words if w != "*"]
+		if stars == 0:
+			return [None] if base == "void" else [scalars[base]]
+		if stars > 1:
+			return [C.POINTER(C.c_void_p)]
+		if base == "char":
+			return [C.c_char_p]
+		if base in mirrors:
+			return [C.POINTER(mirrors[base]), C.c_void_p]
+		return [C.c_void_p] + ([C.POINTER(scalars[base])] if base in scalars else [])
+
+	tokens = lambda decl: [w for w in decl.replace("*", " * ").split() if w != "const"]
+	for ret, name, params in protos:
+		restype, argtypes = lib.PROTOTYPES[name]
+		assert restype in allowed(tokens(ret)), (name, ret.strip())
+		params = [] if params.strip() == "void" else [tokens(p)[:-1] for p in params.split(",")]
+		assert len(argtypes) == len(params), name
+		for k, (words, t) in enumerate(zip(params, argtypes)):
+			assert t in allowed(words), (name, k, " ".join(words))
+
+
+def test_binding_constants_match_the_header():
+	from openmvs_b200 import lib
+	defines = dict(re.findall(r"^#define B200MVS_(\w+)\s+(\d+)", _header(), flags=re.M))
+	kept = [n for n in defines if hasattr(lib, n)]
+	assert {"ABI_VERSION", "SGM_MAX_LEVELS"} <= set(kept)
+	for n in kept:
+		assert getattr(lib, n) == int(defines[n]), n
 
 
 def test_create_without_gpu_fails_loudly():

@@ -549,6 +549,18 @@ def test_batch_call_over_two_contexts_equals_single_calls(env, small_scene):
 		assert np.array_equal(a.depthMap, b.depthMap) and np.array_equal(a.confMap, b.confMap) and np.array_equal(a.viewsMap, b.viewsMap)
 
 
+def test_batch_call_rejects_a_wrong_shaped_map(env, small_scene):
+	"""The engine reads and writes every output map of a job whole, at the reference image's size: the batch call checks the
+	given maps like the single call does, before anything reaches the library."""
+	e = env
+	from openmvs_b200.depth_estimator import EstimateDepthMapsBatch
+	sc, ref, views = small_scene
+	h, w = views[0].image.shape
+	dd = e.DepthData(_host_views(e, views), sc.dmin, sc.dmax, depthMap=np.zeros((h-1, w), np.float32))
+	with pytest.raises(ValueError):
+		EstimateDepthMapsBatch([dd], [e.pm])
+
+
 def test_scene_pipeline_with_geometric_passes(env, small_scene, tmp_path):
 	"""Pass 1 for every view, then geometric-consistency passes fed by the other views' depth-maps
 	(compute_depth_maps, the estimation part of Scene::ComputeDepthMaps) on one GPU; every estimated view is emitted as a
