@@ -88,15 +88,16 @@ typedef struct {
 	                                           refinement tries in it (0: always nRandomIters-derived tries) */
 } b200mvs_params;
 
-/* Diagnostic switches (all zero = the shipped kernels); replaces the environment variables of round 1. */
+/* Diagnostic switches (all zero = the shipped kernels); replaces the environment variables of round 1.  The PatchMatch kernels
+ * have none: reserved0..2 hold the places of three retired switches and are ignored. */
 typedef struct {
-	int scalarTaps;      /* reserved, ignored: sm_90a has no packed fp32 instructions, the bilinear taps are always evaluated one at a time */
-	int noTMA;           /* 1: the sweep kernel reads the reference patch with plain loads instead of the TMA-staged tile */
+	int reserved0;       /* ignored */
+	int reserved1;       /* ignored */
 	int sgmAggregation;  /* 0 auto; 1 general ragged kernel; 2 register-pipelined uniform kernel; 3 bulk-copy ring kernel (one launch
 	                        per direction); 4 front kernel (fused directions, auto default for uniform ranges) */
 	int sgmCost;         /* 0 auto (tensor-core kernel for dense volumes with one range of 64 / 128 / 192 / 256 disparities, SIMT otherwise);
 	                        1 SIMT cost kernel; 2 tensor-core (wgmma) cost kernel or an error */
-	int sweepFourCtas;   /* reserved, ignored: the sweep kernel has one instantiation (80 registers, 3 CTAs per SM, no spills) */
+	int reserved2;       /* ignored */
 	int frontLayout;     /* wave-front aggregation: 0 auto; 1 two tilted fronts +-(x+2y), four directions each; 2 four straight
 	                        fronts; 3 eight passes of one direction */
 	int frontSerial;     /* 1: one pass per launch into one sum volume (default: two passes share a launch, each with its own
@@ -117,7 +118,8 @@ typedef struct {
 	int levels;
 	double ms_sweep_kernels; /* summed device time of the red-black half-sweep launches (CUDA events) */
 	int sweep_launches;
-	int tma_active;          /* 1: the sweep kernels staged the reference tile with TMA (cp.async.bulk.tensor) */
+	int tma_active;          /* 1: the sweep kernels staged the reference tile with TMA (cp.async.bulk.tensor); always 1 after a
+	                            successful estimate call, which fails when the tile cannot be staged */
 } b200mvs_stats;
 
 /* ---- lifetime (PatchMatchCUDA ctor / Init / Release, PatchMatchCUDA.cpp:60-117) ---- */

@@ -63,7 +63,6 @@ struct b200mvs_ctx {
 	DevBuf maskBuf, maskLevel;                // staged host mask, mask of the current pyramid level
 	DevBuf refPad;                            // 16-byte aligned copy of a reference image whose pitch TMA cannot address
 	CUtensorMap tmapRef;                      // descriptor of the current level's reference image
-	bool tmapValid = false;
 	std::vector<cudaEvent_t> sweepEv;         // event pairs around the sweep launches (stats only)
 	int nSweepEv = 0; bool timeSweeps = false;
 	int launches = 0;

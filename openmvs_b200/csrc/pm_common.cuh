@@ -1,5 +1,6 @@
 // pm_common.cuh — shared definitions of the PatchMatch kernels (sm_90a) and their launch functions.
 #pragma once
+#include <cuda.h>   // CUtensorMap (type only; the encoder is fetched through cudaGetDriverEntryPoint)
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -32,7 +33,6 @@ struct PMParams {
 	int evalCap;                             // > 0: tries per pixel and sweep <= max(1, evalCap - propagation candidates tested)
 	int skipUnchanged;                       // 1: a direction whose candidates kept their plane is not re-tested (sign bit of cost)
 	int sweep, colour;
-	int tma;                                 // reference tile staged by TMA (tensor map passed beside the params)
 	uint32_t seed;
 	const float* lowres;                     // low-resolution depth prior or null
 	const uint8_t* mask; int maskPitch;      // ignore-mask of this level (0 = skip the pixel) or null; pitch in bytes
@@ -56,7 +56,7 @@ __device__ __forceinline__ float u32_to_unit(uint32_t u) { return (float)u*(1.0f
 // launch functions (pm_kernels.cu)
 cudaError_t pm_configure_device();
 cudaError_t pm_launch_score(const PMParams& P, bool geom, cudaStream_t s);
-cudaError_t pm_launch_sweep(const PMParams& P, const void* tmapRef, bool geom, cudaStream_t s);
+cudaError_t pm_launch_sweep(const PMParams& P, const CUtensorMap& tmapRef, bool geom, cudaStream_t s);
 void pm_tma_box(int* w, int* h);
 cudaError_t pm_launch_finalize(int n, float keep, const float4* plane, const float* cost, const uint32_t* bestViews,
 	float* depth, float* normal, float* conf, uint32_t* viewsMap, cudaStream_t s);

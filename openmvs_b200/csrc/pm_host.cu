@@ -135,14 +135,70 @@ int check_estimate(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, floa
 	return B200MVS_OK;
 }
 
-void to_dview(const b200mvs_view& s, const float* img, int pitch, const float* dmap, int dpitch, DView& d) {
-	d.img = img; d.w = s.width; d.h = s.height; d.pitch = pitch;
-	memcpy(d.K, s.K, sizeof(d.K)); memcpy(d.R, s.R, sizeof(d.R)); memcpy(d.C, s.C, sizeof(d.C));
-	d.dmap = dmap; d.dw = s.dwidth; d.dh = s.dheight; d.dpitch = dpitch;
-	memcpy(d.Kd, s.Kd, sizeof(d.Kd)); memcpy(d.Rd, s.Rd, sizeof(d.Rd)); memcpy(d.Cd, s.Cd, sizeof(d.Cd));
+// One image of a caller's view as it lies in memory: `rows` rows of `row` bytes, `pitch` bytes apart (stride 0: packed rows)
+struct Rows { const void* p; size_t row, pitch; int rows; size_t extent() const { return pitch*rows; } };
+Rows rows_of(const void* p, size_t row, int stride, int rows) { return {p, row, stride ? (size_t)stride : row, rows}; }
+// the float gray image, or else the 8-bit colour image
+Rows image_rows(const b200mvs_view& v) {
+	return v.image ? rows_of(v.image, (size_t)v.width*sizeof(float), v.stride_bytes, v.height)
+	               : rows_of(v.image8, (size_t)v.width*v.channels8, v.stride8_bytes, v.height);
+}
+Rows depth_rows(const b200mvs_view& v) { return rows_of(v.depth, (size_t)v.dwidth*sizeof(float), v.dstride_bytes, v.dheight); }
+
+enum class Residency { Host, Device };
+
+// The engine's views of the caller's: device float images and depth-maps with their pitch in floats.  Host views are
+// uploaded packed into the context's scratch on stream s (h2d: the bytes copied); an 8-bit colour image is converted to
+// gray on the device (toGray) in either residency; device float images and depth-maps are used in place.
+int stage_views(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, Residency res, cudaStream_t s,
+	std::vector<DView>& dv, uint64_t& h2d)
+{
+	const bool host = res == Residency::Host;
+	auto upload = [&](DevBuf& b, const Rows& r) {
+		cudaError_t e = b.reserve(r.row*r.rows);
+		if (e == cudaSuccess) e = cudaMemcpy2DAsync(b.p, r.row, r.p, r.pitch, r.row, r.rows, cudaMemcpyHostToDevice, s);
+		if (e == cudaSuccess) h2d += r.row*r.rows;
+		return e;
+	};
+	if ((int)ctx->imgs.size() < nViews) { ctx->imgs.resize(nViews); ctx->dmaps.resize(nViews); ctx->img8.resize(nViews); }
+	dv.resize(nViews);
+	h2d = 0;
+	for (int i = 0; i < nViews; ++i) {
+		const b200mvs_view& v = views[i];
+		const Rows im = image_rows(v), dm = depth_rows(v);
+		DView& d = dv[i];
+		d.w = v.width; d.h = v.height; d.dw = v.dwidth; d.dh = v.dheight;
+		memcpy(d.K, v.K, sizeof(d.K)); memcpy(d.R, v.R, sizeof(d.R)); memcpy(d.C, v.C, sizeof(d.C));
+		memcpy(d.Kd, v.Kd, sizeof(d.Kd)); memcpy(d.Rd, v.Rd, sizeof(d.Rd)); memcpy(d.Cd, v.Cd, sizeof(d.Cd));
+		if (v.image && !host) {
+			d.img = v.image; d.pitch = (int)(im.pitch/sizeof(float));
+		} else {
+			CK(ctx->imgs[i].reserve((size_t)v.width*v.height*sizeof(float)));
+			d.img = ctx->imgs[i].as<float>(); d.pitch = v.width;
+			const void* src = im.p; size_t pitch = im.pitch;
+			if (host) {
+				DevBuf& b = v.image ? ctx->imgs[i] : ctx->img8[i];
+				CK(upload(b, im));
+				src = b.p; pitch = im.row;
+			}
+			if (!v.image) {
+				CK(rs_launch_to_gray((const uint8_t*)src, v.width, v.height, (int)pitch, v.channels8, v.bgr8 != 0, ctx->imgs[i].as<float>(),
+					v.width, s)); ++ctx->launches;
+			}
+		}
+		d.dmap = v.depth; d.dpitch = (int)(dm.pitch/sizeof(float));
+		if (v.depth && host) {
+			CK(upload(ctx->dmaps[i], dm));
+			d.dmap = ctx->dmaps[i].as<float>(); d.dpitch = v.dwidth;
+		}
+	}
+	return B200MVS_OK;
 }
 
 inline int cvRoundI(double v) { return (int)std::nearbyint(v); }
+
+// width or height n of an image at pyramid level sc (ScaleDepthData, SceneDensify.cpp:578-601: cvRound of the scaled size)
+int level_size(int n, int sc) { return cvRoundI(n*(1.0/(double)(1<<sc))); }
 
 // The engine's red-black schedule for nEstimationIters reference iterations (DESIGN.md §2): nSweeps red-black sweeps with nR
 // refinement tries each.  nSweepsPerIter > 0 pins it (nSweeps = nSweepsPerIter x iterations, nR = ceil(nRandomIters /
@@ -175,12 +231,13 @@ EncodeTiledFn encode_tiled_fn() {
 }
 
 // TMA descriptor of the reference image of one level: 2-D float tensor {W, H}, box = the tile a CTA
-// of the sweep kernel stages (72 x 16).  TMA needs a 16-byte aligned base and row pitch; an image that
-// does not satisfy this (odd width, cv::Mat ROI) is first copied to an aligned scratch image.
+// of the sweep kernel stages (72 x 16; the box may exceed the image, TMA zero-fills the outside).  TMA needs a
+// 16-byte aligned base and row pitch; an image that does not satisfy this (odd width, cv::Mat ROI) is first
+// copied to an aligned scratch image.  The sweep kernel has no other way to read the reference patch, so a
+// missing encoder or a refused descriptor fails the call.
 int prepare_ref_tmap(b200mvs_ctx* ctx, const DView& ref, cudaStream_t s) {
-	ctx->tmapValid = false;
-	EncodeTiledFn enc = ctx->dbg.noTMA ? nullptr : encode_tiled_fn();
-	if (!enc) return B200MVS_OK;
+	EncodeTiledFn enc = encode_tiled_fn();
+	if (!enc) return fail(ctx, B200MVS_ERR_CUDA, "cuTensorMapEncodeTiled: the driver does not provide the entry point");
 	const float* base = ref.img; size_t pitchB = (size_t)ref.pitch*4;
 	if (((uintptr_t)base & 15) || (pitchB & 15)) {
 		pitchB = (((size_t)ref.w*4)+15)&~(size_t)15;
@@ -195,7 +252,8 @@ int prepare_ref_tmap(b200mvs_ctx* ctx, const DView& ref, cudaStream_t s) {
 	const cuuint32_t estr[2] = {1, 1};
 	const CUresult r = enc(&ctx->tmapRef, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)base, dims, strides, box, estr,
 		CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-	ctx->tmapValid = (r == CUDA_SUCCESS);
+	if (r != CUDA_SUCCESS)
+		return fail(ctx, B200MVS_ERR_CUDA, ("cuTensorMapEncodeTiled failed for the reference image (CUresult " + std::to_string((int)r) + ")").c_str());
 	return B200MVS_OK;
 }
 
@@ -206,7 +264,7 @@ int launch_sweep_timed(b200mvs_ctx* ctx, const PMParams& P, bool geom, cudaStrea
 		}
 		CK(cudaEventRecord(ctx->sweepEv[2*ctx->nSweepEv], s));
 	}
-	CK(pm_launch_sweep(P, ctx->tmapValid ? &ctx->tmapRef : nullptr, geom, s)); ++ctx->launches;
+	CK(pm_launch_sweep(P, ctx->tmapRef, geom, s)); ++ctx->launches;
 	if (ctx->timeSweeps) {
 		CK(cudaEventRecord(ctx->sweepEv[2*ctx->nSweepEv+1], s));
 		++ctx->nSweepEv;
@@ -240,10 +298,8 @@ int estimate_on_device(b200mvs_ctx* ctx, const DView* views, int nViews, float d
 		if (ctx->mask) CK(ctx->maskLevel.reserve((size_t)(W/2+2)*(H/2+2)));
 		if ((int)ctx->pyr.size() < nViews) ctx->pyr.resize(nViews);
 		// level 1 is the largest pyramid level: size the buffers once, so that no level re-allocates mid-stream
-		for (int i = 0; i < nViews; ++i) {
-			const size_t dw = (size_t)cvRoundI(views[i].w*0.5), dh = (size_t)cvRoundI(views[i].h*0.5);
-			CK(ctx->pyr[i].reserve(dw*dh*sizeof(float)*(views[i].dmap ? 2 : 1)));
-		}
+		for (int i = 0; i < nViews; ++i)
+			CK(ctx->pyr[i].reserve((size_t)level_size(views[i].w, 1)*level_size(views[i].h, 1)*sizeof(float)*(views[i].dmap ? 2 : 1)));
 	}
 	float4* plane = ctx->plane.as<float4>();
 	float* cost = ctx->cost.as<float>();
@@ -253,15 +309,13 @@ int estimate_on_device(b200mvs_ctx* ctx, const DView* views, int nViews, float d
 		// ScaleDepthData (SceneDensify.cpp:578-601): INTER_AREA images, rescaled K
 		std::vector<DView> lv(views, views+nViews);
 		if (sc > 0) {
-			const double scale = 1.0/(double)(1<<sc);
+			const double inv = (double)(1<<sc);
 			for (int i = 0; i < nViews; ++i) {
-				const int dw = cvRoundI(views[i].w*scale), dh = cvRoundI(views[i].h*scale);
+				const int dw = level_size(views[i].w, sc), dh = level_size(views[i].h, sc);
 				if (dw < 2*PM_HALF+2 || dh < 2*PM_HALF+2)
 					return fail(ctx, B200MVS_ERR_ARG, "image too small for nSubResolutionLevels");
-				const size_t need = (size_t)dw*dh*sizeof(float)*(views[i].dmap ? 2 : 1);
-				CK(ctx->pyr[i].reserve(need));
-				float* im = ctx->pyr[i].as<float>();
-				CK(rs_launch_area(views[i].img, views[i].w, views[i].h, views[i].pitch, im, dw, dh, 1.0/scale, 1.0/scale, s)); ++ctx->launches;
+				float* im = ctx->pyr[i].as<float>();   // sized for level 1 above, the largest
+				CK(rs_launch_area(views[i].img, views[i].w, views[i].h, views[i].pitch, im, dw, dh, inv, inv, s)); ++ctx->launches;
 				lv[i].img = im; lv[i].w = dw; lv[i].h = dh; lv[i].pitch = dw;
 				scaleK(views[i].K, views[i].w, views[i].h, dw, dh, lv[i].K);
 				if (views[i].dmap) {
@@ -294,7 +348,6 @@ int estimate_on_device(b200mvs_ctx* ctx, const DView* views, int nViews, float d
 		build_params(o, lv.data(), nViews, dMin, dMax, lowres, plane, cost, best, P, geom);
 		P.nRandomIters = nR;
 		P.skipUnchanged = o.bSkipUnchanged ? 1 : 0;
-		P.tma = ctx->tmapValid ? 1 : 0;
 		if (ctx->mask) {
 			// the mask of this level: cv::resize(..., INTER_NEAREST) of the full-resolution mask (DepthMap.cpp:309)
 			if (sc > 0) {
@@ -328,7 +381,7 @@ int pm_stats(b200mvs_ctx* ctx, b200mvs_stats* stats, std::chrono::steady_clock::
 	if (rc) return rc;
 	for (int k = 0; k < ctx->nSweepEv; ++k) { float t = 0; CK(cudaEventElapsedTime(&t, ctx->sweepEv[2*k], ctx->sweepEv[2*k+1])); stats->ms_sweep_kernels += t; }
 	stats->sweep_launches = ctx->nSweepEv;
-	stats->tma_active = ctx->tmapValid ? 1 : 0;
+	stats->tma_active = 1;   // every sweep stages its reference tile by TMA (the call fails without a descriptor)
 	return B200MVS_OK;
 }
 
@@ -361,20 +414,11 @@ int b200mvs_estimate_device(b200mvs_ctx* ctx, const b200mvs_view* views, int nVi
 	if (rc) return rc;
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t s = stream_of(ctx, stream);
-	std::vector<DView> dv(nViews);
+	std::vector<DView> dv;
+	uint64_t h2d;
 	ctx->launches = 0;
-	for (int i = 0; i < nViews; ++i) {
-		const float* img = views[i].image; int pitch = views[i].stride_bytes ? views[i].stride_bytes/4 : views[i].width;
-		if (!img) {
-			// 8-bit colour image resident in HBM: toGray into the context's scratch
-			if ((int)ctx->imgs.size() < nViews) { ctx->imgs.resize(nViews); ctx->dmaps.resize(nViews); ctx->img8.resize(nViews); }
-			CK(ctx->imgs[i].reserve((size_t)views[i].width*views[i].height*sizeof(float)));
-			CK(rs_launch_to_gray(views[i].image8, views[i].width, views[i].height, views[i].stride8_bytes ? views[i].stride8_bytes : views[i].width*views[i].channels8,
-				views[i].channels8, views[i].bgr8 != 0, ctx->imgs[i].as<float>(), views[i].width, s)); ++ctx->launches;
-			img = ctx->imgs[i].as<float>(); pitch = views[i].width;
-		}
-		to_dview(views[i], img, pitch, views[i].depth, views[i].dstride_bytes ? views[i].dstride_bytes/4 : views[i].dwidth, dv[i]);
-	}
+	rc = stage_views(ctx, views, nViews, Residency::Device, s, dv, h2d);
+	if (rc) return rc;
 	const auto t0 = std::chrono::steady_clock::now();
 	ctx->nSweepEv = 0; ctx->timeSweeps = stats != nullptr;
 	if (stats) CK(cudaEventRecord(ctx->ev0, s));
@@ -396,35 +440,11 @@ int b200mvs_estimate_async(b200mvs_ctx* ctx, const b200mvs_view* views, int nVie
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t s = ctx->stream;
 	ctx->t0 = std::chrono::steady_clock::now();
-	if ((int)ctx->imgs.size() < nViews) { ctx->imgs.resize(nViews); ctx->dmaps.resize(nViews); ctx->img8.resize(nViews); }
-	std::vector<DView> dv(nViews);
-	uint64_t h2d = 0, d2h = 0;
+	std::vector<DView> dv;
+	uint64_t h2d, d2h = 0;
 	ctx->launches = 0;
-	for (int i = 0; i < nViews; ++i) {
-		const b200mvs_view& v = views[i];
-		const size_t row = (size_t)v.width*sizeof(float);
-		CK(ctx->imgs[i].reserve(row*v.height));
-		if (v.image) {
-			CK(cudaMemcpy2DAsync(ctx->imgs[i].p, row, v.image, v.stride_bytes ? v.stride_bytes : row, row, v.height, cudaMemcpyHostToDevice, s));
-			h2d += row*v.height;
-		} else {
-			// 8-bit colour image: upload channels8 bytes per pixel, convert on the device (toGray)
-			const size_t row8 = (size_t)v.width*v.channels8;
-			CK(ctx->img8[i].reserve(row8*v.height));
-			CK(cudaMemcpy2DAsync(ctx->img8[i].p, row8, v.image8, v.stride8_bytes ? v.stride8_bytes : row8, row8, v.height, cudaMemcpyHostToDevice, s));
-			h2d += row8*v.height;
-			CK(rs_launch_to_gray(ctx->img8[i].as<uint8_t>(), v.width, v.height, (int)row8, v.channels8, v.bgr8 != 0, ctx->imgs[i].as<float>(), v.width, s)); ++ctx->launches;
-		}
-		const float* dm = nullptr;
-		if (v.depth) {
-			const size_t drow = (size_t)v.dwidth*sizeof(float);
-			CK(ctx->dmaps[i].reserve(drow*v.dheight));
-			CK(cudaMemcpy2DAsync(ctx->dmaps[i].p, drow, v.depth, v.dstride_bytes ? v.dstride_bytes : drow, drow, v.dheight, cudaMemcpyHostToDevice, s));
-			h2d += drow*v.dheight;
-			dm = ctx->dmaps[i].as<float>();
-		}
-		to_dview(v, ctx->imgs[i].as<float>(), v.width, dm, v.dwidth, dv[i]);
-	}
+	rc = stage_views(ctx, views, nViews, Residency::Host, s, dv, h2d);
+	if (rc) return rc;
 	const size_t P0 = (size_t)views[0].width*views[0].height;
 	DevBuf& dD = ctx->mapD; DevBuf& dN = ctx->mapN;
 	CK(dD.reserve(P0*sizeof(float))); CK(dN.reserve(P0*3*sizeof(float)));
@@ -479,10 +499,9 @@ int b200mvs_estimate_batch(b200mvs_ctx** ctxs, int nCtx, b200mvs_job* jobs, int 
 		const b200mvs_job& J = jobs[j];
 		if (!J.views || J.nViews <= 0) continue;
 		for (int i = 0; i < J.nViews; ++i) {
-			const b200mvs_view& v = J.views[i];
-			if (v.image) pin.add(v.image, (size_t)(v.stride_bytes ? v.stride_bytes : v.width*4)*v.height);
-			else if (v.image8) pin.add(v.image8, (size_t)(v.stride8_bytes ? v.stride8_bytes : v.width*v.channels8)*v.height);
-			if (v.depth) pin.add(v.depth, (size_t)(v.dstride_bytes ? v.dstride_bytes : v.dwidth*4)*v.dheight);
+			const Rows im = image_rows(J.views[i]), dm = depth_rows(J.views[i]);
+			pin.add(im.p, im.extent());
+			pin.add(dm.p, dm.extent());
 		}
 		const size_t P0 = (size_t)J.views[0].width*J.views[0].height;
 		pin.add(J.depth, P0*4); pin.add(J.normal, P0*12); pin.add(J.conf, P0*4); pin.add(J.viewsMap, P0*4);
@@ -521,21 +540,21 @@ int b200mvs_pm_unpack(b200mvs_ctx* ctx, int width, int height, const float* plan
 	CK(pm_launch_unpack(width*height, (const float4*)plane4, depth, normal, stream_of(ctx, stream)));
 	return B200MVS_OK;
 }
+// tmap: also encode the reference image's TMA descriptor (the sweep needs it, the score kernel does not)
 static int block_params(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, float dMin, float dMax, const float* lowres,
-	float* plane4, float* cost, cudaStream_t s, PMParams& P, bool& geom)
+	float* plane4, float* cost, bool tmap, cudaStream_t s, PMParams& P, bool& geom)
 {
 	int rc = check_views(ctx, views, nViews);
 	if (rc) return rc;
 	if (!plane4 || !cost) return fail(ctx, B200MVS_ERR_ARG, "null state pointer");
 	for (int i = 0; i < nViews; ++i)
 		if (!views[i].image) return fail(ctx, B200MVS_ERR_ARG, "the building blocks take float gray images");
-	std::vector<DView> dv(nViews);
-	for (int i = 0; i < nViews; ++i)
-		to_dview(views[i], views[i].image, views[i].stride_bytes ? views[i].stride_bytes/4 : views[i].width,
-			views[i].depth, views[i].dstride_bytes ? views[i].dstride_bytes/4 : views[i].dwidth, dv[i]);
-	{ const int rc2 = prepare_ref_tmap(ctx, dv[0], s); if (rc2) return rc2; }
+	std::vector<DView> dv;
+	uint64_t h2d;
+	rc = stage_views(ctx, views, nViews, Residency::Device, s, dv, h2d);
+	if (rc) return rc;
+	if (tmap) { rc = prepare_ref_tmap(ctx, dv[0], s); if (rc) return rc; }
 	build_params(ctx->prm, dv.data(), nViews, dMin, dMax, lowres, (float4*)plane4, cost, nullptr, P, geom);
-	P.tma = ctx->tmapValid ? 1 : 0;
 	return B200MVS_OK;
 }
 int b200mvs_pm_score(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, float dMin, float dMax,
@@ -545,7 +564,7 @@ int b200mvs_pm_score(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, fl
 	if (!ctx) return B200MVS_ERR_ARG;
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t s = stream_of(ctx, stream);
-	int rc = block_params(ctx, views, nViews, dMin, dMax, lowres, plane4, cost, s, P, geom);
+	int rc = block_params(ctx, views, nViews, dMin, dMax, lowres, plane4, cost, false, s, P, geom);
 	if (rc) return rc;
 	CK(pm_launch_score(P, geom, s));
 	return B200MVS_OK;
@@ -557,13 +576,13 @@ int b200mvs_pm_sweep(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, fl
 	if (!ctx) return B200MVS_ERR_ARG;
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t s = stream_of(ctx, stream);
-	int rc = block_params(ctx, views, nViews, dMin, dMax, lowres, plane4, cost, s, P, geom);
+	int rc = block_params(ctx, views, nViews, dMin, dMax, lowres, plane4, cost, true, s, P, geom);
 	if (rc) return rc;
 	P.sweep = sweep; P.nRandomIters = nRandomIters;
 	for (int colour = 0; colour < 2; ++colour) {
 		if (half >= 0 && half != colour) continue;
 		P.colour = colour;
-		CK(pm_launch_sweep(P, ctx->tmapValid ? &ctx->tmapRef : nullptr, geom, s));
+		CK(pm_launch_sweep(P, ctx->tmapRef, geom, s));
 	}
 	return B200MVS_OK;
 }

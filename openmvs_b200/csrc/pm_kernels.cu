@@ -16,8 +16,6 @@
 // Measured design history and the variants that were dropped: DESIGN.md section 5.1.
 #include "pm_common.cuh"
 #include <math_constants.h>
-#include <cstring>
-#include <cuda.h>   // CUtensorMap (type only; the encoder is fetched through cudaGetDriverEntryPoint)
 
 namespace {
 
@@ -67,13 +65,25 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
 		:: "r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
 }
 
-// FillPixelPatch + GetWeight from the staged tile; (lx, ly) = pixel position inside the tile.
-// The tile shares its shared memory with the weights (pm_sweep_kernel), so every thread of the CTA calls this, and
-// the weights are written only after all threads have read their patch.
-__device__ __forceinline__ void fill_patch_tile(const float* tile, int lx, int ly, PatchW& p) {
+// The reference texel at offset (dx, dy) from the pixel: from the image in global memory (pass A) or from the staged tile
+// (pass B; (lx, ly) = pixel position inside the tile)
+struct ImageTexels {
+	const float* __restrict__ img; int pitch, x, y;
+	__device__ __forceinline__ float operator()(int dx, int dy) const { return __ldg(img + (size_t)(y+dy)*pitch + (x+dx)); }
+};
+struct TileTexels {
+	const float* tile; int lx, ly;
+	__device__ __forceinline__ float operator()(int dx, int dy) const { return tile[(ly+dy)*TILE_W + (lx+dx)]; }
+};
+
+// FillPixelPatch + GetWeight (DepthMap.cpp:422-462, DepthMap.h:403-412).  WEIGHTS_ALIAS_TILE: the weights share their
+// shared memory with the tile the texels come from (pm_sweep_kernel), so every thread of the CTA calls this, and the
+// weights are written only after all threads have read their patch.
+template <bool WEIGHTS_ALIAS_TILE, typename Texels>
+__device__ __forceinline__ void fill_patch(const Texels& texel, PatchW& p) {
 	const float sigmaColor = -1.f/(2.f*0.1f*0.1f);
 	const float sigmaSpatial = -1.f/(2.f*9.f);
-	const float center = tile[ly*TILE_W + lx];
+	const float center = texel(0, 0);
 	float acc = 0.f, sumW = 0.f;
 	float w[PM_TEXELS], I[PM_TEXELS];
 	#pragma unroll
@@ -81,7 +91,7 @@ __device__ __forceinline__ void fill_patch_tile(const float* tile, int lx, int l
 		#pragma unroll
 		for (int j = 0; j < 5; ++j) {
 			const int dy = 2*i-PM_HALF, dx = 2*j-PM_HALF;
-			const float v = tile[(ly+dy)*TILE_W + (lx+dx)];
+			const float v = texel(dx, dy);
 			const float dI = v-center;
 			const float wgt = expf(dI*dI*sigmaColor + float(dx*dx+dy*dy)*sigmaSpatial);
 			w[i*5+j] = wgt;
@@ -98,45 +108,11 @@ __device__ __forceinline__ void fill_patch_tile(const float* tile, int lx, int l
 		tw[k] = w[k]*t;
 		nsq += tw[k]*t;
 	}
-	__syncthreads();
+	if (WEIGHTS_ALIAS_TILE)
+		__syncthreads();
 	#pragma unroll
 	for (int k = 0; k < PM_TEXELS; ++k)
 		p.set(k, w[k], tw[k]);
-	p.sumW = sumW;
-	p.normSq0 = nsq;
-}
-
-// FillPixelPatch + GetWeight (DepthMap.cpp:422-462, DepthMap.h:403-412) from global memory (pass A, and
-// the sweep when no TMA descriptor is available)
-__device__ __forceinline__ void fill_patch(const float* __restrict__ img, int pitch, int x, int y, PatchW& p) {
-	const float sigmaColor = -1.f/(2.f*0.1f*0.1f);
-	const float sigmaSpatial = -1.f/(2.f*9.f);
-	const float center = __ldg(img + (size_t)y*pitch + x);
-	float acc = 0.f, sumW = 0.f;
-	float w[PM_TEXELS], I[PM_TEXELS];
-	#pragma unroll
-	for (int i = 0; i < 5; ++i) {
-		#pragma unroll
-		for (int j = 0; j < 5; ++j) {
-			const int dy = 2*i-PM_HALF, dx = 2*j-PM_HALF;
-			const float v = __ldg(img + (size_t)(y+dy)*pitch + (x+dx));
-			const float dI = v-center;
-			const float wgt = expf(dI*dI*sigmaColor + float(dx*dx+dy*dy)*sigmaSpatial);
-			w[i*5+j] = wgt;
-			I[i*5+j] = v;
-			acc += v*wgt;
-			sumW += wgt;
-		}
-	}
-	const float tm = acc/sumW;
-	float nsq = 0.f;
-	#pragma unroll
-	for (int k = 0; k < PM_TEXELS; ++k) {
-		const float t = I[k]-tm;
-		const float tw = w[k]*t;
-		nsq += tw*t;
-		p.set(k, w[k], tw);
-	}
 	p.sumW = sumW;
 	p.normSq0 = nsq;
 }
@@ -152,6 +128,31 @@ struct Hyp {      // one plane hypothesis at the current pixel
 __device__ __forceinline__ float fast_rcp(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float pow2neg(unsigned i) { return __int_as_float((int)(127u-i)<<23); } // 2^-i, scaleRanges[] (DepthMap.cpp:358-359)
 __device__ __forceinline__ float dot3(const float3& a, const float3& b) { return a.x*b.x + a.y*b.y + a.z*b.z; }
+
+// the viewing ray X0 = Kref^-1 (x, y, 1) of pixel (x, y); its z component is 1
+__device__ __forceinline__ float2 pixel_ray(const PMParams& P, float fx, float fy) {
+	return make_float2(fx*P.ifx + fy*P.sk + P.ox, fy*P.ify + P.oy);
+}
+
+// A pixel that is estimated: its patch lies inside the image and the ignore-mask (DepthData::ApplyIgnoreMask,
+// DepthMap.cpp:215-230; masked pixels are not in the pixel list, DepthMap.cpp:343) keeps it
+__device__ __forceinline__ bool pixel_active(const PMParams& P, int x, int y) {
+	return x >= PM_HALF && y >= PM_HALF && x < P.W-PM_HALF && y < P.H-PM_HALF
+		&& !(P.mask && P.mask[(size_t)y*P.maskPitch + x] == 0);
+}
+
+// The low-resolution depth prior of pixel idx and its weight (DepthMap.cpp:552-561); false when the patch is too flat
+// (fDescriptorMinMagnitudeThreshold) and no prior vouches for the pixel
+__device__ __forceinline__ bool pixel_prior(const PMParams& P, size_t idx, float normSq0, float& priorD, float& priorF) {
+	priorD = 0.f; priorF = 0.f;
+	if (P.lowres)
+		priorD = fmaxf(__ldg(P.lowres + idx), 0.f);
+	if (normSq0 < P.thMagnitudeSq && !(priorD > 0.f))
+		return false;
+	if (priorD > 0.f)
+		priorF = expf(normSq0*(-1.f/0.02f));
+	return true;
+}
 
 // masked bilinear depth sample (TImage::sample with functor, libs/Common/Types.inl:2297-2313)
 __device__ __forceinline__ bool sample_depth_masked(const float* __restrict__ img, int pitch, float px, float py, float ref, float& v) {
@@ -363,9 +364,8 @@ __device__ __forceinline__ void make_hyp(const PMParams& P, int x, int y, float 
 				close_offset(dir, k, ox, oy);
 				const float4 np = P.plane[(size_t)(y+oy)*P.W + (x+ox)];
 				const float3 cn = make_float3(np.x, np.y, np.z);
-				const float nfx = float(x+ox), nfy = float(y+oy);
-				const float rx = nfx*P.ifx + nfy*P.sk + P.ox, ry = nfy*P.ify + P.oy;
-				const float dist = (n.x*rx + n.y*ry + n.z)*np.w + planeD;
+				const float2 r = pixel_ray(P, float(x+ox), float(y+oy));
+				const float dist = (n.x*r.x + n.y*r.y + n.z)*np.w + planeD;
 				const float rd = dist/d;
 				const float factorDepth = expf(rd*rd*P.smoothSigmaDepth);
 				float ca = dot3(n, cn)/sqrtf(nn*dot3(cn, cn));
@@ -431,19 +431,14 @@ pm_score_kernel(const __grid_constant__ PMParams P)
 	if (x >= P.W || y >= P.H)
 		return;
 	const size_t idx = (size_t)y*P.W + x;
-	const bool inside = x >= PM_HALF && y >= PM_HALF && x < P.W-PM_HALF && y < P.H-PM_HALF;
 	PatchW pt;
 	pt.s = smemW + threadIdx.y*BLOCK_X + threadIdx.x;
 	float priorD = 0.f, priorF = 0.f;
-	// ignore-mask (DepthData::ApplyIgnoreMask, DepthMap.cpp:215-230; masked pixels are not in the pixel list,
-	// DepthMap.cpp:343): depth / normal zero, never scored.  Internally their cost is 2 like every rejected pixel.
-	bool ok = inside && !(P.mask && P.mask[(size_t)y*P.maskPitch + x] == 0);
+	// a rejected or masked pixel: depth / normal zero, never scored; internally its cost is 2
+	bool ok = pixel_active(P, x, y);
 	if (ok) {
-		fill_patch(P.img0, P.pitch0, x, y, pt);
-		if (P.lowres)
-			priorD = fmaxf(__ldg(P.lowres + idx), 0.f);
-		if (pt.normSq0 < P.thMagnitudeSq && !(priorD > 0.f))
-			ok = false;
+		fill_patch<false>(ImageTexels{P.img0, P.pitch0, x, y}, pt);
+		ok = pixel_prior(P, idx, pt.normSq0, priorD, priorF);
 	}
 	if (!ok) {
 		P.plane[idx] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -451,10 +446,9 @@ pm_score_kernel(const __grid_constant__ PMParams P)
 		if (P.bestViews) P.bestViews[idx] = 0xFFFFFFFFu;
 		return;
 	}
-	if (priorD > 0.f)
-		priorF = expf(pt.normSq0*(-1.f/0.02f));
 	const float fx = float(x), fy = float(y);
-	const float X0x = fx*P.ifx + fy*P.sk + P.ox, X0y = fy*P.ify + P.oy;
+	const float2 X0 = pixel_ray(P, fx, fy);
+	const float X0x = X0.x, X0y = X0.y;
 	float4 pl = P.plane[idx];
 	float3 n = make_float3(pl.x, pl.y, pl.z);
 	float d = pl.w;
@@ -492,49 +486,35 @@ pm_sweep_kernel(const __grid_constant__ PMParams P, const __grid_constant__ CUte
 {
 	extern __shared__ __align__(128) unsigned char smemRaw[];
 	// [ patch weights | mbarrier ]; the reference tile occupies the start of the weights until the weights are
-	// written (fill_patch_tile): 4.6 KB less shared memory per CTA, which the SM's L1/shared array gives to L1
+	// written (fill_patch): 4.6 KB less shared memory per CTA, which the SM's L1/shared array gives to L1
 	float2* smemW = (float2*)smemRaw;
 	float* tile = (float*)smemRaw;
 	uint64_t* bar = (uint64_t*)(smemRaw + PM_TEXELS*NTHREADS*sizeof(float2));
 	const int tid = threadIdx.y*BLOCK_X + threadIdx.x;
-	if (P.tma) {
-		if (tid == 0) {
-			mbar_init(bar, 1);
-			asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // make the init visible to the async proxy
-		}
-		__syncthreads();
-		if (tid == 0) {
-			mbar_expect_tx(bar, TILE_BYTES);
-			tma_load_2d(tile, &tmapRef, (int)blockIdx.x*(2*BLOCK_X)-PM_HALF, (int)blockIdx.y*BLOCK_Y-PM_HALF, bar);
-		}
-		mbar_wait(bar, 0);
+	if (tid == 0) {
+		mbar_init(bar, 1);
+		asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // make the init visible to the async proxy
 	}
+	__syncthreads();
+	if (tid == 0) {
+		mbar_expect_tx(bar, TILE_BYTES);
+		tma_load_2d(tile, &tmapRef, (int)blockIdx.x*(2*BLOCK_X)-PM_HALF, (int)blockIdx.y*BLOCK_Y-PM_HALF, bar);
+	}
+	mbar_wait(bar, 0);
 	const int y = blockIdx.y*BLOCK_Y + threadIdx.y;
 	const int x = blockIdx.x*(2*BLOCK_X) + 2*threadIdx.x + ((y+P.colour)&1);
-	const bool active = x >= PM_HALF && y >= PM_HALF && x < P.W-PM_HALF && y < P.H-PM_HALF
-		&& !(P.mask && P.mask[(size_t)y*P.maskPitch + x] == 0);
+	const bool active = pixel_active(P, x, y);
 	const int W = P.W, H = P.H;
 	const size_t idx = (size_t)y*W + x;
 	PatchW pt;
 	pt.s = smemW + tid;
-	if (P.tma) {
-		fill_patch_tile(tile, 2*(int)threadIdx.x + ((y+P.colour)&1) + PM_HALF, (int)threadIdx.y + PM_HALF, pt);
-		if (!active)
-			return;
-	} else {
-		if (!active)
-			return;
-		fill_patch(P.img0, P.pitch0, x, y, pt);
-	}
-	float priorD = 0.f, priorF = 0.f;
-	if (P.lowres)
-		priorD = fmaxf(__ldg(P.lowres + idx), 0.f);
-	if (pt.normSq0 < P.thMagnitudeSq && !(priorD > 0.f))
+	fill_patch<true>(TileTexels{tile, 2*(int)threadIdx.x + ((y+P.colour)&1) + PM_HALF, (int)threadIdx.y + PM_HALF}, pt);
+	float priorD, priorF;
+	if (!active || !pixel_prior(P, idx, pt.normSq0, priorD, priorF))
 		return;
-	if (priorD > 0.f)
-		priorF = expf(pt.normSq0*(-1.f/0.02f));
 	const float fx = float(x), fy = float(y);
-	const float X0x = fx*P.ifx + fy*P.sk + P.ox, X0y = fy*P.ify + P.oy;
+	const float2 X0 = pixel_ray(P, fx, fy);
+	const float X0x = X0.x, X0y = X0.y;
 
 	// neighbours: causal pair of the sweep direction first (DepthMap.cpp:641-766)
 	const int dir = P.sweep & 1;
@@ -758,12 +738,10 @@ cudaError_t pm_launch_score(const PMParams& P, bool geom, cudaStream_t s) {
 	if (geom) pm_score_kernel<true><<<grid, block, W_BYTES, s>>>(P); else pm_score_kernel<false><<<grid, block, W_BYTES, s>>>(P);
 	return cudaGetLastError();
 }
-// tmapRef: TMA descriptor of the reference image with box {72, 16} (pm_tma_box), or null (P.tma must be 0)
-cudaError_t pm_launch_sweep(const PMParams& P, const void* tmapRef, bool geom, cudaStream_t s) {
+// tmapRef: TMA descriptor of the reference image P.img0 with box {72, 16} (pm_tma_box)
+cudaError_t pm_launch_sweep(const PMParams& P, const CUtensorMap& tmapRef, bool geom, cudaStream_t s) {
 	dim3 block(BLOCK_X, BLOCK_Y), grid((P.W+2*BLOCK_X-1)/(2*BLOCK_X), (P.H+BLOCK_Y-1)/BLOCK_Y);
-	CUtensorMap map; memset(&map, 0, sizeof(map));
-	if (tmapRef) memcpy(&map, tmapRef, sizeof(map));
-	if (geom) pm_sweep_kernel<true><<<grid, block, SWEEP_SMEM, s>>>(P, map); else pm_sweep_kernel<false><<<grid, block, SWEEP_SMEM, s>>>(P, map);
+	if (geom) pm_sweep_kernel<true><<<grid, block, SWEEP_SMEM, s>>>(P, tmapRef); else pm_sweep_kernel<false><<<grid, block, SWEEP_SMEM, s>>>(P, tmapRef);
 	return cudaGetLastError();
 }
 void pm_tma_box(int* w, int* h) { *w = TILE_W; *h = TILE_H; }

@@ -255,11 +255,12 @@ class _Context:
 
 	def SetDebug(self, **kw):
 		"""b200mvs_set_debug: diagnostic kernel switches, the fields of b200mvs_debug; no arguments = defaults.
-		PatchMatch: scalarTaps, noTMA, sweepFourCtas.  SGM: sgmAggregation (0 auto, 1 general, 2 register-pipelined uniform,
-		3 bulk-copy ring, 4 wave fronts), sgmCost, frontLayout / frontSerial / frontBlock / frontLag / frontCtas / frontDepth."""
+		SGM: sgmAggregation (0 auto, 1 general, 2 register-pipelined uniform, 3 bulk-copy ring, 4 wave fronts), sgmCost,
+		frontLayout / frontSerial / frontBlock / frontLag / frontCtas / frontDepth / frontSubCell.  PatchMatch has no switches.
+		An unknown or reserved field name raises AttributeError."""
 		d = _lib.Debug()
 		for k, v in kw.items():
-			if k == "reserved" or not hasattr(d, k):
+			if k.startswith("reserved") or not hasattr(d, k):
 				raise AttributeError(k)
 			setattr(d, k, int(v))
 		self._call("set_debug", C.byref(d))

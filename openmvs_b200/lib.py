@@ -34,8 +34,8 @@ class Params(C.Structure):
 
 class Debug(C.Structure):
 	"""b200mvs_debug"""
-	_fields_ = [("scalarTaps", C.c_int), ("noTMA", C.c_int), ("sgmAggregation", C.c_int), ("sgmCost", C.c_int),
-		("sweepFourCtas", C.c_int), ("frontLayout", C.c_int), ("frontSerial", C.c_int), ("frontBlock", C.c_int), ("frontLag", C.c_int),
+	_fields_ = [("reserved0", C.c_int), ("reserved1", C.c_int), ("sgmAggregation", C.c_int), ("sgmCost", C.c_int),
+		("reserved2", C.c_int), ("frontLayout", C.c_int), ("frontSerial", C.c_int), ("frontBlock", C.c_int), ("frontLag", C.c_int),
 		("frontCtas", C.c_int), ("frontDepth", C.c_int), ("frontSubCell", C.c_int), ("reserved", C.c_int*4)]
 
 

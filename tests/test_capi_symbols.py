@@ -159,3 +159,16 @@ def test_null_context_and_bad_arguments_return_status_codes():
 	assert dll.b200mvs_filter_depth_map_device(None, None, None, 0, None, C.c_float(0), C.c_float(1), None, None, None, None, None, None) == 1
 	assert dll.b200mvs_remove_small_segments(None, None, None, None, 0, 0, C.c_float(0.01), 100, None) == 1
 	assert dll.b200mvs_gap_interpolation_device(None, None, None, None, 0, 0, C.c_float(0.01), 7, None) == 1
+
+
+def test_set_debug_refuses_reserved_and_unknown_fields():
+	"""The retired PatchMatch switches are reserved fields of b200mvs_debug: naming one (or an old name) is an error, not a
+	silent no-op.  The check runs before any call into the library."""
+	from openmvs_b200 import lib
+	from openmvs_b200.depth_estimator import PatchMatchB200
+	names = [f for f, _ in lib.Debug._fields_]
+	assert names[:2] == ["reserved0", "reserved1"] and names[4] == "reserved2"
+	pm = PatchMatchB200.__new__(PatchMatchB200)   # no context: SetDebug must refuse the name before using one
+	for k in ("reserved", "reserved0", "reserved1", "reserved2", "noTMA", "scalarTaps", "sweepFourCtas"):
+		with pytest.raises(AttributeError):
+			pm.SetDebug(**{k: 1})

@@ -678,3 +678,122 @@ def test_baseline_config0_two_view_640x480(env):
 	iou_f, agree_f = agreement(g["zz1_depth"].astype(np.float32), gd)
 	_record("config0_vs_golden_fixture", iou=iou_f, agree=agree_f, agree_zz_self_fixture=float(g["agree_zz1_zz8"]))
 	assert iou_f > 0.99 and agree_f > float(g["agree_zz1_zz8"])-0.02
+
+
+def _crop_reference(views, x0, y0, w, h):
+	"""views with the reference replaced by its w x h crop at (x0, y0) (principal point shifted with it)"""
+	from openmvs_b200 import synth
+	v = views[0]
+	K = v.K.copy(); K[0, 2] -= x0; K[1, 2] -= y0
+	crop = lambda a: np.ascontiguousarray(a[y0:y0+h, x0:x0+w])
+	return [synth.View(crop(v.image), K, v.R, v.C, crop(v.depth_gt), crop(v.normal_gt))]+list(views[1:])
+
+
+def test_reference_smaller_than_the_tma_box(env, small_scene):
+	"""A 64 x 14 reference image: the sweep's 72 x 16 TMA box exceeds it in both dimensions (the outside is zero-filled).
+	Pass A and one sweep from the oracle's state, with the thresholds of the 320 x 240 sweep test; then a whole estimate."""
+	e = env
+	sc, ref, views = small_scene
+	views = _crop_reference(views, 128, 113, 64, 14)
+	_set(e, nSubResolutionLevels=0, nEstimationGeometricIters=0, nPropagation=4)
+	nR = 3
+	prm = e.O.default_params(schedule=1, propagation=e.O.rb_propagation(4, e.OPT.nPropagationFar, 0), nRandomIters=nR, nSubResolutionLevels=0, threads=4)
+	d, n, c = e.O.pm_score(views, prm, sc.dmin, sc.dmax)
+	assert d.shape == (14, 64) and (d > 0).sum() > 100
+	dv = _dev_views(e, views)
+	plane = torch.zeros(14, 64, 4, device=e.dev); cost = torch.zeros(14, 64, device=e.dev)
+	e.pm.ScoreDepthMap(dv, sc.dmin, sc.dmax, plane, cost)
+	pg, cg = plane.cpu().numpy(), cost.cpu().numpy()
+	assert np.abs(pg[..., 3]-d).max() < 1e-5 and np.abs(pg[..., :3]-n).max() < 1e-5
+	assert np.abs(cg-c).mean() < 2e-5
+	plane = _plane(e, d, n); cost = torch.from_numpy(c).to(e.dev)
+	e.pm.SweepDepthMap(dv, sc.dmin, sc.dmax, plane, cost, 0, nRandomIters=nR)
+	d, n, c = e.O.pm_iterate(views, prm, sc.dmin, sc.dmax, d, n, c, 0)
+	pg, cg = plane.cpu().numpy(), cost.cpu().numpy()
+	m = d > 0
+	rel = np.abs(pg[..., 3]-d)[m]/d[m]
+	assert (rel > 1e-3).mean() < 2e-3 and (rel > 1e-5).mean() < 0.12
+	assert np.abs(cg-c)[m].mean() < 5e-5
+	assert np.array_equal(pg[..., 3] > 0, m)
+	_set(e, nEstimationIters=2, nSweepsPerIter=2, nRandomIters=6)
+	dd = e.DepthData(dv, sc.dmin, sc.dmax)
+	e.pm.EstimateDepthMap(dd)
+	assert e.pm.stats.tma_active == 1 and e.pm.stats.sweep_launches == 2*2*2
+	assert (dd.depthMap > 0).any()
+
+
+def _wide(a, extra=5):
+	"""a copy of the 2-D array a inside a wider allocation: a view with a row pitch larger than its width"""
+	h, w = a.shape
+	buf = torch.zeros(h, w+extra, dtype=a.dtype, device=a.device) if torch.is_tensor(a) else np.zeros((h, w+extra), a.dtype)
+	buf[:, :w] = a
+	return buf[:, :w]
+
+
+def test_building_blocks_on_strided_device_images(env, small_scene):
+	"""ScoreDepthMap / SweepDepthMap on device images sliced out of wider allocations equal the contiguous calls bit for bit
+	(the reference pitch (w+5)*4 is not 16-byte aligned, so the sweep also stages a re-pitched copy)."""
+	e = env
+	sc, ref, views = small_scene
+	_set(e, nSubResolutionLevels=0, nEstimationGeometricIters=0, nPropagation=4)
+	h, w = views[0].image.shape
+	packed = _dev_views(e, views)
+	strided = [e.ViewData(_wide(v.image), v.camera) for v in packed]
+	assert strided[0].image.stride(0) == w+5
+	out = []
+	for dv in (packed, strided):
+		plane = torch.zeros(h, w, 4, device=e.dev); cost = torch.zeros(h, w, device=e.dev)
+		e.pm.ScoreDepthMap(dv, sc.dmin, sc.dmax, plane, cost)
+		scored = (plane.clone(), cost.clone())
+		e.pm.SweepDepthMap(dv, sc.dmin, sc.dmax, plane, cost, 0, nRandomIters=3)
+		out.append(scored+(plane, cost))
+	for a, b in zip(*out):
+		assert torch.equal(a, b)
+
+
+def test_geometric_pass_with_strided_neighbour_depth_maps(env, small_scene):
+	"""A geometric pass whose neighbour depth-maps have a row pitch larger than their width (host numpy and device torch)
+	equals the call on packed depth-maps bit for bit."""
+	e = env
+	from openmvs_b200 import depth_estimator as DE, lib
+	import ctypes as C
+	sc, ref, views = small_scene
+	rng = np.random.RandomState(3)
+	depths = [None]+[(v.depth_gt.copy(), v.K, v.R, v.C) for v in views[1:]]
+	init_d = sc.views[ref].depth_gt*(1+0.002*rng.randn(*sc.views[ref].depth_gt.shape).astype(np.float32))
+	init_n = sc.views[ref].normal_gt.copy()
+	_set(e, nSubResolutionLevels=0, nEstimationGeometricIters=2, nEstimationIters=3, nSweepsPerIter=2, nRandomIters=6, fEstimationGeometricWeight=0.1)
+	try:
+		# device: depth-maps sliced out of wider tensors
+		packed = _dev_views(e, views, depths)
+		strided = [e.ViewData(v.image, v.camera) for v in packed]
+		for s, p in zip(strided[1:], packed[1:]):
+			s.depthMap, s.cameraDepthMap = _wide(p.depthMap), p.cameraDepthMap
+		assert strided[1].depthMap.stride(0) == strided[1].depthMap.shape[1]+5
+		dev = []
+		for vs in (packed, strided):
+			dd = e.DepthData(vs, sc.dmin, sc.dmax, depthMap=torch.from_numpy(init_d).to(e.dev), normalMap=torch.from_numpy(init_n).to(e.dev))
+			e.pm.EstimateDepthMap(dd, nGeometricIter=0)
+			dev.append(dd)
+		# host: the binding packs numpy depth-maps, so the strided views are built at the C-ABI
+		hviews = [e.ViewData(np.ascontiguousarray(v.image), e.Camera(v.K, v.R, v.C)) for v in views]
+		for hv, dp in zip(hviews[1:], depths[1:]):
+			hv.depthMap, hv.cameraDepthMap = dp[0], e.Camera(*dp[1:])
+		base = e.DepthData(hviews, sc.dmin, sc.dmax, depthMap=init_d.copy(), normalMap=init_n.copy())
+		e.pm.EstimateDepthMap(base, nGeometricIter=0)
+		arr, keep, _ = DE._make_views(hviews)
+		for i in range(1, len(hviews)):
+			wd = _wide(hviews[i].depthMap)
+			keep.append(wd)
+			arr[i].depth = wd.ctypes.data; arr[i].dstride_bytes = wd.strides[0]
+		assert arr[1].dstride_bytes == (arr[1].dwidth+5)*4
+		hd = e.DepthData(hviews, sc.dmin, sc.dmax, depthMap=init_d.copy(), normalMap=init_n.copy())
+		e.pm._set_params()
+		e.pm._call("estimate", arr, len(arr), sc.dmin, sc.dmax, 0, *DE._host_maps(hd), C.byref(e.pm.stats))
+	finally:
+		_set(e, nEstimationGeometricIters=0)
+	a, b = dev
+	assert (a.depthMap > 0).float().mean() > 0.5
+	for name in ("depthMap", "normalMap", "confMap", "viewsMap"):
+		assert torch.equal(getattr(a, name), getattr(b, name)), name
+		assert np.array_equal(getattr(base, name), getattr(hd, name)), name
