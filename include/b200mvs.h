@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define B200MVS_ABI_VERSION 6 /* struct layouts of this header; b200mvs_abi_version() returns the library's */
+#define B200MVS_ABI_VERSION 7 /* struct layouts of this header; b200mvs_abi_version() returns the library's */
 #define B200MVS_MAX_VIEWS 32 /* neighbours per reference view (MAX_VIEWS, PatchMatchCUDA.inl:35) */
 
 typedef struct b200mvs_ctx b200mvs_ctx;
@@ -131,7 +131,7 @@ int  b200mvs_set_debug(b200mvs_ctx* ctx, const b200mvs_debug* d /* NULL: default
 /* sweeps and refinement tries per sweep the engine runs for p (geometric != 0: for one geometric-consistency pass) */
 int  b200mvs_get_schedule(const b200mvs_params* p, int geometric, int* nSweeps, int* nRefinePerSweep);
 int  b200mvs_abi_version(void);
-size_t b200mvs_sizeof(int what); /* 0 view, 1 params, 2 stats, 3 job, 4 sgm_pixel, 5 sgm_params, 6 dmap, 7 filter_params, 8 debug */
+size_t b200mvs_sizeof(int what); /* 0 view, 1 params, 2 stats, 3 job, 4 sgm_pixel, 5 sgm_params, 6 dmap, 7 filter_params, 8 debug, 9 sgm_pair */
 /* Ignore-mask of the reference view for the following estimate calls (OPTDENSE::nIgnoreMaskLabel >= 0:
  * DepthEstimator::ImportIgnoreMask + DepthData::ApplyIgnoreMask, libs/MVS/DepthMap.cpp:215-230,300-323;
  * SceneDensify.cpp:660-664,679-693): one byte per pixel of the full-resolution reference image, 0 = ignored.  Ignored pixels
@@ -316,6 +316,54 @@ int b200mvs_resize_area_u8_device(b200mvs_ctx* ctx, const uint8_t* src, int widt
 	void* stream);
 int b200mvs_sgm_level_mask_device(b200mvs_ctx* ctx, const uint8_t* mask, int width, int height, int levelWidth, int levelHeight,
 	uint8_t* validMask, void* stream);
+
+/* ---- SGM disparity maps to the depth-map of an image: fusion-mode -2 (Scene::DenseReconstructionEstimate -> SemiGlobalMatcher::Fuse,
+ * libs/MVS/SceneDensify.cpp:2049-2056, libs/MVS/SemiGlobalMatcher.cpp:739-859) -------------------------------------------------------
+ * One pair: the left disparity map of a rectified pair over its valid region, as b200mvs_sgm_match_hierarchical_device returns it and
+ * the pair's .dimap file holds it (ImportDisparityDataRawFull, :2174-2184): disparity * subpixelSteps, NO_DISP = 32767; the optional
+ * summed path cost of the same size; Q (4x4, row-major) maps the rectified pixel (c+3, r+3) and its disparity d to the pixel and depth
+ * of the image the depth-map is made for (Image::Disparity2Depth, libs/MVS/Image.cpp:392-404).  Pointers are device pointers for the
+ * _device calls and host pointers for b200mvs_sgm_fuse. */
+#define B200MVS_SGM_MAX_PAIRS 32
+typedef struct b200mvs_sgm_pair b200mvs_sgm_pair;
+struct b200mvs_sgm_pair {
+	const int16_t* disparity;  /* width x height, row-major */
+	const uint16_t* cost;      /* width x height or NULL: confidence 0 */
+	int width, height;         /* the valid region (rectified size - 6) */
+	int subpixelSteps;         /* >= 1 */
+	double Q[16];
+};
+
+/* Q of a pair whose left image is the other view (the file <other>_<this>.dimap, SemiGlobalMatcher.cpp:770-779): Qout = P * invK * Q
+ * with invK the inverse of the pair-left camera's K and P = K [Rrel | -Rrel Crel] of the relative pose Rrel = R Rleft^T,
+ * Crel = Rleft (C - Cleft).  Kleft / Rleft / Cleft: the pair's left camera; K / R / C: the camera of the image the depth-map is made
+ * for.  Host code (double); Qout may alias Q. */
+int b200mvs_sgm_pair_q(const double* Q, const double* Kleft, const double* Rleft, const double* Cleft, const double* K, const double* R,
+	const double* C, double* Qout);
+
+/* ProjectDisparity2DepthMap (SemiGlobalMatcher.cpp:1925-2039) of one pair into a width x height image, DEVICE pointers: per pixel
+ * the weighted mean of the nearest projected source on each side, depth = 0 where none is within 0.75 pixel.  depthRange: 2 floats
+ * per pixel (the depths at floor(disparity) -/+ 1); conf (nullable): 1/(cost+1), 0 without a cost map.  Rejected pixels have depth,
+ * range and conf 0. */
+int b200mvs_sgm_project_disparity_device(b200mvs_ctx* ctx, const b200mvs_sgm_pair* pair, int width, int height, float* depth,
+	float* depthRange, float* conf, void* stream);
+
+/* SemiGlobalMatcher::Fuse (SemiGlobalMatcher.cpp:795-848): the pairs projected as above, then per pixel the mean depth and conf of the
+ * largest cluster of agreeing depths (the first on ties) when it holds at least minViews pairs (the reference passes 2), else 0.
+ * K (nullable, 9 doubles): also EstimateNormalMap of the fused depths into normal (3 floats per pixel), like nEstimateNormals == 2.
+ * Either every pair has a cost map or none has one (then conf = 0).  conf nullable; normal required with K.  1 <= nPairs <=
+ * B200MVS_SGM_MAX_PAIRS.  The device form enqueues on `stream` and reads nothing back; the host form uploads the maps, waits and
+ * fills stats (nullable). */
+int b200mvs_sgm_fuse_device(b200mvs_ctx* ctx, const b200mvs_sgm_pair* pairs, int nPairs, int width, int height, int minViews,
+	const double* K, float* depth, float* conf, float* normal, void* stream);
+int b200mvs_sgm_fuse(b200mvs_ctx* ctx, const b200mvs_sgm_pair* pairs, int nPairs, int width, int height, int minViews,
+	const double* K, float* depth, float* conf, float* normal, b200mvs_stats* stats);
+
+/* EstimateNormalMap(K, depthMap, normalMap) (libs/MVS/DepthMap.cpp:1522-1613), DEVICE pointers: per pixel the least-squares depth
+ * gradient over the 3x3 neighbours within 3 % of its depth (at least 3), turned into a unit camera-space normal with the float K
+ * converted from the 9 doubles of K; 0 where the depth is 0 or the gradient is undetermined. */
+int b200mvs_estimate_normal_map_device(b200mvs_ctx* ctx, const float* depth, int width, int height, const double* K, float* normal,
+	void* stream);
 
 /* ---- depth-map post-processing after the estimation (SURVEY.md §8(f) rank 2) -----------------
  * DepthMapsData::FilterDepthMap / RemoveSmallSegments / GapInterpolation

@@ -35,6 +35,7 @@ size_t b200mvs_sizeof(int what) {
 	case 6: return sizeof(b200mvs_dmap);
 	case 7: return sizeof(b200mvs_filter_params);
 	case 8: return sizeof(b200mvs_debug);
+	case 9: return sizeof(b200mvs_sgm_pair);
 	default: return 0;
 	}
 }

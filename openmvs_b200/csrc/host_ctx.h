@@ -55,6 +55,7 @@ struct b200mvs_ctx {
 	enum { TS_IMG, TS_MASKL, TS_MASKR, TS_MASKT, TS_DL, TS_DR, TS_DL0, TS_DR0, TS_PXL, TS_PXR, TS_RANGES, TS_SCAN, TS_KEYS, TS_LABELS,
 		TS_SIZES, TS_SMALL, TS_COUNT };
 	DevBuf ts[TS_COUNT];
+	DevBuf sfKeys, sfMaps, sfIn, sfOut;       // SGM fusion: splat keys, per-pair depth / range / conf maps, staged pairs and outputs (host API)
 	DevBuf fltZ, fltIn, fltOutD, fltOutC;     // FilterDepthMap: z-buffer keys, staged maps (host API), outputs
 	DevBuf ppA, ppB, ppD, ppN, ppC;           // RemoveSmallSegments labels/sizes, GapInterpolation temporaries, staging
 	DevBuf ppK, ppArcs, ppPatch;              // RemoveSmallSegments: seed keys, one-way edges (+ counter), patched segment sizes

@@ -68,3 +68,16 @@ cudaError_t tsgm_launch_area_u8(const uint8_t* src, int sw, int sh, int cn, uint
 cudaError_t tsgm_launch_fill(int16_t* d, size_t n, int16_t v, cudaStream_t s);
 cudaError_t tsgm_launch_minmax(const int16_t* d, size_t n, int* out2, cudaStream_t s);
 cudaError_t tsgm_launch_dense_map(SGMPixel* px, size_t n, int lo, int hi, cudaStream_t s);
+
+// sgm_fuse.cu: one pair of fusion-mode -2 as the kernels read it (the device view of b200mvs_sgm_pair), and all pairs of a call,
+// passed by value as the kernel parameter (about 5 KB)
+struct SGMFusePair { const int16_t* disp; const uint16_t* cost; int vw, vh, steps, pad; double Q[16]; };
+struct SGMFuseArgs { SGMFusePair pair[B200MVS_SGM_MAX_PAIRS]; int n; };
+// keys: n x 4 x W x H, set to all ones here; depth / range / conf (conf nullable in the gather): pair p at offset p x pairStride
+cudaError_t sgmf_launch_project(const SGMFuseArgs& A, int W, int H, unsigned long long* keys, cudaStream_t s);
+cudaError_t sgmf_launch_gather(const SGMFuseArgs& A, int W, int H, const unsigned long long* keys, float* depth, float2* range, float* conf,
+	size_t pairStride, cudaStream_t s);
+cudaError_t sgmf_launch_fuse(int nPairs, int W, int H, const float* depth, const float2* range, const float* conf, size_t pairStride,
+	int minViews, float* outDepth, float* outConf, cudaStream_t s);
+// K = (fx, fy, cx, cy) as floats; normal: 3 floats per pixel
+cudaError_t sgmf_launch_normals(const float* depth, int W, int H, float4 K, float* normal, cudaStream_t s);

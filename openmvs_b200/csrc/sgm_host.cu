@@ -565,4 +565,167 @@ int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
 	return B200MVS_OK;
 }
 
+// ---- fusion-mode -2: the pairs' disparity maps projected into an image and fused (SemiGlobalMatcher::Fuse) ----
+
+// Q of a reversed pair (SemiGlobalMatcher.cpp:770-779), products as cv::Matx computes them (s = 0; s += a(i,k) b(k,j))
+int b200mvs_sgm_pair_q(const double* Q, const double* Kl, const double* Rl, const double* Cl, const double* K, const double* R,
+	const double* C, double* Qout)
+{
+	if (!Q || !Kl || !Rl || !Cl || !K || !R || !C || !Qout) return B200MVS_ERR_ARG;
+	if (Kl[0] == 0 || Kl[4] == 0) return B200MVS_ERR_ARG;
+	// ComputeRelativePose(Rl, Cl, R, C): Rrel = R Rl^T, Crel = Rl (C - Cl) (libs/Common/Util.inl:39-42)
+	double Rr[9], Cr[3], dC[3] = {C[0]-Cl[0], C[1]-Cl[1], C[2]-Cl[2]};
+	for (int i = 0; i < 3; ++i) {
+		for (int j = 0; j < 3; ++j) { double s = 0; for (int k = 0; k < 3; ++k) s += R[i*3+k]*Rl[j*3+k]; Rr[i*3+j] = s; }
+		double s = 0; for (int k = 0; k < 3; ++k) s += Rl[i*3+k]*dC[k]; Cr[i] = s;
+	}
+	// P = [K Rrel | K Rrel (-Crel)] over the last row of the identity (AssembleProjectionMatrix, libs/MVS/Camera.cpp:173-180)
+	double P[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 1};
+	for (int i = 0; i < 3; ++i) {
+		for (int j = 0; j < 3; ++j) { double s = 0; for (int k = 0; k < 3; ++k) s += K[i*3+k]*Rr[k*3+j]; P[i*4+j] = s; }
+		double s = 0; for (int k = 0; k < 3; ++k) s += P[i*4+k]*(-Cr[k]); P[i*4+3] = s;
+	}
+	// invK of the pair's left camera in the identity (Camera::InvK, libs/MVS/Camera.h:177-185)
+	double iK[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+	iK[0] = 1.0/Kl[0]; iK[5] = 1.0/Kl[4]; iK[2] = -Kl[2]*iK[0]; iK[6] = -Kl[5]*iK[5];
+	double T[16], O[16];
+	auto mul4 = [](const double* a, const double* b, double* c) {
+		for (int i = 0; i < 4; ++i) for (int j = 0; j < 4; ++j) { double s = 0; for (int k = 0; k < 4; ++k) s += a[i*4+k]*b[k*4+j]; c[i*4+j] = s; }
+	};
+	mul4(P, iK, T); mul4(T, Q, O);
+	memcpy(Qout, O, sizeof(O));
+	return B200MVS_OK;
+}
+
+// checks the pairs and target size of a projection / fusion call and fills the kernels' parameter block; no device work
+static int sgmf_args(b200mvs_ctx* ctx, const b200mvs_sgm_pair* pairs, int nPairs, int width, int height, SGMFuseArgs& A) {
+	if (!pairs || nPairs < 1 || nPairs > B200MVS_SGM_MAX_PAIRS)
+		return fail(ctx, B200MVS_ERR_ARG, "sgm fuse: null pair array or a pair count outside [1, B200MVS_SGM_MAX_PAIRS]");
+	if (width <= 0 || height <= 0 || (size_t)width*height >= (1u<<31))
+		return fail(ctx, B200MVS_ERR_ARG, "sgm fuse: empty image or one of 2^31 pixels or more");
+	memset(&A, 0, sizeof(A));
+	A.n = nPairs;
+	for (int p = 0; p < nPairs; ++p) {
+		const b200mvs_sgm_pair& q = pairs[p];
+		if (!q.disparity || q.width <= 0 || q.height <= 0 || (size_t)q.width*q.height >= (1u<<31) || q.subpixelSteps < 1 || q.subpixelSteps > 32767)
+			return fail(ctx, B200MVS_ERR_ARG, "sgm fuse: a pair without a disparity map, with an empty or oversized map, or subpixelSteps outside [1, 32767]");
+		// the reference would read the released confidence map of a pair without costs (SemiGlobalMatcher.cpp:2036-2037, :842)
+		if ((q.cost != nullptr) != (pairs[0].cost != nullptr))
+			return fail(ctx, B200MVS_ERR_ARG, "sgm fuse: either every pair has a cost map or none has one");
+		SGMFusePair& d = A.pair[p];
+		d.disp = q.disparity; d.cost = q.cost; d.vw = q.width; d.vh = q.height; d.steps = q.subpixelSteps;
+		memcpy(d.Q, q.Q, sizeof(d.Q));
+	}
+	return B200MVS_OK;
+}
+
+int b200mvs_sgm_project_disparity_device(b200mvs_ctx* ctx, const b200mvs_sgm_pair* pair, int width, int height, float* depth,
+	float* depthRange, float* conf, void* stream)
+{
+	if (!ctx) return B200MVS_ERR_ARG;
+	SGMFuseArgs A;
+	if (int rc = sgmf_args(ctx, pair, 1, width, height, A)) return rc;
+	if (!depth || !depthRange || ((uintptr_t)depthRange & 7))
+		return fail(ctx, B200MVS_ERR_ARG, "project disparity: null depth or range map, or a range map not 8-byte aligned");
+	CK(cudaSetDevice(ctx->device));
+	cudaStream_t s = stream_of(ctx, stream);
+	const size_t n = (size_t)width*height;
+	CK(ctx->sfKeys.reserve(4*n*sizeof(unsigned long long)));
+	CK(sgmf_launch_project(A, width, height, ctx->sfKeys.as<unsigned long long>(), s));
+	CK(sgmf_launch_gather(A, width, height, ctx->sfKeys.as<unsigned long long>(), depth, (float2*)depthRange, conf, n, s));
+	ctx->launches = 2;
+	return B200MVS_OK;
+}
+
+static int sgmf_normals(b200mvs_ctx* ctx, const float* depth, int width, int height, const double* K, float* normal, cudaStream_t s) {
+	// EstimateNormalMap takes Matrix3x3f: the caller's double K converted element by element
+	CK(sgmf_launch_normals(depth, width, height, make_float4((float)K[0], (float)K[4], (float)K[2], (float)K[5]), normal, s));
+	return B200MVS_OK;
+}
+
+int b200mvs_sgm_fuse_device(b200mvs_ctx* ctx, const b200mvs_sgm_pair* pairs, int nPairs, int width, int height, int minViews,
+	const double* K, float* depth, float* conf, float* normal, void* stream)
+{
+	if (!ctx) return B200MVS_ERR_ARG;
+	SGMFuseArgs A;
+	if (int rc = sgmf_args(ctx, pairs, nPairs, width, height, A)) return rc;
+	if (!depth || minViews < 0 || (K && !normal))
+		return fail(ctx, B200MVS_ERR_ARG, "sgm fuse: null depth map, negative minViews, or K without a normal map");
+	CK(cudaSetDevice(ctx->device));
+	cudaStream_t s = stream_of(ctx, stream);
+	const size_t n = (size_t)width*height, np = (size_t)nPairs*n;
+	CK(ctx->sfKeys.reserve(4*np*sizeof(unsigned long long)));
+	CK(ctx->sfMaps.reserve(np*4*sizeof(float)));
+	float2* range = ctx->sfMaps.as<float2>(); float* pd = (float*)(range+np); float* pc = pd+np;
+	CK(sgmf_launch_project(A, width, height, ctx->sfKeys.as<unsigned long long>(), s));
+	CK(sgmf_launch_gather(A, width, height, ctx->sfKeys.as<unsigned long long>(), pd, range, pc, n, s));
+	CK(sgmf_launch_fuse(nPairs, width, height, pd, range, pc, n, minViews, depth, conf, s));
+	ctx->launches = 3;
+	if (K) {
+		if (int rc = sgmf_normals(ctx, depth, width, height, K, normal, s)) return rc;
+		++ctx->launches;
+	}
+	return B200MVS_OK;
+}
+
+int b200mvs_sgm_fuse(b200mvs_ctx* ctx, const b200mvs_sgm_pair* pairs, int nPairs, int width, int height, int minViews,
+	const double* K, float* depth, float* conf, float* normal, b200mvs_stats* stats)
+{
+	if (!ctx) return B200MVS_ERR_ARG;
+	SGMFuseArgs A;
+	if (int rc = sgmf_args(ctx, pairs, nPairs, width, height, A)) return rc;
+	if (!depth || minViews < 0 || (K && !normal))
+		return fail(ctx, B200MVS_ERR_ARG, "sgm fuse: null depth map, negative minViews, or K without a normal map");
+	CK(cudaSetDevice(ctx->device));
+	cudaStream_t s = ctx->stream;
+	const auto t0 = std::chrono::steady_clock::now();
+	// stage the maps: disparities (and costs) of every pair, 16-byte aligned slices
+	std::vector<b200mvs_sgm_pair> dev(pairs, pairs+nPairs);
+	std::vector<size_t> off(nPairs);
+	size_t total = 0;
+	for (int p = 0; p < nPairs; ++p) {
+		off[p] = total;
+		const size_t m = (size_t)pairs[p].width*pairs[p].height;
+		total += ((m*2+15) & ~(size_t)15)*(pairs[p].cost ? 2 : 1);
+	}
+	CK(ctx->sfIn.reserve(total));
+	uint64_t h2d = 0;
+	for (int p = 0; p < nPairs; ++p) {
+		const size_t m = (size_t)pairs[p].width*pairs[p].height;
+		uint8_t* base = ctx->sfIn.as<uint8_t>()+off[p];
+		CK(cudaMemcpyAsync(base, pairs[p].disparity, m*2, cudaMemcpyHostToDevice, s));
+		dev[p].disparity = (const int16_t*)base; h2d += m*2;
+		if (pairs[p].cost) {
+			uint8_t* cb = base+((m*2+15) & ~(size_t)15);
+			CK(cudaMemcpyAsync(cb, pairs[p].cost, m*2, cudaMemcpyHostToDevice, s));
+			dev[p].cost = (const uint16_t*)cb; h2d += m*2;
+		}
+	}
+	const size_t n = (size_t)width*height;
+	CK(ctx->sfOut.reserve(n*5*sizeof(float)));
+	float* dD = ctx->sfOut.as<float>(); float* dC = dD+n; float* dN = dC+n;
+	CK(cudaEventRecord(ctx->ev0, s));
+	if (int rc = b200mvs_sgm_fuse_device(ctx, dev.data(), nPairs, width, height, minViews, K, dD, conf ? dC : nullptr, K ? dN : nullptr, s))
+		return rc;
+	CK(cudaEventRecord(ctx->ev1, s));
+	CK(cudaMemcpyAsync(depth, dD, n*4, cudaMemcpyDeviceToHost, s));
+	if (conf) CK(cudaMemcpyAsync(conf, dC, n*4, cudaMemcpyDeviceToHost, s));
+	if (K) CK(cudaMemcpyAsync(normal, dN, n*12, cudaMemcpyDeviceToHost, s));
+	CK(cudaStreamSynchronize(s));
+	if (stats) return fill_stats(ctx, stats, t0, 1, h2d, n*4+(conf ? n*4 : 0)+(K ? n*12 : 0));
+	return B200MVS_OK;
+}
+
+int b200mvs_estimate_normal_map_device(b200mvs_ctx* ctx, const float* depth, int width, int height, const double* K, float* normal,
+	void* stream)
+{
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!depth || !K || !normal || depth == normal || width <= 0 || height <= 0 || (size_t)width*height >= (1u<<31))
+		return fail(ctx, B200MVS_ERR_ARG, "estimate normal map: null or aliased maps, null K, or an empty or oversized map");
+	CK(cudaSetDevice(ctx->device));
+	if (int rc = sgmf_normals(ctx, depth, width, height, K, normal, stream_of(ctx, stream))) return rc;
+	ctx->launches = 1;
+	return B200MVS_OK;
+}
+
 } // extern "C"

@@ -709,6 +709,112 @@ class SemiGlobalMatcher(_Context):
 		self._call("sgm_level_mask_device", mask.data_ptr(), w, h, lw, lh, out.data_ptr(), _stream_handle(mask.device))
 		return out
 
+	# fusion-mode -2: the disparity maps of the pairs that contain an image, projected into it and fused (SemiGlobalMatcher::Fuse,
+	# libs/MVS/SemiGlobalMatcher.cpp:739-859)
+	@staticmethod
+	def PairQ(Q, Kleft, Rleft, Cleft, K, R, C):
+		"""b200mvs_sgm_pair_q: the Q of a pair whose left image is the other view (camera Kleft, Rleft, Cleft), re-targeted to the image
+		of camera (K, R, C), as Fuse does for the file <other>_<this>.dimap.  Host arithmetic, no GPU needed -> (4, 4) float64"""
+		lib = _lib.load()
+		arrs = [np.ascontiguousarray(a, np.float64).ravel() for a in (Q, Kleft, Rleft, Cleft, K, R, C)]
+		if [a.size for a in arrs] != [16, 9, 9, 3, 9, 9, 3]:
+			raise ValueError("Q must be 4x4, the K and R 3x3 and the C 3-vectors")
+		out = np.zeros(16, np.float64)
+		rc = lib.b200mvs_sgm_pair_q(*[a.ctypes.data for a in arrs], out.ctypes.data)
+		if rc != 0:
+			raise _lib.B200MVSError("b200mvs_sgm_pair_q failed with status %d (a zero focal length in Kleft)" % rc)
+		return out.reshape(4, 4)
+
+	@staticmethod
+	def _pairs(pairs, device: bool):
+		"""[(disparity, cost or None, Q, subpixelSteps), ...] -> (ctypes b200mvs_sgm_pair array, keepalive list)"""
+		if not 1 <= len(pairs) <= _lib.SGM_MAX_PAIRS:
+			raise ValueError("between 1 and %d pairs" % _lib.SGM_MAX_PAIRS)
+		arr = (_lib.SgmPair*len(pairs))()
+		keep = []
+		for o, (disp, cost, Q, steps) in zip(arr, pairs):
+			if device:
+				if not (_is_torch(disp) and disp.is_cuda and str(disp.dtype) == "torch.int16" and disp.is_contiguous()):
+					raise ValueError("disparity must be a contiguous int16 CUDA tensor")
+				if cost is not None and not (_is_torch(cost) and cost.is_cuda and cost.dtype.itemsize == 2 and cost.is_contiguous()
+						and cost.device == disp.device):
+					raise ValueError("cost must be a contiguous 16-bit CUDA tensor on the disparity's device")
+				dptr, cptr = disp.data_ptr(), (cost.data_ptr() if cost is not None else None)
+			else:
+				disp = np.ascontiguousarray(disp, np.int16)
+				cost = None if cost is None else np.ascontiguousarray(cost, np.uint16)
+				dptr, cptr = disp.ctypes.data, (cost.ctypes.data if cost is not None else None)
+			if len(disp.shape) != 2:
+				raise ValueError("disparity must be a 2-D map")
+			if cost is not None and tuple(cost.shape) != tuple(disp.shape):
+				raise ValueError("cost map of shape %s for a disparity map of shape %s" % (tuple(cost.shape), tuple(disp.shape)))
+			keep += [disp, cost]
+			o.disparity, o.cost = dptr, cptr
+			o.height, o.width = (int(x) for x in disp.shape)
+			o.subpixelSteps = int(steps)
+			o.Q[:] = list(np.asarray(Q, np.float64).reshape(16))
+		return arr, keep
+
+	def ProjectDisparity2DepthMap(self, disparityMap, costMap, Q, subpixelSteps: int, size):
+		"""SemiGlobalMatcher::ProjectDisparity2DepthMap (SemiGlobalMatcher.cpp:1925-2039) of one pair on CUDA tensors (disparityMap
+		int16, costMap 16-bit or None) into an image of size = (W, H) -> (depth (H, W), depthRange (H, W, 2), conf (H, W)) float32
+		tensors; rejected pixels are 0 in all three, conf is 0 without a cost map."""
+		import torch
+		W, H = int(size[0]), int(size[1])
+		arr, keep = self._pairs([(disparityMap, costMap, Q, subpixelSteps)], True)
+		dev = disparityMap.device
+		depth = torch.empty((H, W), dtype=torch.float32, device=dev)
+		rng = torch.empty((H, W, 2), dtype=torch.float32, device=dev)
+		conf = torch.empty((H, W), dtype=torch.float32, device=dev)
+		self._call("sgm_project_disparity_device", arr, W, H, depth.data_ptr(), rng.data_ptr(), conf.data_ptr(), _stream_handle(dev))
+		return depth, rng, conf
+
+	def Fuse(self, pairs, size, minViews: int = 2, K=None):
+		"""SemiGlobalMatcher::Fuse (SemiGlobalMatcher.cpp:739-859) for one image of size = (W, H): pairs = [(disparity, cost or None,
+		Q, subpixelSteps), ...] in the order the reference walks the image's neighbours, Q already re-targeted to this image (PairQ
+		for pairs whose left image is the neighbour).  numpy maps take the host path, CUDA tensors the device path.
+		K (3x3, optional): also EstimateNormalMap of the result (nEstimateNormals == 2).  -> (depth, conf, normal or None)"""
+		W, H = int(size[0]), int(size[1])
+		device = _is_torch(pairs[0][0]) if pairs else False
+		arr, keep = self._pairs(pairs, device)
+		k = None if K is None else np.ascontiguousarray(K, np.float64).reshape(9)
+		kp = None if k is None else k.ctypes.data
+		if device:
+			import torch
+			dev = pairs[0][0].device
+			depth = torch.empty((H, W), dtype=torch.float32, device=dev)
+			conf = torch.empty((H, W), dtype=torch.float32, device=dev)
+			normal = torch.empty((H, W, 3), dtype=torch.float32, device=dev) if k is not None else None
+			self._call("sgm_fuse_device", arr, len(pairs), W, H, int(minViews), kp, depth.data_ptr(), conf.data_ptr(),
+				normal.data_ptr() if normal is not None else None, _stream_handle(dev))
+		else:
+			depth = np.zeros((H, W), np.float32); conf = np.zeros((H, W), np.float32)
+			normal = np.zeros((H, W, 3), np.float32) if k is not None else None
+			self._call("sgm_fuse", arr, len(pairs), W, H, int(minViews), kp, depth.ctypes.data, conf.ctypes.data,
+				normal.ctypes.data if normal is not None else None, C.byref(self.stats))
+		return depth, conf, normal
+
+
+_NORMAL_CTX = {}
+
+
+def EstimateNormalMap(K, depthMap):
+	"""MVS::EstimateNormalMap(K, depthMap, normalMap) (libs/MVS/DepthMap.cpp:1522-1613) on a float32 CUDA tensor -> (H, W, 3) unit
+	camera-space normals (0 where undetermined).  K: 3x3, converted to float as the reference's Matrix3x3f argument.  Runs on a
+	context kept per device."""
+	import torch
+	if not (_is_torch(depthMap) and depthMap.is_cuda and depthMap.dtype == torch.float32 and depthMap.dim() == 2 and depthMap.is_contiguous()):
+		raise ValueError("depthMap must be a contiguous 2-D float32 CUDA tensor")
+	dev = depthMap.device
+	ctx = _NORMAL_CTX.get(dev.index)
+	if ctx is None:
+		ctx = _NORMAL_CTX[dev.index] = _Context(dev.index)
+	k = np.ascontiguousarray(K, np.float64).reshape(9)
+	h, w = depthMap.shape
+	normal = torch.empty((h, w, 3), dtype=torch.float32, device=dev)
+	ctx._call("estimate_normal_map_device", depthMap.data_ptr(), w, h, k.ctypes.data, normal.data_ptr(), _stream_handle(dev))
+	return normal
+
 
 @dataclasses.dataclass
 class PointCloud:

@@ -10,6 +10,9 @@ ExportDepthDataRaw / ImportDepthDataRaw follow the reference's raw layout
 
 Host-side plumbing (numpy); files are written atomically (.tmp + rename) like DepthData::Save
 (libs/MVS/DepthMap.cpp:237-251).
+
+The .dimap disparity-data files of the SGM path (ExportDisparityDataRaw[Full] / ImportDisparityDataRaw[Full]) are the hand-off
+between SGM matching (fusion-mode -1) and the fusion of the pairs into depth-maps (fusion-mode -2).
 """
 from __future__ import annotations
 
@@ -74,6 +77,70 @@ def ImportDepthDataRaw(fileName, flags: int = 15) -> dict:
 				if flags & flag:
 					out[key] = np.frombuffer(raw, dt).reshape(shape).copy()
 	return out
+
+
+NO_DISP = 32767          # SemiGlobalMatcher::NO_DISP
+NO_ACCUMCOST = 65535     # SemiGlobalMatcher::NO_ACCUMCOST
+_DIMAP_HEAD = struct.Struct("<ii9d16dhii")   # image size, H, Q, subpixelSteps, map columns and rows (packed, no padding)
+
+
+def ExportDisparityDataRaw(fileName, disparityMap, costMap, imageSize, H, Q, subpixelSteps) -> bool:
+	""".dimap file of one SGM pair (SemiGlobalMatcher::ExportDisparityDataRaw, libs/MVS/SemiGlobalMatcher.cpp:2094-2122), packed little
+	endian: int32 image width and height, 9 doubles H, 16 doubles Q, int16 subpixelSteps, int32 columns and rows of the map, the int16
+	disparity map (disparity * subpixelSteps, NO_DISP where invalid), then the uint16 cost map when there is one."""
+	disp = np.ascontiguousarray(disparityMap, "<i2")
+	rows, cols = disp.shape
+	cost = None if costMap is None else np.ascontiguousarray(costMap, "<u2")
+	if cost is not None and cost.shape != disp.shape:
+		raise ValueError("cost map of shape %s for a disparity map of shape %s" % (cost.shape, disp.shape))
+	head = _DIMAP_HEAD.pack(int(imageSize[0]), int(imageSize[1]), *np.asarray(H, np.float64).reshape(9).tolist(),
+		*np.asarray(Q, np.float64).reshape(16).tolist(), int(subpixelSteps), cols, rows)
+	with open(fileName, "wb") as f:
+		f.write(head)
+		f.write(disp.tobytes())
+		if cost is not None:
+			f.write(cost.tobytes())
+	return True
+
+
+def ExportDisparityDataRawFull(fileName, disparityMap, costMap, imageSize, H, Q, subpixelSteps) -> bool:
+	"""ExportDisparityDataRaw of the maps padded with the 3-pixel border the matcher leaves out (NO_DISP / NO_ACCUMCOST;
+	SemiGlobalMatcher.cpp:2124-2138): the form SGM matching writes and fusion reads."""
+	disp = np.asarray(disparityMap)
+	pad = lambda m, v: np.pad(np.asarray(m), 3, constant_values=v)
+	return ExportDisparityDataRaw(fileName, pad(disp, NO_DISP), None if costMap is None else pad(costMap, NO_ACCUMCOST), imageSize, H, Q,
+		subpixelSteps)
+
+
+def ImportDisparityDataRaw(fileName) -> dict:
+	"""-> dict(disparityMap (int16), costMap (uint16 or None: no bytes after the disparity map), imageSize, H (3x3), Q (4x4),
+	subpixelSteps) of a .dimap file (SemiGlobalMatcher::ImportDisparityDataRaw, SemiGlobalMatcher.cpp:2140-2172)"""
+	with open(fileName, "rb") as f:
+		raw = f.read()
+	if len(raw) < _DIMAP_HEAD.size:
+		raise ValueError("%s is too short for a disparity-data file" % fileName)
+	v = _DIMAP_HEAD.unpack_from(raw)
+	iw, ih, H, Q, steps, cols, rows = v[0], v[1], v[2:11], v[11:27], v[27], v[28], v[29]
+	if iw <= 0 or ih <= 0 or cols <= 0 or rows <= 0:
+		raise ValueError("invalid disparity-data header")
+	n = cols*rows
+	rest = raw[_DIMAP_HEAD.size:]
+	if len(rest) not in (2*n, 4*n):
+		raise ValueError("%s holds %d bytes of maps, expected %d or %d" % (fileName, len(rest), 2*n, 4*n))
+	disp = np.frombuffer(rest[:2*n], "<i2").reshape(rows, cols).astype(np.int16)
+	cost = np.frombuffer(rest[2*n:], "<u2").reshape(rows, cols).astype(np.uint16) if len(rest) == 4*n else None
+	return dict(disparityMap=disp, costMap=cost, imageSize=(iw, ih), H=np.array(H, np.float64).reshape(3, 3),
+		Q=np.array(Q, np.float64).reshape(4, 4), subpixelSteps=int(steps))
+
+
+def ImportDisparityDataRawFull(fileName) -> dict:
+	"""ImportDisparityDataRaw with the 3-pixel border cropped (SemiGlobalMatcher.cpp:2174-2184): the maps of the valid region"""
+	d = ImportDisparityDataRaw(fileName)
+	crop = lambda m: None if m is None else np.ascontiguousarray(m[3:-3, 3:-3])
+	if min(d["disparityMap"].shape) <= 6:
+		raise ValueError("a full disparity map must be larger than its 3-pixel border")
+	d["disparityMap"], d["costMap"] = crop(d["disparityMap"]), crop(d["costMap"])
+	return d
 
 
 class AsyncDepthDataWriter:

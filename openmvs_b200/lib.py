@@ -7,8 +7,9 @@ import os
 
 from . import build as _build
 
-ABI_VERSION = 6  # B200MVS_ABI_VERSION of include/b200mvs.h these structs mirror
+ABI_VERSION = 7  # B200MVS_ABI_VERSION of include/b200mvs.h these structs mirror
 SGM_MAX_LEVELS = 9  # B200MVS_SGM_MAX_LEVELS: entries of the level-size arrays of b200mvs_sgm_levels
+SGM_MAX_PAIRS = 32  # B200MVS_SGM_MAX_PAIRS: pairs one b200mvs_sgm_fuse call takes
 
 
 class View(C.Structure):
@@ -60,6 +61,12 @@ class SgmPixel(C.Structure):
 class SgmParams(C.Structure):
 	"""b200mvs_sgm_params"""
 	_fields_ = [("P1", C.c_int), ("P2", C.c_int), ("P2alpha", C.c_float), ("P2beta", C.c_float)]
+
+
+class SgmPair(C.Structure):
+	"""b200mvs_sgm_pair"""
+	_fields_ = [("disparity", C.c_void_p), ("cost", C.c_void_p), ("width", C.c_int), ("height", C.c_int), ("subpixelSteps", C.c_int),
+		("Q", C.c_double*16)]
 
 
 class DMap(C.Structure):
@@ -128,6 +135,11 @@ PROTOTYPES = {
 	"b200mvs_sgm_filter_speckles_device": (I, [P, P, I, I, I, I, I, P]),
 	"b200mvs_resize_area_u8_device": (I, [P, P, I, I, I, I, P, P]),
 	"b200mvs_sgm_level_mask_device": (I, [P, P, I, I, I, I, P, P]),
+	"b200mvs_sgm_pair_q": (I, [P, P, P, P, P, P, P, P]),
+	"b200mvs_sgm_project_disparity_device": (I, [P, P, I, I, P, P, P, P]),
+	"b200mvs_sgm_fuse_device": (I, [P, P, I, I, I, I, P, P, P, P, P]),
+	"b200mvs_sgm_fuse": (I, [P, P, I, I, I, I, P, P, P, P, PStats]),
+	"b200mvs_estimate_normal_map_device": (I, [P, P, I, I, P, P, P]),
 	"b200mvs_filter_default_params": (None, [C.POINTER(FilterParams)]),
 	"b200mvs_filter_depth_map": (I, [P, PDMap, PDMap, I, C.POINTER(FilterParams), F, F, P, P, IP, PStats]),
 	"b200mvs_filter_depth_map_device": (I, [P, PDMap, PDMap, I, C.POINTER(FilterParams), F, F, P, P, P, P, IP, P]),
@@ -174,7 +186,7 @@ def load(build_if_missing: bool = True):
 	for name, (restype, argtypes) in PROTOTYPES.items():
 		f = getattr(lib, name)
 		f.restype, f.argtypes = restype, argtypes
-	for what, T in enumerate((View, Params, Stats, Job, SgmPixel, SgmParams, DMap, FilterParams, Debug)):
+	for what, T in enumerate((View, Params, Stats, Job, SgmPixel, SgmParams, DMap, FilterParams, Debug, SgmPair)):
 		if lib.b200mvs_sizeof(what) != C.sizeof(T):
 			raise RuntimeError("struct %s: library %d bytes, bindings %d bytes" % (T.__name__, lib.b200mvs_sizeof(what), C.sizeof(T)))
 	_LIB = lib

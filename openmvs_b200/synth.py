@@ -76,6 +76,41 @@ def look_at(C, target=np.zeros(3)):
 	return np.stack([x, y, z])
 
 
+def _render(K, R, C, tex, xs, ys, xp):
+	"""ray cast of the height-field through the pixel centres (xs, ys) of camera (K, R, C) -> (image, depth, camera-space normal)"""
+	# rays in world space, parameterised so that t == camera-space depth: D = R^T K^-1 (x,y,1)
+	dx = (xs-K[0, 2])/K[0, 0]
+	dy = (ys-K[1, 2])/K[1, 1]
+	D = [dx*R[0, k] + dy*R[1, k] + R[2, k] for k in range(3)]
+	t = (0.0-C[2])/D[2]
+	for _ in range(12):
+		px = C[0]+t*D[0]
+		py = C[1]+t*D[1]
+		h, hx, hy = _height(px, py, xp)
+		F = C[2]+t*D[2]-h
+		dF = D[2]-(hx*D[0]+hy*D[1])
+		t = t-F/dF
+	px = C[0]+t*D[0]
+	py = C[1]+t*D[1]
+	h, hx, hy = _height(px, py, xp)
+	inv = 1.0/xp.sqrt(hx*hx + hy*hy + 1.0)
+	nw = [-hx*inv, -hy*inv, inv]
+	nc = xp.stack([nw[0]*R[k, 0] + nw[1]*R[k, 1] + nw[2]*R[k, 2] for k in range(3)], -1)
+	return tex(px, py, xp), t, nc
+
+
+def render_view(K, R, C, width: int, height: int, seed: int = 1234, px_per_unit: float | None = None, radius: float = 5.5) -> View:
+	"""The surface and texture of make_scene seen through any pinhole camera (K, R, C) at width x height: gray image, ground-truth
+	depth and normal, exact per pixel (no resampling).  The texture is make_scene's for the same seed and px_per_unit (make_scene uses
+	its focal length / radius; default here: K[0, 0] / radius).  Cameras that share R and K and differ by a shift along their x axis
+	give a rectified pair directly."""
+	K = np.asarray(K, np.float64); R = np.asarray(R, np.float64); C = np.asarray(C, np.float64)
+	tex = _Texture(seed, px_per_unit=(K[0, 0]/radius) if px_per_unit is None else px_per_unit)
+	ys, xs = np.mgrid[0:height, 0:width].astype(np.float64)
+	img, t, nc = _render(K, R, C, tex, xs, ys, np)
+	return View(img.astype(np.float32), K.copy(), R.copy(), C.copy(), t.astype(np.float32), nc.astype(np.float32))
+
+
 def make_scene(width: int, height: int, n_views: int, seed: int = 1234, radius: float = 5.5,
 		step_deg: float = 4.0, focal_ratio: float = 0.9, cols: int | None = None, device=None, gt_views=None) -> Scene:
 	"""n_views cameras on a (rows x cols) angular grid `step_deg` apart, radius `radius`.
@@ -102,25 +137,7 @@ def make_scene(width: int, height: int, n_views: int, seed: int = 1234, radius: 
 		ay = np.deg2rad(step_deg*(r-(rows-1)/2.0))
 		C = radius*np.array([np.sin(ax)*np.cos(ay), np.sin(ay), np.cos(ax)*np.cos(ay)])
 		R = look_at(C)
-		# rays in world space, parameterised so that t == camera-space depth: D = R^T K^-1 (x,y,1)
-		dx = (xs-K[0, 2])/K[0, 0]
-		dy = (ys-K[1, 2])/K[1, 1]
-		D = [dx*R[0, k] + dy*R[1, k] + R[2, k] for k in range(3)]
-		t = (0.0-C[2])/D[2]
-		for _ in range(12):
-			px = C[0]+t*D[0]
-			py = C[1]+t*D[1]
-			h, hx, hy = _height(px, py, xp)
-			F = C[2]+t*D[2]-h
-			dF = D[2]-(hx*D[0]+hy*D[1])
-			t = t-F/dF
-		px = C[0]+t*D[0]
-		py = C[1]+t*D[1]
-		h, hx, hy = _height(px, py, xp)
-		inv = 1.0/xp.sqrt(hx*hx + hy*hy + 1.0)
-		nw = [-hx*inv, -hy*inv, inv]
-		nc = xp.stack([nw[0]*R[k, 0] + nw[1]*R[k, 1] + nw[2]*R[k, 2] for k in range(3)], -1)
-		img = tex(px, py, xp)
+		img, t, nc = _render(K, R, C, tex, xs, ys, xp)
 		keep = gt_views is None or i in gt_views   # large scenes: ground truth only for the views that are checked (16 B per pixel)
 		if device is None:
 			views.append(View(img.astype(np.float32), K.copy(), R, C, t.astype(np.float32) if keep else None, nc.astype(np.float32) if keep else None))
