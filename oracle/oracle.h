@@ -139,6 +139,28 @@ int oracle_sgm_match(const float* leftGray, const uint8_t* leftBGR, const float*
 void oracle_sgm_cross_check(int16_t* l2r, const int16_t* r2l, int width, int height, int thCross);
 void oracle_sgm_refine(const oracle_sgm_pixel* pixels, const uint16_t* accums, int16_t* disparity, int nPixels, int subpixelSteps);
 
+/* ---- helpers of the hierarchical (tSGM) level loop of SemiGlobalMatcher::Match(scene, ...) (tsgm_oracle.cpp) ---- */
+/* Disparity2RangeMap: pixels of the mw x mh 2x grid from the cols x rows disparity map; returns numCosts */
+uint64_t oracle_tsgm_range_map(const int16_t* disparityMap, int cols, int rows, const uint8_t* maskMap, int mw, int mh,
+	int minNumDisp, int minNumDispInvalid, oracle_sgm_pixel* pixels);
+void oracle_tsgm_flip_direction(const int16_t* l2r, int16_t* r2l, int width, int height);
+void oracle_tsgm_upscale_mask(const uint8_t* maskMap, int width, int height, uint8_t* maskMap2x, int w2, int h2);
+void oracle_tsgm_extract_mask(const int16_t* disparityMap, uint8_t* maskMap, int width, int height, int thValid);
+
+/* ---- fusion-mode -2 (SemiGlobalMatcher::ProjectDisparity2DepthMap and ::Fuse, libs/MVS/SemiGlobalMatcher.cpp:1925-2039 and
+ * :739-859; sgm_fuse_oracle.cpp) ---- */
+/* ProjectDisparity2DepthMap of one pair into a W x H image: depth, range (2 floats per pixel), conf (nullable) -> numDepths */
+int oracle_sgmf_project(const int16_t* disparity, const uint16_t* cost, int vw, int vh, int steps, const double* Q, int W, int H,
+	float* depth, float* range, float* conf);
+/* the cluster vote of Fuse (:795-848) over nPairs projected maps (pair p at offset p x W x H; ranges 2 floats per pixel) */
+void oracle_sgmf_fuse(int nPairs, const float* depths, const float* ranges, const float* confs, int W, int H, unsigned minViews,
+	float* depth, float* conf);
+/* Q' = P invK Q of a reversed pair (:770-779) */
+void oracle_sgmf_pair_q(const double* Q, const double* Kl, const double* Rl, const double* Cl, const double* K, const double* R,
+	const double* C, double* Qout);
+/* EstimateNormalMap(Matrix3x3f(K), depth, normal) (libs/MVS/DepthMap.cpp:1522-1613); normal: 3 floats per pixel */
+void oracle_sgmf_normals(const float* D, int W, int H, const double* Kd, float* N);
+
 /* ---- depth-map post-processing (libs/MVS/SceneDensify.cpp:810-1299) ---- */
 /* one estimated depth-map with its camera (DepthData of a view: depthMap, confMap, images[0].camera) */
 typedef struct {

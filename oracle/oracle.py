@@ -6,16 +6,20 @@ import this module.  The product package openmvs_b200 never does.
 from __future__ import annotations
 
 import ctypes as C
+import glob
 import os
 import subprocess
 import tempfile
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
+# what the Makefile compiles (every .cpp of this directory) and the header they share
+_SOURCES = sorted(glob.glob(os.path.join(_HERE, "*.cpp"))) + [os.path.join(_HERE, "oracle.h")]
 _LIB = None
 
 
 class OView(C.Structure):
+	"""oracle_view"""
 	_fields_ = [("image", C.c_void_p), ("width", C.c_int), ("height", C.c_int),
 		("K", C.c_double*9), ("R", C.c_double*9), ("C", C.c_double*3),
 		("depth", C.c_void_p), ("dwidth", C.c_int), ("dheight", C.c_int),
@@ -23,6 +27,7 @@ class OView(C.Structure):
 
 
 class OParams(C.Structure):
+	"""oracle_params"""
 	_fields_ = [("nEstimationIters", C.c_int), ("nEstimationGeometricIters", C.c_int), ("nRandomIters", C.c_int),
 		("fNCCThresholdKeep", C.c_float), ("fDescriptorMinMagnitudeThreshold", C.c_float),
 		("fRandomDepthRatio", C.c_float), ("fRandomAngle1Range", C.c_float), ("fRandomAngle2Range", C.c_float),
@@ -31,10 +36,70 @@ class OParams(C.Structure):
 		("schedule", C.c_int), ("propagation", C.c_int), ("seed", C.c_uint32), ("threads", C.c_int)]
 
 
+class ODMap(C.Structure):
+	"""oracle_dmap"""
+	_fields_ = [("depth", C.c_void_p), ("conf", C.c_void_p), ("width", C.c_int), ("height", C.c_int),
+		("K", C.c_double*9), ("R", C.c_double*9), ("C", C.c_double*3)]
+
+
+NO_DISP = 32767  # invalid disparity (SemiGlobalMatcher::NO_DISP)
+# oracle_sgm_pixel
+SGM_PIXEL = np.dtype([("idx", "<u8"), ("dmin", "<i2"), ("dmax", "<i2"), ("reserved", "<i4")])
+
+I, U, F, D, P, U16, U64 = C.c_int, C.c_uint, C.c_float, C.c_double, C.c_void_p, C.c_uint16, C.c_uint64
+PView, PParams, PDMap = C.POINTER(OView), C.POINTER(OParams), C.POINTER(ODMap)
+
+# name -> (restype, argtypes) of every function oracle.h declares, in header order; arrays (also oracle_sgm_pixel records) are
+# c_void_p (checked against the header's prototypes by tests/test_oracle_binding.py)
+PROTOTYPES = {
+	"oracle_default_params": (None, [PParams]),
+	"oracle_philox4x32": (None, [P, P, P]),
+	"oracle_pm_score": (I, [PView, I, PParams, F, F, P, P, P, P]),
+	"oracle_pm_iterate": (I, [PView, I, PParams, F, F, P, I, I, P, P, P]),
+	"oracle_pm_iterate_flags": (I, [PView, I, PParams, F, F, P, I, I, P, P, P, P]),
+	"oracle_pm_finalize": (I, [I, I, F, P, P, P]),
+	"oracle_pm_estimate": (I, [PView, I, PParams, F, F, I, P, P, P]),
+	"oracle_pm_counters": (None, [P]),
+	"oracle_pm_estimate_range": (I, [PView, I, PParams, F, F, I, I, I, P, P, P, P]),
+	"oracle_pm_score_pixel": (F, [PView, I, PParams, F, F, P, I, I, F, P, P, I, P]),
+	"oracle_dir2normal": (None, [F, F, P]),
+	"oracle_normal2dir": (None, [P, P, P]),
+	"oracle_correct_normal": (None, [P, P]),
+	"oracle_interpolate_pixel": (F, [P, I, I, I, I, F, P, F, F]),
+	"oracle_zigzag": (None, [I, I, I, P]),
+	"oracle_resize_area": (None, [P, I, I, P, I, I, D, D]),
+	"oracle_resize_linear": (None, [P, I, I, P, I, I]),
+	"oracle_resize_nearest": (None, [P, I, I, I, P, I, I]),
+	"oracle_scale_K": (None, [P, I, I, I, I, P]),
+	"oracle_sgm_p2s": (None, [U16, F, F, P]),
+	"oracle_sgm_match": (I, [P, P, P, I, I, P, U64, U16, U16, F, F, I, P, P, P, P]),
+	"oracle_sgm_cross_check": (None, [P, P, I, I, I]),
+	"oracle_sgm_refine": (None, [P, P, P, I, I]),
+	"oracle_tsgm_range_map": (U64, [P, I, I, P, I, I, I, I, P]),
+	"oracle_tsgm_flip_direction": (None, [P, P, I, I]),
+	"oracle_tsgm_upscale_mask": (None, [P, I, I, P, I, I]),
+	"oracle_tsgm_extract_mask": (None, [P, P, I, I, I]),
+	"oracle_sgmf_project": (I, [P, P, I, I, I, P, I, I, P, P, P]),
+	"oracle_sgmf_fuse": (None, [I, P, P, P, I, I, U, P, P]),
+	"oracle_sgmf_pair_q": (None, [P]*8),
+	"oracle_sgmf_normals": (None, [P, I, I, P, P]),
+	"oracle_filter_project": (None, [PDMap, PDMap, P, P]),
+	"oracle_filter_depth_map": (I, [PDMap, PDMap, I, I, I, F, I, F, F, P, P, P]),
+	"oracle_remove_small_segments": (None, [P, P, P, I, I, F, U]),
+	"oracle_count_asymmetric_edges": (I, [P, I, I, F]),
+	"oracle_gap_interpolation": (None, [P, P, P, I, I, F, U]),
+	"oracle_to_gray": (None, [P, I, I, I, I, I, P]),
+}
+
+
+def _fresh(so: str) -> bool:
+	return os.path.exists(so) and all(os.path.getmtime(s) <= os.path.getmtime(so) for s in _SOURCES)
+
+
 def build(force: bool = False) -> str:
+	"""-> path of liboracle.so, (re)built in place by the Makefile when missing or older than a source"""
 	so = os.path.join(_HERE, "liboracle.so")
-	srcs = [os.path.join(_HERE, f) for f in ("pm_oracle.cpp", "sgm_oracle.cpp", "filter_oracle.cpp", "oracle.h")]
-	if force or not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs if os.path.exists(s)):
+	if force or not _fresh(so):
 		subprocess.check_call(["make", "-C", _HERE, "-s", "-B"])
 	return so
 
@@ -57,10 +122,7 @@ def build_fast() -> str:
 	os.makedirs(out, exist_ok=True)
 	so = os.path.join(out, "liboracle_fast.so")
 	tag = os.path.join(out, "liboracle_fast.cpu")
-	srcs = [os.path.join(_HERE, f) for f in ("pm_oracle.cpp", "sgm_oracle.cpp", "filter_oracle.cpp", "oracle.h")]
-	fresh = os.path.exists(so) and os.path.exists(tag) and open(tag).read() == _cpu_model() and all(
-		os.path.getmtime(s) <= os.path.getmtime(so) for s in srcs)
-	if not fresh:
+	if not (_fresh(so) and os.path.exists(tag) and open(tag).read() == _cpu_model()):
 		subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "liboracle_fast.so", "FAST_OUT=" + so])
 		open(tag, "w").write(_cpu_model())
 	return so
@@ -90,8 +152,9 @@ def lib():
 		key = "fast" if _FAST else "parity"
 		if key not in _LIBS:
 			L = C.CDLL(build_fast() if _FAST else build())
-			L.oracle_pm_score_pixel.restype = C.c_float
-			L.oracle_interpolate_pixel.restype = C.c_float
+			for name, (restype, argtypes) in PROTOTYPES.items():
+				f = getattr(L, name)
+				f.restype, f.argtypes = restype, argtypes
 			_LIBS[key] = L
 		_LIB = _LIBS[key]
 	return _LIB
@@ -241,10 +304,8 @@ def sgm_match(left_gray, left_bgr, right_gray, pixels, num_costs, P1=3, P2=4, al
 		c = np.array(costs, np.uint8, copy=True); st |= 8
 	a = np.zeros(num_costs, np.uint16)
 	disp = np.zeros((h-6, w-6), np.int16); cost = np.zeros((h-6, w-6), np.uint16)
-	f = lib().oracle_sgm_match
-	f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint64, C.c_uint16, C.c_uint16,
-		C.c_float, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-	rc = f(_fptr(lg), _fptr(lc), _fptr(rg), w, h, _fptr(px), num_costs, P1, P2, alpha, beta, st, _fptr(c), _fptr(a), _fptr(disp), _fptr(cost))
+	rc = lib().oracle_sgm_match(_fptr(lg), _fptr(lc), _fptr(rg), w, h, _fptr(px), num_costs, P1, P2, alpha, beta, st, _fptr(c), _fptr(a),
+		_fptr(disp), _fptr(cost))
 	assert rc == 0
 	return c, a, disp, cost
 
@@ -263,11 +324,6 @@ def sgm_refine(pixels, accums, disparity, steps=4):
 
 
 # ---- depth-map post-processing (filter_oracle.cpp) ----
-class ODMap(C.Structure):
-	_fields_ = [("depth", C.c_void_p), ("conf", C.c_void_p), ("width", C.c_int), ("height", C.c_int),
-		("K", C.c_double*9), ("R", C.c_double*9), ("C", C.c_double*3)]
-
-
 def make_dmaps(maps):
 	"""maps: list of (depth HxW, conf HxW or None, K, R, C) -> (ctypes array, keepalive)"""
 	arr = (ODMap*len(maps))()

@@ -8,6 +8,7 @@
 //  - a pixel whose agreeing entries have total weight 0 (0/0 in the reference) gets depth 0;
 //  - a source whose projected position puts its 3x3 block outside the image is skipped before the float -> int conversion (the
 //    reference writes nothing for it either, but converts the position first, which is undefined for huge values).
+#include "oracle.h"
 #include <cfloat>
 #include <cmath>
 #include <cstdint>
@@ -46,7 +47,6 @@ bool depth_similar(float d0, float d1, float th) { return std::fabs(d0-d1)/d0 < 
 
 extern "C" {
 
-// ProjectDisparity2DepthMap of one pair into a W x H image: depth, range (2 floats per pixel), conf (nullable) -> numDepths
 int oracle_sgmf_project(const int16_t* disparity, const uint16_t* cost, int vw, int vh, int steps, const double* Q, int W, int H,
 	float* depth, float* range, float* conf)
 {
@@ -116,7 +116,6 @@ int oracle_sgmf_project(const int16_t* disparity, const uint16_t* cost, int vw, 
 	return numDepths;
 }
 
-// the cluster vote of Fuse (:795-848) over nPairs projected maps (pair p at offset p x W x H; ranges 2 floats per pixel)
 void oracle_sgmf_fuse(int nPairs, const float* depths, const float* ranges, const float* confs, int W, int H, unsigned minViews,
 	float* depth, float* conf)
 {
@@ -153,7 +152,6 @@ void oracle_sgmf_fuse(int nPairs, const float* depths, const float* ranges, cons
 	}
 }
 
-// Q' = P invK Q of a reversed pair (:770-779)
 void oracle_sgmf_pair_q(const double* Q, const double* Kl, const double* Rl, const double* Cl, const double* K, const double* R,
 	const double* C, double* Qout)
 {
@@ -175,7 +173,6 @@ void oracle_sgmf_pair_q(const double* Q, const double* Kl, const double* Rl, con
 	std::memcpy(Qout, O, sizeof(O));
 }
 
-// EstimateNormalMap(Matrix3x3f(K), depth, normal); normal: 3 floats per pixel
 void oracle_sgmf_normals(const float* D, int W, int H, const double* Kd, float* N) {
 	const float fx = (float)Kd[0], fy = (float)Kd[4], cx = (float)Kd[2], cy = (float)Kd[5];
 	for (int r = 0; r < H; ++r) {

@@ -1,92 +1,42 @@
 """ctypes binding of tsgm_oracle.cpp and the level loop of the hierarchical (tSGM) pair matcher (TEST INFRASTRUCTURE, like
 oracle.py: only tests/ and scripts may import it; the product package openmvs_b200 never does).
 
-tsgm_oracle.cpp restates the reference's Disparity2RangeMap, FlipDirection, UpscaleMask and ExtractMask.  It is built into a
-library of its own (the parity flags of the main oracle build), next to this file when the tree is writable, else in a per-user
-temporary directory.  tsgm_match composes the whole loop from these helpers, oracle.py's sgm_match / sgm_cross_check /
-sgm_refine, and OpenCV (cv2) for the pyramid, the mask resize and filterSpeckles.
+tsgm_oracle.cpp (part of liboracle.so) restates the reference's Disparity2RangeMap, FlipDirection, UpscaleMask and ExtractMask.
+tsgm_match composes the whole loop from these helpers, oracle.py's sgm_match / sgm_cross_check / sgm_refine, and OpenCV (cv2) for
+the pyramid, the mask resize and filterSpeckles.
 """
 from __future__ import annotations
-
-import ctypes as C
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 from . import oracle as O
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRCS = [os.path.join(_HERE, f) for f in ("tsgm_oracle.cpp", "oracle.h")]
-_CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unused-function", "-shared"]
-_LIB = None
-
-
-def _fresh(so: str) -> bool:
-	return os.path.exists(so) and all(os.path.getmtime(s) <= os.path.getmtime(so) for s in _SRCS)
-
-
-def build(force: bool = False) -> str:
-	"""-> path of libtsgm_oracle.so, (re)built with g++ when missing or older than its sources"""
-	for out in (_HERE, os.path.join(tempfile.gettempdir(), "openmvs_b200_tsgm_oracle_%d" % os.getuid())):
-		so = os.path.join(out, "libtsgm_oracle.so")
-		if not force and _fresh(so):
-			return so
-		# build to a temporary name and rename: a concurrent process never loads a half-written library
-		tmp = "%s.tmp.%d" % (so, os.getpid())
-		try:
-			os.makedirs(out, exist_ok=True)
-			subprocess.check_call([os.environ.get("CXX", "g++")] + _CXXFLAGS + ["-o", tmp, _SRCS[0]])
-			os.replace(tmp, so)
-			return so
-		except (OSError, subprocess.CalledProcessError):
-			if out != _HERE:
-				raise
-		finally:
-			if os.path.exists(tmp):
-				os.unlink(tmp)
-	raise RuntimeError("libtsgm_oracle.so could not be built")
-
-
-def lib():
-	global _LIB
-	if _LIB is None:
-		L = C.CDLL(build())
-		L.oracle_tsgm_range_map.restype = C.c_uint64
-		L.oracle_tsgm_range_map.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
-		_LIB = L
-	return _LIB
-
-
-NO_DISP = 32767
-SGM_PIXEL = np.dtype([("idx", "<u8"), ("dmin", "<i2"), ("dmax", "<i2"), ("reserved", "<i4")])
+from .oracle import NO_DISP, SGM_PIXEL
 
 
 def tsgm_range_map(disparity, mask, minNumDisp, minNumDispInvalid):
 	"""Disparity2RangeMap -> (pixel records of the mask's 2x grid, numCosts)"""
 	d = np.ascontiguousarray(disparity, np.int16); m = np.ascontiguousarray(mask, np.uint8)
 	px = np.zeros(m.size, SGM_PIXEL)
-	n = lib().oracle_tsgm_range_map(O._fptr(d), d.shape[1], d.shape[0], O._fptr(m), m.shape[1], m.shape[0], int(minNumDisp),
+	n = O.lib().oracle_tsgm_range_map(O._fptr(d), d.shape[1], d.shape[0], O._fptr(m), m.shape[1], m.shape[0], int(minNumDisp),
 		int(minNumDispInvalid), O._fptr(px))
 	return px, int(n)
 
 
 def tsgm_flip_direction(l2r):
 	a = np.ascontiguousarray(l2r, np.int16); out = np.zeros_like(a)
-	lib().oracle_tsgm_flip_direction(O._fptr(a), O._fptr(out), a.shape[1], a.shape[0])
+	O.lib().oracle_tsgm_flip_direction(O._fptr(a), O._fptr(out), a.shape[1], a.shape[0])
 	return out
 
 
 def tsgm_upscale_mask(mask, size2x):
 	m = np.ascontiguousarray(mask, np.uint8); out = np.zeros((size2x[1], size2x[0]), np.uint8)
-	lib().oracle_tsgm_upscale_mask(O._fptr(m), m.shape[1], m.shape[0], O._fptr(out), int(size2x[0]), int(size2x[1]))
+	O.lib().oracle_tsgm_upscale_mask(O._fptr(m), m.shape[1], m.shape[0], O._fptr(out), int(size2x[0]), int(size2x[1]))
 	return out
 
 
 def tsgm_extract_mask(disparity, mask, thValid=3):
 	d = np.ascontiguousarray(disparity, np.int16); m = np.array(mask, np.uint8, copy=True, order="C")
-	lib().oracle_tsgm_extract_mask(O._fptr(d), O._fptr(m), d.shape[1], d.shape[0], int(thValid))
+	O.lib().oracle_tsgm_extract_mask(O._fptr(d), O._fptr(m), d.shape[1], d.shape[0], int(thValid))
 	return m
 
 

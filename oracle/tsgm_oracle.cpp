@@ -1,18 +1,9 @@
 // tsgm_oracle.cpp — CPU restatement of the helpers of the hierarchical (tSGM) level loop of
 // SemiGlobalMatcher::Match(scene, ...) (TEST INFRASTRUCTURE, see oracle.h).  Sequential, in the reference's loop order.
-// Built into a library of its own by oracle/tsgm.py, which also binds it.
+// Part of liboracle.so; oracle/tsgm.py binds it.
 #include "oracle.h"
 #include <algorithm>
 #include <vector>
-
-extern "C" {
-/* Disparity2RangeMap: pixels of the mw x mh 2x grid from the cols x rows disparity map; returns numCosts */
-uint64_t oracle_tsgm_range_map(const int16_t* disparityMap, int cols, int rows, const uint8_t* maskMap, int mw, int mh,
-	int minNumDisp, int minNumDispInvalid, oracle_sgm_pixel* pixels);
-void oracle_tsgm_flip_direction(const int16_t* l2r, int16_t* r2l, int width, int height);
-void oracle_tsgm_upscale_mask(const uint8_t* maskMap, int width, int height, uint8_t* maskMap2x, int w2, int h2);
-void oracle_tsgm_extract_mask(const int16_t* disparityMap, uint8_t* maskMap, int width, int height, int thValid);
-}
 
 namespace {
 typedef int16_t Disparity;

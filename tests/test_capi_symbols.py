@@ -7,15 +7,85 @@ import re
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADER = os.path.join(ROOT, "include", "b200mvs.h")
 
 
-def _header():
-	"""include/b200mvs.h without comments"""
-	return re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "b200mvs.h")).read(), flags=re.S)
+def _header(path=HEADER):
+	"""a C header without comments"""
+	return re.sub(r"/\*.*?\*/", "", open(path).read(), flags=re.S)
 
 
 def _declared():
 	return sorted(set(re.findall(r"\b(b200mvs_[a-z_0-9]+)\s*\(", _header())))
+
+
+def _layout(mirror):
+	"""(size, [(field, offset), ...]) of a ctypes Structure or of a numpy structured dtype"""
+	if isinstance(mirror, type):
+		return C.sizeof(mirror), [(f[0], getattr(mirror, f[0]).offset) for f in mirror._fields_]
+	return mirror.itemsize, [(f, mirror.fields[f][1]) for f in mirror.names]
+
+
+def check_struct_layouts(tmp_path, header, mirrors):
+	"""sizeof / offsetof of every struct of `header` as gcc sees them == its mirror (struct name -> ctypes Structure or numpy
+	structured dtype).  -> gcc's numbers, {"struct": size, "struct.field": offset}"""
+	import subprocess
+	lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "%s"' % os.path.basename(header), 'int main(void) {']
+	for cname, m in mirrors.items():
+		lines.append('printf("%s %%zu\\n", sizeof(%s));' % (cname, cname))
+		for fname, _ in _layout(m)[1]:
+			lines.append('printf("%s.%s %%zu\\n", offsetof(%s, %s));' % (cname, fname, cname, fname))
+	lines.append('return 0; }')
+	src = tmp_path/"layout.c"
+	src.write_text("\n".join(lines))
+	exe = str(tmp_path/"layout")
+	subprocess.check_call(["gcc", "-std=c99", "-I", os.path.dirname(header), "-o", exe, str(src)])
+	got = dict(l.split() for l in subprocess.check_output([exe], text=True).splitlines())
+	for cname, m in mirrors.items():
+		size, fields = _layout(m)
+		assert int(got[cname]) == size, cname
+		for fname, offset in fields:
+			assert int(got["%s.%s" % (cname, fname)]) == offset, (cname, fname)
+	return {k: int(v) for k, v in got.items()}
+
+
+def check_prototypes(header, prefix, prototypes, mirrors):
+	"""Every entry of `prototypes` (name -> (restype, argtypes), a ctypes binding's table) has the arity, argument types and return
+	type of its prototype in `header`, one entry per function named `prefix`..., in header order.  mirrors: every struct the header
+	defines -> its ctypes Structure (or the numpy dtype of records passed as arrays).  ctypes passes a wrongly declared argument as
+	garbage without any error."""
+	src = re.sub(r"^\s*#.*$", "", _header(header), flags=re.M)
+	protos = re.findall(r"([\w\s*]+?)\b(%s\w+)\s*\(([^()]*)\)\s*;" % prefix, src)
+	assert [name for _, name, _ in protos] == list(prototypes)  # one entry per prototype, in header order
+	assert set(re.findall(r"}\s*(%s\w+)\s*;" % prefix, src)) == set(mirrors)
+	scalars = {"int": C.c_int, "unsigned": C.c_uint, "float": C.c_float, "double": C.c_double, "long long": C.c_longlong,
+		"uint64_t": C.c_uint64, "size_t": C.c_size_t, "uint8_t": C.c_uint8, "int16_t": C.c_int16, "uint16_t": C.c_uint16,
+		"uint32_t": C.c_uint32}
+
+	def allowed(words):
+		"""ctypes types that pass the C type `words` (tokens without const and the parameter name) correctly"""
+		stars = words.count("*")
+		base = " ".join(w for w in words if w != "*")
+		if stars == 0:
+			return [None] if base == "void" else [scalars[base]]
+		if stars > 1:
+			return [C.POINTER(C.c_void_p)]
+		if base == "char":
+			return [C.c_char_p]
+		if base in mirrors:
+			return ([C.POINTER(mirrors[base])] if isinstance(mirrors[base], type) else []) + [C.c_void_p]
+		return [C.c_void_p] + ([C.POINTER(scalars[base])] if base in scalars else [])
+
+	tokens = lambda decl: [w for w in decl.replace("*", " * ").split() if w != "const"]
+	# a parameter without its name; an array parameter (`float n[3]`) is the pointer it decays to
+	param = lambda decl: tokens(decl)[:-1] + (["*"] if "[" in tokens(decl)[-1] else [])
+	for ret, name, params in protos:
+		restype, argtypes = prototypes[name]
+		assert restype in allowed(tokens(ret)), (name, ret.strip())
+		params = [] if params.strip() == "void" else [param(p) for p in params.split(",")]
+		assert len(argtypes) == len(params), name
+		for k, (words, t) in enumerate(zip(params, argtypes)):
+			assert t in allowed(words), (name, k, " ".join(words))
 
 
 def _mirrors():
@@ -49,60 +119,15 @@ def test_struct_layouts_match_header_sizes():
 
 def test_struct_layouts_match_a_c_compiler(tmp_path):
 	"""sizeof / offsetof of every struct of include/b200mvs.h as gcc sees them == the ctypes mirrors in openmvs_b200/lib.py"""
-	import subprocess
-	structs = _mirrors()
-	lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "b200mvs.h"', 'int main(void) {']
-	for cname, ct in structs.items():
-		lines.append('printf("%s %%zu\\n", sizeof(%s));' % (cname, cname))
-		for fname, _ in ct._fields_:
-			lines.append('printf("%s.%s %%zu\\n", offsetof(%s, %s));' % (cname, fname, cname, fname))
-	lines += ['printf("b200mvs_sgm_pixel %zu\\n", sizeof(b200mvs_sgm_pixel));', 'return 0; }']
-	src = tmp_path/"layout.c"
-	src.write_text("\n".join(lines))
-	exe = str(tmp_path/"layout")
-	subprocess.check_call(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), "-o", exe, str(src)])
-	got = dict(l.split() for l in subprocess.check_output([exe], text=True).splitlines())
-	for cname, ct in structs.items():
-		assert int(got[cname]) == C.sizeof(ct), cname
-		for fname, _ in ct._fields_:
-			assert int(got["%s.%s" % (cname, fname)]) == getattr(ct, fname).offset, (cname, fname)
-	assert int(got["b200mvs_sgm_pixel"]) == 16  # SemiGlobalMatcher::PixelData
+	got = check_struct_layouts(tmp_path, HEADER, _mirrors())
+	assert got["b200mvs_sgm_pixel"] == 16  # SemiGlobalMatcher::PixelData
 
 
 def test_binding_prototypes_match_the_header():
-	"""Every entry of lib.PROTOTYPES has the arity, argument types and return type of its prototype in include/b200mvs.h:
-	ctypes passes a wrongly declared argument as garbage without any error."""
+	"""Every entry of lib.PROTOTYPES has the arity, argument types and return type of its prototype in include/b200mvs.h"""
 	from openmvs_b200 import lib
-	src = re.sub(r"^\s*#.*$", "", _header(), flags=re.M)
-	protos = re.findall(r"([\w\s*]+?)\b(b200mvs_\w+)\s*\(([^()]*)\)\s*;", src)
-	assert [name for _, name, _ in protos] == lib.SYMBOLS  # one entry per prototype, in header order
-	mirrors = _mirrors()
-	assert set(re.findall(r"}\s*(b200mvs_\w+)\s*;", src)) == set(mirrors)
-	scalars = {"int": C.c_int, "unsigned": C.c_uint, "float": C.c_float, "uint64_t": C.c_uint64, "size_t": C.c_size_t,
-		"uint8_t": C.c_uint8, "int16_t": C.c_int16, "uint16_t": C.c_uint16, "uint32_t": C.c_uint32}
-
-	def allowed(words):
-		"""ctypes types that pass the C type `words` (tokens without const and the parameter name) correctly"""
-		stars = words.count("*")
-		base, = [w for w in words if w != "*"]
-		if stars == 0:
-			return [None] if base == "void" else [scalars[base]]
-		if stars > 1:
-			return [C.POINTER(C.c_void_p)]
-		if base == "char":
-			return [C.c_char_p]
-		if base in mirrors:
-			return [C.POINTER(mirrors[base]), C.c_void_p]
-		return [C.c_void_p] + ([C.POINTER(scalars[base])] if base in scalars else [])
-
-	tokens = lambda decl: [w for w in decl.replace("*", " * ").split() if w != "const"]
-	for ret, name, params in protos:
-		restype, argtypes = lib.PROTOTYPES[name]
-		assert restype in allowed(tokens(ret)), (name, ret.strip())
-		params = [] if params.strip() == "void" else [tokens(p)[:-1] for p in params.split(",")]
-		assert len(argtypes) == len(params), name
-		for k, (words, t) in enumerate(zip(params, argtypes)):
-			assert t in allowed(words), (name, k, " ".join(words))
+	assert lib.SYMBOLS == list(lib.PROTOTYPES)
+	check_prototypes(HEADER, "b200mvs_", lib.PROTOTYPES, _mirrors())
 
 
 def test_binding_constants_match_the_header():
