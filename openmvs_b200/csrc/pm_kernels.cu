@@ -23,6 +23,7 @@ constexpr int BLOCK_X = 32;  // lanes: 32 same-colour pixels = 64-pixel span
 constexpr int BLOCK_Y = 8;
 
 constexpr int NTHREADS = BLOCK_X*BLOCK_Y;
+static_assert(BLOCK_X == 32, "pm_sweep_kernel: a warp is one row of the CTA");
 
 // bilateral weights of the 5x5 reference patch (WeightedPatchFix<25>, DepthMap.h:145-155), kept in shared
 // memory as float2{w,tw}[tap][thread] (conflict-free LDS.64): 50 registers per thread less than a register copy
@@ -478,18 +479,22 @@ pm_score_kernel(const __grid_constant__ PMParams P)
 //   2. test the candidates' planes (InterpolatePixel + CorrectNormal), skipping a direction whose candidates
 //      all kept their plane in their last update (they lost against this pixel one sweep ago) — P.skipUnchanged;
 //   3. the refinement state machine (DepthMap.cpp:800-852).
-// Every lane keeps its own to-do list of directions, so a warp runs max-over-lanes(list length) test steps.
+// Every lane keeps its own to-do list of directions; the warp scores the lists of its 32 pixels as one packed list, so it
+// runs ceil(sum of list lengths / 32) test steps instead of max-over-lanes(list length).
 // 3 CTAs per SM: 80 registers without spills (a 64-register, 4-CTA build spills and measured slower, DESIGN.md §5.1)
 template <bool GEOM>
 __global__ void __launch_bounds__(BLOCK_X*BLOCK_Y, 3)
 pm_sweep_kernel(const __grid_constant__ PMParams P, const __grid_constant__ CUtensorMap tmapRef)
 {
 	extern __shared__ __align__(128) unsigned char smemRaw[];
-	// [ patch weights | mbarrier ]; the reference tile occupies the start of the weights until the weights are
-	// written (fill_patch): 4.6 KB less shared memory per CTA, which the SM's L1/shared array gives to L1
+	// [ patch weights | {sumW, normSq0} per thread | mbarrier ]; the reference tile occupies the start of the weights
+	// until the weights are written (fill_patch): 4.6 KB less shared memory per CTA, which the SM's L1/shared array gives
+	// to L1.  A lane scores hypotheses of other pixels of its row (propagation candidates), so a pixel's patch statistics
+	// live in shared memory beside its weights.
 	float2* smemW = (float2*)smemRaw;
 	float* tile = (float*)smemRaw;
-	uint64_t* bar = (uint64_t*)(smemRaw + PM_TEXELS*NTHREADS*sizeof(float2));
+	float2* smemStats = (float2*)(smemRaw + PM_TEXELS*NTHREADS*sizeof(float2));
+	uint64_t* bar = (uint64_t*)(smemStats + NTHREADS);
 	const int tid = threadIdx.y*BLOCK_X + threadIdx.x;
 	if (tid == 0) {
 		mbar_init(bar, 1);
@@ -502,19 +507,24 @@ pm_sweep_kernel(const __grid_constant__ PMParams P, const __grid_constant__ CUte
 	}
 	mbar_wait(bar, 0);
 	const int y = blockIdx.y*BLOCK_Y + threadIdx.y;
-	const int x = blockIdx.x*(2*BLOCK_X) + 2*threadIdx.x + ((y+P.colour)&1);
+	const int lane = threadIdx.x;  // BLOCK_X == 32: a warp is one row of the CTA
+	const int x0 = blockIdx.x*(2*BLOCK_X) + ((y+P.colour)&1);  // x of lane l: x0 + 2*l
+	const int x = x0 + 2*lane;
 	const bool active = pixel_active(P, x, y);
 	const int W = P.W, H = P.H;
 	const size_t idx = (size_t)y*W + x;
-	PatchW pt;
-	pt.s = smemW + tid;
-	fill_patch<true>(TileTexels{tile, 2*(int)threadIdx.x + ((y+P.colour)&1) + PM_HALF, (int)threadIdx.y + PM_HALF}, pt);
+	{
+		PatchW pt;
+		pt.s = smemW + tid;
+		fill_patch<true>(TileTexels{tile, 2*lane + ((y+P.colour)&1) + PM_HALF, (int)threadIdx.y + PM_HALF}, pt);
+		smemStats[tid] = make_float2(pt.sumW, pt.normSq0);
+	}
+	__syncwarp(); // the other lanes of the row read this pixel's weights and statistics
+	// A lane whose pixel is not estimated stays in the loop below without hypotheses of its own, so that the warp's
+	// shuffles always have all 32 lanes and the packed list maps onto every lane
 	float priorD, priorF;
-	if (!active || !pixel_prior(P, idx, pt.normSq0, priorD, priorF))
-		return;
-	const float fx = float(x), fy = float(y);
-	const float2 X0 = pixel_ray(P, fx, fy);
-	const float X0x = X0.x, X0y = X0.y;
+	const bool live = active && pixel_prior(P, idx, smemStats[tid].y, priorD, priorF);
+	const float fy = float(y);
 
 	// neighbours: causal pair of the sweep direction first (DepthMap.cpp:641-766)
 	const int dir = P.sweep & 1;
@@ -523,7 +533,7 @@ pm_sweep_kernel(const __grid_constant__ PMParams P, const __grid_constant__ CUte
 	unsigned todo = 0;    // bit k: direction k has a candidate to test
 	unsigned farSel = 0;  // 2 bits per direction: ring of the candidate (distance 2*ring+1)
 	#pragma unroll
-	for (int k = 0; k < 4; ++k) {
+	for (int k = 0; k < 4 && live; ++k) {
 		const int kk = dir ? (k^2) : k;
 		int ox, oy;
 		close_offset(dir, k, ox, oy);
@@ -555,59 +565,94 @@ pm_sweep_kernel(const __grid_constant__ PMParams P, const __grid_constant__ CUte
 			}
 		}
 	}
-	float depth, conf = fabsf(P.cost[idx]);
-	float3 normal;
-	{
+	const unsigned nOwn = __popc(todo);               // this pixel's propagation candidates
+	const unsigned info = todo | farSel<<4 | closeMask<<12;
+	float depth = 0.f, conf = 0.f;
+	float3 normal = make_float3(0.f, 0.f, 0.f);
+	uint32_t bestViews = 0xFFFFFFFFu;
+	if (live) {
 		const float4 pl = P.plane[idx];
 		depth = pl.w; normal = make_float3(pl.x, pl.y, pl.z);
+		conf = fabsf(P.cost[idx]);
+		if (P.bestViews) bestViews = P.bestViews[idx];
 	}
-	uint32_t bestViews = P.bestViews ? P.bestViews[idx] : 0xFFFFFFFFu;
+
+	// The warp's propagation candidates as one list: lane after lane, each lane's in __ffs order.  The bits of the
+	// candidate counts (0-4) as three ballots give every lane the prefix sum of any lane: listed(m) = candidates of
+	// the lanes in mask m.  Packed step s scores list entries 32s .. 32s+31, entry 32s+l on lane l, for the pixel that
+	// owns it; so the candidate phase takes ceil(total/32) steps instead of the largest count of a lane.
+	const unsigned c0 = __ballot_sync(0xFFFFFFFFu, nOwn & 1u), c1 = __ballot_sync(0xFFFFFFFFu, nOwn & 2u), c2 = __ballot_sync(0xFFFFFFFFu, nOwn & 4u);
+	const auto listed = [&](unsigned m) { return __popc(c0 & m) + 2*__popc(c1 & m) + 4*__popc(c2 & m); };
+	const int nList = listed(0xFFFFFFFFu);
 
 	// ---- propagation (DepthMap.cpp:775-799), then the refinement state machine (DepthMap.cpp:800-852) ----
-	// One loop and one copy of the scoring code for both: a lane first pops its propagation candidates, then runs its
-	// refinement tries; lanes with fewer candidates start refining while the others still propagate.  Per pixel the order is
-	// the reference's (candidates, then tries), and every try has its own Philox slot (restart try k: slot k, refinement try
-	// k: slot nR+k), so the result does not depend on the step at which a lane executes it.
+	// One loop and one copy of the scoring code for both: the packed candidate steps, then every lane runs its own
+	// refinement tries.  A candidate's plane comes from a pixel of the other colour and its hypothesis depends only on
+	// the owner pixel, so any lane can score it; the owner then takes the scores in its candidate order (conf > nconf),
+	// as the reference does.  Every try has its own Philox slot (restart try k: slot k, refinement try k: slot nR+k).
 	// evalCap > 0 (engine schedule, b200mvs_params.nEvalCap): a pixel that tests c candidates spends at most
 	// max(1, evalCap - c) tries of each kind — pixels whose four directions all changed give up their finest perturbation.
 	const int nR = P.nRandomIters;
-	const int nRl = P.evalCap > 0 ? min(nR, max(P.evalCap-__popc(todo), 1)) : nR;
+	// (the pixel's own count, listed(1u<<lane), and nRl are recomputed where they are used: 80 registers without spills)
+	const auto nRl = [&]() { return P.evalCap > 0 ? min(nR, max(P.evalCap-listed(1u<<lane), 1)) : nR; };
 	const uint2 key = make_uint2(P.seed, 0xB200C0DEu);
+	const uint32_t pix = (uint32_t)idx; // Philox counter
 	const uint32_t phase = 1u + (uint32_t)P.sweep;
-	int mode = 0;               // 0 undecided, 1 restart (fully random), 2 refine, 3 done
-	bool entered = false;       // the state machine has taken its first decision
+	int mode = live ? 0 : 3;    // 0 undecided, 1 restart (fully random), 2 refine, 3 done
+	bool entered = !live;       // the state machine has taken its first decision
 	bool useClose = true;
 	unsigned idxScale = 0;
-	float scaleRange = 1.f, depthRange = 0.f, pa = 0.f, pb = 0.f;
-	int nRestart = 0, nRefine = 0; // tries spent
+	float depthRange = 0.f, pa = 0.f, pb = 0.f;
+	int nTry = 0; // tries spent in the current mode (restart or refine)
 	#pragma unroll 1
-	for (;;) {
-		bool have = false, isRefine = false, alive = false, uc = true;
+	for (int step = 0;; ++step) {
+		const bool packed = 32*step < nList; // warp-uniform
+		bool have = false, isRefine = false, alive = packed, uc = true;
 		float hd = 0.f, na = 0.f, nb = 0.f; float3 hn = make_float3(0.f, 0.f, 1.f);
-		if (todo != 0u) {
-			const int k = __ffs((int)todo)-1;
-			todo &= todo-1u;
-			const int kk = dir ? (k^2) : k;
-			const int dist = 2*(int)((farSel>>(2*k))&3u)+1;
-			const int qx = x + ((kk == 0) ? -dist : (kk == 2) ? dist : 0);
-			const int qy = y + ((kk == 1) ? -dist : (kk == 3) ? dist : 0);
-			const float4 qp = P.plane[(size_t)qy*W + qx];
-			// InterpolatePixel (DepthMap.cpp:915-959): the candidate's plane intersected with this pixel's ray,
-			// restricted to the row / column; the reference's ray coordinates carry no skew term
-			const bool vertical = (kk & 1) != 0;
-			const float ncomp = vertical ? qp.y : qp.x;
-			const float nx1 = vertical ? X0y : fmaf(fx, P.ifx, P.ox0);
-			const float x1 = vertical ? fmaf(float(qy), P.ify, P.oy) : fmaf(float(qx), P.ifx, P.ox0);
-			const float denom = qp.z + nx1*ncomp;
-			hd = qp.w;
-			if (!(fabsf(denom) < 0.0001f)) {
-				const float dn = qp.w*(qp.z + x1*ncomp)/denom;
-				if (P.dMin <= dn && dn < P.dMax)
-					hd = dn;
+		int owner = lane, k = 0;  // the hypothesis is for the pixel of lane `owner`
+		if (packed) {
+			const int j = 32*step + lane;
+			have = j < nList;
+			if (have) {
+				// owner: the lane whose candidates end after entry j (listed() of lanes 0..m grows with m)
+				owner = 0;
+				#pragma unroll
+				for (int b = 16; b > 0; b >>= 1)
+					if (listed((2u<<(owner+b-1))-1u) <= j) owner += b;
+				k = j - listed((1u<<owner)-1u); // the owner's k-th candidate
 			}
-			hn = make_float3(qp.x, qp.y, qp.z);
-			correct_normal(hn, X0x, X0y);
-			have = true; alive = true;
+		}
+		const unsigned oinfo = __shfl_sync(0xFFFFFFFFu, info, owner);
+		const int sx = x0 + 2*owner;
+		const float sfx = float(sx);
+		const float2 X0 = pixel_ray(P, sfx, fy);
+		const float X0x = X0.x, X0y = X0.y;
+		if (packed) {
+			if (have) {
+				unsigned t = oinfo & 15u;
+				for (int i = 0; i < k; ++i) t &= t-1u;
+				const int d4 = __ffs((int)t)-1;
+				const int kk = dir ? (d4^2) : d4;
+				const int dist = 2*(int)((oinfo>>(4+2*d4))&3u)+1;
+				const int qx = sx + ((kk == 0) ? -dist : (kk == 2) ? dist : 0);
+				const int qy = y + ((kk == 1) ? -dist : (kk == 3) ? dist : 0);
+				const float4 qp = P.plane[(size_t)qy*W + qx];
+				// InterpolatePixel (DepthMap.cpp:915-959): the candidate's plane intersected with this pixel's ray,
+				// restricted to the row / column; the reference's ray coordinates carry no skew term
+				const bool vertical = (kk & 1) != 0;
+				const float ncomp = vertical ? qp.y : qp.x;
+				const float nx1 = vertical ? X0y : fmaf(sfx, P.ifx, P.ox0);
+				const float x1 = vertical ? fmaf(float(qy), P.ify, P.oy) : fmaf(float(qx), P.ifx, P.ox0);
+				const float denom = qp.z + nx1*ncomp;
+				hd = qp.w;
+				if (!(fabsf(denom) < 0.0001f)) {
+					const float dn = qp.w*(qp.z + x1*ncomp)/denom;
+					if (P.dMin <= dn && dn < P.dMax)
+						hd = dn;
+				}
+				hn = make_float3(qp.x, qp.y, qp.z);
+				correct_normal(hn, X0x, X0y);
+			}
 		} else {
 			if (!entered || (mode == 1 && conf < P.thConfRand)) {
 				// RefineIters: choose the perturbation scale from the current score
@@ -618,27 +663,28 @@ pm_sweep_kernel(const __grid_constant__ PMParams P, const __grid_constant__ CUte
 				else if (conf >= P.thConfRand && mode == 0) { mode = 1; useClose = false; toRefine = false; }
 				if (toRefine) {
 					mode = 2;
-					scaleRange = pow2neg(idxScale);
+					nTry = 0;
 					depthRange = depth*P.depthRatio;
 					pa = atan2f(normal.y, normal.x);
 					pb = acosf(normal.z);
 				}
 			}
-			if (mode == 1 && nRestart >= nRl) mode = 3; // all random tries failed: no refinement this sweep
-			alive = (mode == 1) || (mode == 2 && nRefine < nRl);
+			if (mode == 1 && nTry >= nRl()) mode = 3; // all random tries failed: no refinement this sweep
+			alive = (mode == 1) || (mode == 2 && nTry < nRl());
 			uc = useClose;
 			if (mode == 1) {
 				// completely random plane (DepthMap.cpp:810-825)
-				const uint4 r = philox4x32_10(make_uint4((uint32_t)idx, phase, (uint32_t)nRestart, 0u), key);
-				++nRestart;
+				const uint4 r = philox4x32_10(make_uint4(pix, phase, (uint32_t)nTry, 0u), key);
+				++nTry;
 				const float s = P.dMinSqr + (P.dMaxSqr-P.dMinSqr)*u32_to_unit(r.x);
 				hd = s*s;
 				hn = random_normal(u32_to_unit(r.y), u32_to_unit(r.z), X0x, X0y);
 				have = true;
-			} else if (mode == 2 && nRefine < nRl) {
+			} else if (mode == 2 && nTry < nRl()) {
 				// perturb around the current estimate (DepthMap.cpp:832-851)
-				const uint4 r = philox4x32_10(make_uint4((uint32_t)idx, phase, (uint32_t)(nR+nRefine), 0u), key);
-				++nRefine;
+				const uint4 r = philox4x32_10(make_uint4(pix, phase, (uint32_t)(nR+nTry), 0u), key);
+				++nTry;
+				const float scaleRange = pow2neg(idxScale);
 				hd = depth + depthRange*scaleRange*(2.f*u32_to_unit(r.x)-1.f);
 				if (P.dMin <= hd && hd < P.dMax) {
 					na = pa + P.angle1Range*scaleRange*(2.f*u32_to_unit(r.y)-1.f);
@@ -649,25 +695,49 @@ pm_sweep_kernel(const __grid_constant__ PMParams P, const __grid_constant__ CUte
 				}
 			}
 		}
-		if (!__any_sync(__activemask(), alive))
+		if (!__any_sync(0xFFFFFFFFu, alive))
 			break;
-		if (!__any_sync(__activemask(), have))
+		if (!__any_sync(0xFFFFFFFFu, have))
 			continue;
+		float nconf = 0.f;
+		uint32_t bv = 0u;
 		if (have) {
+			const int otid = threadIdx.y*BLOCK_X + owner;
+			PatchW pt;
+			pt.s = smemW + otid;
+			const float2 st = smemStats[otid];
+			pt.sumW = st.x; pt.normSq0 = st.y;
+			float oPriorD, oPriorF;
+			pixel_prior(P, (size_t)y*W + sx, st.y, oPriorD, oPriorF);
 			Hyp h;
-			make_hyp(P, x, y, X0x, X0y, hd, hn, dir, uc ? closeMask : 0u, h);
-			uint32_t bv;
-			const float nconf = score_pixel<GEOM>(P, pt, fx, fy, X0x, X0y, h, priorF, priorD, bv);
-			if (conf > nconf) {
-				conf = nconf; depth = hd; normal = hn; bestViews = bv;
-				if (isRefine) {
-					pa = na; pb = nb;
-					++idxScale;
-					scaleRange = pow2neg(idxScale);
+			make_hyp(P, sx, y, X0x, X0y, hd, hn, dir, uc ? (oinfo>>12) : 0u, h);
+			nconf = score_pixel<GEOM>(P, pt, sfx, fy, X0x, X0y, h, oPriorF, oPriorD, bv);
+		}
+		if (packed) {
+			// the owner takes the scores of its candidates of this step (at most four, contiguous lanes) in order
+			#pragma unroll
+			for (int i = 0; i < 4; ++i) {
+				const int src = listed((1u<<lane)-1u) + i - 32*step; // list position of this pixel's candidate i, in this step
+				const bool mine = i < listed(1u<<lane) && src >= 0 && src < 32;
+				const int l = mine ? src : lane;
+				const float c = __shfl_sync(0xFFFFFFFFu, nconf, l);
+				const uint32_t b = __shfl_sync(0xFFFFFFFFu, bv, l);
+				const float d = __shfl_sync(0xFFFFFFFFu, hd, l);
+				const float n0 = __shfl_sync(0xFFFFFFFFu, hn.x, l), n1 = __shfl_sync(0xFFFFFFFFu, hn.y, l), n2 = __shfl_sync(0xFFFFFFFFu, hn.z, l);
+				if (mine && conf > c) {
+					conf = c; depth = d; normal = make_float3(n0, n1, n2); bestViews = b;
 				}
+			}
+		} else if (have && conf > nconf) {
+			conf = nconf; depth = hd; normal = hn; bestViews = bv;
+			if (isRefine) {
+				pa = na; pb = nb;
+				++idxScale;
 			}
 		}
 	}
+	if (!live)
+		return;
 	const float4 pl = P.plane[idx]; // re-read (only this thread writes it) rather than kept live across the loop
 	const bool same = depth == pl.w && normal.x == pl.x && normal.y == pl.y && normal.z == pl.z;
 	P.plane[idx] = make_float4(normal.x, normal.y, normal.z, depth);
@@ -714,7 +784,9 @@ __global__ void pm_unpack_kernel(int n, const float4* __restrict__ plane, float*
 
 // ---- host launchers ---------------------------------------------------------------------
 constexpr size_t W_BYTES = (size_t)PM_TEXELS*NTHREADS*sizeof(float2);
-constexpr size_t SWEEP_SMEM = W_BYTES + 16;  // the reference tile lives inside the weights (pm_sweep_kernel)
+// weights, per-thread patch statistics, mbarrier; the reference tile lives inside the weights (pm_sweep_kernel).  3 CTAs
+// (53.3 KB + 1 KB reserved each) fit the SM's 164 KB shared-memory carveout, which leaves 92 KB of L1
+constexpr size_t SWEEP_SMEM = W_BYTES + NTHREADS*sizeof(float2) + 16;
 static_assert(TILE_BYTES <= W_BYTES, "the reference tile must fit inside the patch weights");
 
 template <bool GEOM>
