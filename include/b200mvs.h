@@ -440,7 +440,7 @@ int b200mvs_scale_image_device(b200mvs_ctx* ctx, const float* image, int width, 
 	float* scaled, int* applied, void* stream);
 
 /* ---- fusion of the depth-maps into a point cloud (SURVEY.md §8(f) rank 4) -----------------------
- * DepthMapsData::FuseDepthMaps (libs/MVS/SceneDensify.cpp:1372-1646): HOST arrays, host code — the result depends on the order in
+ * DepthMapsData::FuseDepthMaps (libs/MVS/SceneDensify.cpp:1372-1646): HOST arrays, host code (device form below) — the result depends on the order in
  * which points claim pixels and zero blocking depths, so the reference's sequential loop is the specification (best connected
  * images first, pixels in raster order).  One b200mvs_fuse_view per scene image (index = image ID); images without a depth-map
  * have depth = NULL.  `depth` is modified like the reference modifies its depth-maps (depths behind an accepted point become 0). */
@@ -465,6 +465,19 @@ typedef struct {
 typedef struct b200mvs_pointcloud b200mvs_pointcloud;   /* PointCloud: points, pointViews, pointWeights, colors, normals */
 void b200mvs_fuse_default_params(b200mvs_fuse_params* p);
 int b200mvs_fuse_depth_maps(b200mvs_fuse_view* views, int nViews, const b200mvs_fuse_params* prm, b200mvs_pointcloud** cloud);
+/* The same fusion on the device: depth / normal / conf / color of every view are DEVICE pointers on the context's device (neighbors
+ * stays a host array), and `depth` is modified in place exactly as the host form modifies it.  The result is the same point cloud,
+ * bit for bit, read back once at the end.  The images stay sequential, one round each in the host form's order; within a round the
+ * pixels are resolved in parallel by an exact fixed point over the neighbour pixels they claim (DESIGN.md §5.5), so a neighbour
+ * list must not repeat an image ID (B200MVS_ERR_ARG; the reference never builds one).  Checks every argument before any launch,
+ * runs on `stream` and waits for it.  stats (nullable): device and wall time, launches, bytes read back. */
+int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, int nViews, const b200mvs_fuse_params* prm,
+	b200mvs_pointcloud** cloud, void* stream, b200mvs_stats* stats);
+/* What each round of the last b200mvs_fuse_depth_maps_device call on ctx did: *nRounds rounds, of which the first maxRounds fill
+ * the arrays (each nullable): the image, the fixed-point iterations, the candidate pixels, the claim and zero edges, the edges whose
+ * neighbour pixel another candidate also reaches, and the device time in ms. */
+int b200mvs_fuse_round_stats(b200mvs_ctx* ctx, int maxRounds, int* nRounds, int* image, int* iterations, uint64_t* candidates,
+	uint64_t* edges, uint64_t* sharedEdges, float* ms);
 uint64_t b200mvs_pointcloud_size(const b200mvs_pointcloud* cloud);
 uint64_t b200mvs_pointcloud_depths(const b200mvs_pointcloud* cloud);               /* valid depths visited (the reference's nDepths) */
 const float* b200mvs_pointcloud_points(const b200mvs_pointcloud* cloud);           /* 3 floats per point */

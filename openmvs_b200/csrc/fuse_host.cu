@@ -1,4 +1,5 @@
-// fuse_host.cu — DepthMapsData::FuseDepthMaps behind the C-ABI (SURVEY.md §8(f) rank 4).  HOST code.
+// fuse_host.cu — DepthMapsData::FuseDepthMaps behind the C-ABI (SURVEY.md §8(f) rank 4): the host form (host code over host
+// arrays) and the host driver of the device form (kernels: fuse_kernels.cu).
 //
 // What it computes (libs/MVS/SceneDensify.cpp:1372-1646): all valid depth-maps are fused into one point cloud, the best
 // connected images first and every pixel in raster order; a pixel that is not yet part of a point creates one, projects it
@@ -6,11 +7,11 @@
 // colour and normal are confidence-weighted means — drops the point when fewer than nMinViewsFuse views agree, and zeroes the
 // neighbour depths that lie behind an accepted point (they would block its view).
 //
-// Why on the host: the result depends on the order — a neighbour pixel claimed by an earlier point is not available to a later
-// one, and a zeroed depth changes what later pixels see — so the reference's single sequential loop IS the specification
-// (north_star keeps fusion on the host; §8(f) ranks it last for that reason).  The maps come straight from the estimation
-// (b200mvs_estimate* / the filter calls); this is the host step after them, written for throughput: flat arrays, the
-// projection matrices composed once, no per-point allocations (views / weights live in one pool).
+// The result depends on the order — a neighbour pixel claimed by an earlier point is not available to a later one, and a zeroed
+// depth changes what later pixels see — so the reference's sequential loop is the specification.  The host form is that loop,
+// written for throughput: flat arrays, the projection matrices composed once, no per-point allocations.  The device form keeps
+// the images sequential (one round per image) and resolves each round's pixels in parallel with the exact fixed point of
+// fuse_kernels.cu (DESIGN.md §5.5); both take their arithmetic from fuse_common.cuh.
 // The CPU restatement used by the tests is oracle/fuse_oracle.py (independent, plain Python loops).
 #include <stdint.h>
 #include <string.h>
@@ -18,44 +19,61 @@
 #include <vector>
 #include <algorithm>
 #include <new>
-#include "../../include/b200mvs.h"
+#include "host_ctx.h"
+#include "fuse_common.cuh"
 
 namespace {
 
 constexpr uint32_t NO_ID = 0xFFFFFFFFu;
+using fuse::Cam;
+using namespace fuse;
 
-struct FuseCam {
-	double K[9], R[9], C[3], P[12];
-};
-// AssembleProjectionMatrix (libs/MVS/Camera.cpp:173-180): P = [K R | -K R C]
-void compose(const b200mvs_fuse_view& v, FuseCam& c) {
-	memcpy(c.K, v.K, sizeof(c.K)); memcpy(c.R, v.R, sizeof(c.R)); memcpy(c.C, v.C, sizeof(c.C));
-	double M[9];
-	for (int i = 0; i < 3; ++i)
-		for (int j = 0; j < 3; ++j)
-			M[3*i+j] = c.K[3*i]*c.R[j] + c.K[3*i+1]*c.R[3+j] + c.K[3*i+2]*c.R[6+j];
-	for (int i = 0; i < 3; ++i) {
-		c.P[4*i] = M[3*i]; c.P[4*i+1] = M[3*i+1]; c.P[4*i+2] = M[3*i+2];
-		c.P[4*i+3] = M[3*i]*(-c.C[0]) + M[3*i+1]*(-c.C[1]) + M[3*i+2]*(-c.C[2]);
+// the argument checks both forms make: map sizes and neighbour IDs; the device form also refuses a neighbour list that repeats an
+// ID (the reference asserts it never does, SceneDensify.cpp:1557), because its rounds need at most one edge per point and target
+const char* fuse_check(const b200mvs_fuse_view* views, int nViews, bool device) {
+	for (int i = 0; i < nViews; ++i) {
+		const b200mvs_fuse_view& v = views[i];
+		if (v.depth && (v.width <= 0 || v.height <= 0 || v.width > 65535 || v.height > 65535)) return "fuse: map size out of range";
+		for (int k = 0; k < v.nNeighbors; ++k) {
+			if (!v.neighbors || v.neighbors[k] >= (uint32_t)nViews || v.neighbors[k] == (uint32_t)i) return "fuse: invalid neighbour ID";
+			if (device)
+				for (int j = 0; j < k; ++j)
+					if (v.neighbors[j] == v.neighbors[k]) return "fuse: repeated neighbour ID";
+		}
 	}
+	return nullptr;
 }
-// Camera::TransformPointI2W(Point3(x, y, depth)) (libs/MVS/Camera.h:339-356), double
-inline void image_to_world(const FuseCam& c, int x, int y, float depth, double out[3]) {
-	const double z = (double)depth;
-	const double cx = ((double)x-c.K[2])*z/c.K[0], cy = ((double)y-c.K[5])*z/c.K[4];
-	out[0] = c.R[0]*cx + c.R[3]*cy + c.R[6]*z + c.C[0];
-	out[1] = c.R[1]*cx + c.R[4]*cy + c.R[7]*z + c.C[1];
-	out[2] = c.R[2]*cx + c.R[5]*cy + c.R[8]*z + c.C[2];
+
+// what both forms derive from the views before fusing: the order of the images and the switches of the loop
+struct FusePlan {
+	std::vector<int> order;
+	bool bNormalMap, bColor, bNormal;
+	unsigned nMin;
+	float normalError, thDepth;
+};
+// any[i]: image i has a depth-map with a depth > 0 in it
+FusePlan fuse_plan(const b200mvs_fuse_view* views, int nViews, const b200mvs_fuse_params* prm, const std::vector<char>& any) {
+	// best connected images first (SceneDensify.cpp:1392-1449); a view is valid when it has a depth-map with a depth in it.
+	// std::sort's order among equal scores is unspecified in the reference: ties go to the lower index here.
+	struct Conn { int idx; float score; };
+	std::vector<Conn> conns;
+	FusePlan p;
+	p.bNormalMap = true;
+	for (int i = 0; i < nViews; ++i) {
+		const b200mvs_fuse_view& v = views[i];
+		if (!v.depth || v.nSceneNeighbors <= 0 || !any[i]) continue;
+		conns.push_back(Conn{i, (float)v.nSceneNeighbors});
+		if (!v.normal) p.bNormalMap = false;
+	}
+	std::stable_sort(conns.begin(), conns.end(), [](const Conn& a, const Conn& b) { return a.score > b.score; });
+	for (const Conn& c: conns) p.order.push_back(c.idx);
+	p.bColor = prm->bEstimateColor != 0;
+	p.bNormal = prm->bEstimateNormal != 0 && p.bNormalMap;
+	p.nMin = (unsigned)std::min(prm->nMinViewsFuse, nViews);
+	p.normalError = cosf(prm->fNormalDiffThreshold*0.017453292519943295f);
+	p.thDepth = prm->fDepthDiffThreshold;
+	return p;
 }
-// R^T n: camera-space normal of the depth-map to world space (SceneDensify.cpp:1526,1554), double sums, float result
-inline void normal_to_world(const FuseCam& c, const float* n, float out[3]) {
-	const double nx = n[0], ny = n[1], nz = n[2];
-	out[0] = (float)(c.R[0]*nx + c.R[3]*ny + c.R[6]*nz);
-	out[1] = (float)(c.R[1]*nx + c.R[4]*ny + c.R[7]*nz);
-	out[2] = (float)(c.R[2]*nx + c.R[5]*ny + c.R[8]*nz);
-}
-// Conf2Weight (SceneDensify.cpp:120-122)
-inline float conf2weight(float conf, float depth) { return 1.f/(fmaxf(1.f-conf, 0.03f)*depth*depth); }
 
 } // namespace
 
@@ -74,47 +92,30 @@ void b200mvs_fuse_default_params(b200mvs_fuse_params* p) {
 }
 
 int b200mvs_fuse_depth_maps(b200mvs_fuse_view* views, int nViews, const b200mvs_fuse_params* prm, b200mvs_pointcloud** out) {
-	if (!views || nViews <= 0 || !out) return B200MVS_ERR_ARG;
+	if (!views || nViews <= 0 || !out || fuse_check(views, nViews, false)) return B200MVS_ERR_ARG;
 	b200mvs_fuse_params def; b200mvs_fuse_default_params(&def);
 	if (!prm) prm = &def;
-	for (int i = 0; i < nViews; ++i) {
-		const b200mvs_fuse_view& v = views[i];
-		if (v.depth && (v.width <= 0 || v.height <= 0 || v.width > 65535 || v.height > 65535)) return B200MVS_ERR_ARG;
-		for (int k = 0; k < v.nNeighbors; ++k)
-			if (!v.neighbors || v.neighbors[k] >= (uint32_t)nViews || v.neighbors[k] == (uint32_t)i) return B200MVS_ERR_ARG;
-	}
 	b200mvs_pointcloud* pc = new (std::nothrow) b200mvs_pointcloud;
 	if (!pc) return B200MVS_ERR_CUDA;
-	std::vector<FuseCam> cams(nViews);
-	for (int i = 0; i < nViews; ++i) compose(views[i], cams[i]);
-	// best connected images first (SceneDensify.cpp:1392-1449); a view is valid when it has a depth-map with a depth in it.
-	// std::sort's order among equal scores is unspecified in the reference: ties go to the lower index here.
-	struct Conn { int idx; float score; };
-	std::vector<Conn> conns;
-	bool bNormalMap = true;
+	std::vector<Cam> cams(nViews);
+	for (int i = 0; i < nViews; ++i) compose(views[i].K, views[i].R, views[i].C, cams[i]);
+	std::vector<char> any(nViews, 0);
 	for (int i = 0; i < nViews; ++i) {
 		const b200mvs_fuse_view& v = views[i];
 		if (!v.depth || v.nSceneNeighbors <= 0) continue;
-		bool any = false;
-		for (size_t k = 0, n = (size_t)v.width*v.height; k < n && !any; ++k) any = v.depth[k] > 0;
-		if (!any) continue;
-		conns.push_back(Conn{i, (float)v.nSceneNeighbors});
-		if (!v.normal) bNormalMap = false;
+		for (size_t k = 0, n = (size_t)v.width*v.height; k < n && !any[i]; ++k) any[i] = v.depth[k] > 0;
 	}
-	std::stable_sort(conns.begin(), conns.end(), [](const Conn& a, const Conn& b) { return a.score > b.score; });
-	const bool bColor = prm->bEstimateColor != 0;
-	const bool bNormal = prm->bEstimateNormal != 0 && bNormalMap;
-	const unsigned nMinViewsFuse = (unsigned)std::min(prm->nMinViewsFuse, nViews);
-	const float normalError = cosf(prm->fNormalDiffThreshold*0.017453292519943295f);
-	const float thDepth = prm->fDepthDiffThreshold;
+	const FusePlan plan = fuse_plan(views, nViews, prm, any);
+	const bool bColor = plan.bColor, bNormal = plan.bNormal, bNormalMap = plan.bNormalMap;
+	const unsigned nMinViewsFuse = plan.nMin;
+	const float normalError = plan.normalError, thDepth = plan.thDepth;
 	std::vector<std::vector<uint32_t>> idxMaps(nViews);
 	pc->offsets.push_back(0);
 	// scratch of the point under construction (a point has at most 1 + nNeighbors views)
 	std::vector<uint32_t> pv; std::vector<float> pw; std::vector<uint16_t> pp; std::vector<float*> invalid;
-	for (const Conn& cn: conns) {
-		const int a = cn.idx;
+	for (const int a: plan.order) {
 		b200mvs_fuse_view& A = views[a];
-		const FuseCam& camA = cams[a];
+		const Cam& camA = cams[a];
 		for (int k = 0; k < A.nNeighbors; ++k) {
 			const uint32_t b = A.neighbors[k];
 			if (idxMaps[b].empty() && views[b].depth) idxMaps[b].assign((size_t)views[b].width*views[b].height, NO_ID);
@@ -138,32 +139,27 @@ int b200mvs_fuse_depth_maps(b200mvs_fuse_view* views, int nViews, const b200mvs_
 				double confidence = (double)pw[0];
 				float normal[3] = {0.f, 0.f, -1.f};
 				if (bNormalMap) normal_to_world(camA, A.normal+3*ia, normal);
-				double X[3] = {(double)point[0]*confidence, (double)point[1]*confidence, (double)point[2]*confidence};
+				double X[3] = {mul_d((double)point[0], confidence), mul_d((double)point[1], confidence), mul_d((double)point[2], confidence)};
 				float Cc[3] = {0.f, 0.f, 0.f};
-				if (bColor && A.color) for (int c = 0; c < 3; ++c) Cc[c] = (float)A.color[3*ia+c]*(float)confidence;
-				float N[3] = {normal[0]*(float)confidence, normal[1]*(float)confidence, normal[2]*(float)confidence};
+				if (bColor && A.color) for (int c = 0; c < 3; ++c) Cc[c] = mul_f((float)A.color[3*ia+c], (float)confidence);
+				float N[3] = {mul_f(normal[0], (float)confidence), mul_f(normal[1], (float)confidence), mul_f(normal[2], (float)confidence)};
 				invalid.clear();
 				for (int k = 0; k < A.nNeighbors; ++k) {
 					const uint32_t b = A.neighbors[k];
 					b200mvs_fuse_view& B = views[b];
 					if (!B.depth) continue;
-					const FuseCam& camB = cams[b];
-					// Camera::ProjectPointP3<float> (Camera.h:308-314): double sums, float components
-					const float px = (float)(camB.P[0]*point[0] + camB.P[1]*point[1] + camB.P[2]*point[2] + camB.P[3]);
-					const float py = (float)(camB.P[4]*point[0] + camB.P[5]*point[1] + camB.P[6]*point[2] + camB.P[7]);
-					const float pz = (float)(camB.P[8]*point[0] + camB.P[9]*point[1] + camB.P[10]*point[2] + camB.P[11]);
-					if (pz <= 0) continue;
-					const int xb = (int)floorf(px/pz+.5f), yb = (int)floorf(py/pz+.5f);   // ROUND2INT (libs/Common/Types.h:947-953)
-					if (xb < 0 || yb < 0 || xb >= B.width || yb >= B.height) continue;
+					const Cam& camB = cams[b];
+					float pz; int xb, yb;
+					if (!project_to_pixel(camB, point, B.width, B.height, pz, xb, yb)) continue;
 					const size_t ib = (size_t)yb*B.width + xb;
 					float& depthB = B.depth[ib];
 					if (depthB == 0) continue;
 					uint32_t& idxPointB = idxMaps[b][ib];
 					if (idxPointB != NO_ID) continue;
-					if (fabsf(pz-depthB)/pz < thDepth) {       // IsDepthSimilar(pt.z, depthB) (libs/Common/Util.inl:797-809)
+					if (depth_similar(pz, depthB, thDepth)) {
 						float normalB[3] = {0.f, 0.f, -1.f};
 						if (bNormalMap) normal_to_world(camB, B.normal+3*ib, normalB);
-						if (normal[0]*normalB[0] + normal[1]*normalB[1] + normal[2]*normalB[2] > normalError) {
+						if (dot3(normal, normalB) > normalError) {
 							const float confB = conf2weight(B.conf ? B.conf[ib] : 1.f, depthB);
 							size_t pos = 0;                      // views stay sorted by image index (InsertSort)
 							while (pos < pv.size() && pv[pos] < b) ++pos;
@@ -172,10 +168,10 @@ int b200mvs_fuse_depth_maps(b200mvs_fuse_view* views, int nViews, const b200mvs_
 							idxPointB = idxPoint;
 							double Xb[3];
 							image_to_world(camB, xb, yb, depthB, Xb);
-							X[0] += Xb[0]*(double)confB; X[1] += Xb[1]*(double)confB; X[2] += Xb[2]*(double)confB;
-							if (bColor && B.color) for (int c = 0; c < 3; ++c) Cc[c] += (float)B.color[3*ib+c]*confB;
-							if (bNormal) for (int c = 0; c < 3; ++c) N[c] += normalB[c]*confB;
-							confidence += (double)confB;
+							for (int c = 0; c < 3; ++c) X[c] = add_d(X[c], mul_d(Xb[c], (double)confB));
+							if (bColor && B.color) for (int c = 0; c < 3; ++c) Cc[c] = add_f(Cc[c], mul_f((float)B.color[3*ib+c], confB));
+							if (bNormal) for (int c = 0; c < 3; ++c) N[c] = add_f(N[c], mul_f(normalB[c], confB));
+							confidence = add_d(confidence, (double)confB);
 							continue;
 						}
 					}
@@ -186,13 +182,13 @@ int b200mvs_fuse_depth_maps(b200mvs_fuse_view* views, int nViews, const b200mvs_
 						idxMaps[pv[v]][(size_t)pp[2*v+1]*views[pv[v]].width + pp[2*v]] = NO_ID;
 					continue;
 				}
-				const double nrm = 1.0/confidence;
-				for (int c = 0; c < 3; ++c) pc->points.push_back((float)(X[c]*nrm));
-				if (bColor && A.color) for (int c = 0; c < 3; ++c) pc->colors.push_back((uint8_t)(Cc[c]*(float)nrm));
+				const double nrm = div_d(1.0, confidence);
+				for (int c = 0; c < 3; ++c) pc->points.push_back((float)mul_d(X[c], nrm));
+				if (bColor && A.color) for (int c = 0; c < 3; ++c) pc->colors.push_back((uint8_t)mul_f(Cc[c], (float)nrm));
 				if (bNormal) {
-					const float n0 = N[0]*(float)nrm, n1 = N[1]*(float)nrm, n2 = N[2]*(float)nrm;
-					const float len = sqrtf(n0*n0 + n1*n1 + n2*n2);
-					pc->normals.push_back(n0/len); pc->normals.push_back(n1/len); pc->normals.push_back(n2/len);
+					const float n0 = mul_f(N[0], (float)nrm), n1 = mul_f(N[1], (float)nrm), n2 = mul_f(N[2], (float)nrm);
+					const float len = sqrt_f(add_f(add_f(mul_f(n0, n0), mul_f(n1, n1)), mul_f(n2, n2)));
+					pc->normals.push_back(div_f(n0, len)); pc->normals.push_back(div_f(n1, len)); pc->normals.push_back(div_f(n2, len));
 				}
 				pc->views.insert(pc->views.end(), pv.begin(), pv.end());
 				pc->weights.insert(pc->weights.end(), pw.begin(), pw.end());
@@ -203,6 +199,283 @@ int b200mvs_fuse_depth_maps(b200mvs_fuse_view* views, int nViews, const b200mvs_
 		}
 	}
 	*out = pc;
+	return B200MVS_OK;
+}
+
+} // extern "C"
+
+namespace {
+
+// grow a device buffer to `need` bytes, keeping its first `used` bytes (enqueued on s)
+cudaError_t grow_keep(DevBuf& b, size_t used, size_t need, cudaStream_t s) {
+	if (need <= b.cap) return cudaSuccess;
+	DevBuf n;
+	cudaError_t e = n.reserve(std::max(need, b.cap + b.cap/2));
+	if (e == cudaSuccess && used) e = cudaMemcpyAsync(n.p, b.p, used, cudaMemcpyDeviceToDevice, s);
+	if (e != cudaSuccess) return e;
+	e = cudaStreamSynchronize(s);
+	std::swap(b.p, n.p); std::swap(b.cap, n.cap);
+	return e;
+}
+
+// map pointers of the device form must be device (or managed) memory of the context's device
+bool on_device(const b200mvs_ctx* ctx, const void* p) {
+	if (!p) return true;
+	cudaPointerAttributes a;
+	if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+	return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == ctx->device;
+}
+
+// the fixed counters of one call, in device memory
+struct FuseCounters {
+	unsigned long long nDepths, shared;
+	uint32_t nCand, nEdges, undecided, totals[2];
+};
+
+} // namespace
+
+extern "C" {
+
+int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, int nViews, const b200mvs_fuse_params* prm,
+	b200mvs_pointcloud** out, void* stream, b200mvs_stats* stats)
+{
+	if (!ctx) return B200MVS_ERR_ARG;
+	if (!views || nViews <= 0 || !out) return fail(ctx, B200MVS_ERR_ARG, "fuse: null pointer");
+	if (const char* why = fuse_check(views, nViews, true)) return fail(ctx, B200MVS_ERR_ARG, why);
+	b200mvs_fuse_params def; b200mvs_fuse_default_params(&def);
+	if (!prm) prm = &def;
+	CK(cudaSetDevice(ctx->device));
+	for (int i = 0; i < nViews; ++i) {
+		const b200mvs_fuse_view& v = views[i];
+		if (!on_device(ctx, v.depth) || !on_device(ctx, v.normal) || !on_device(ctx, v.conf) || !on_device(ctx, v.color))
+			return fail(ctx, B200MVS_ERR_ARG, "fuse: a map is not in device memory of the context's device");
+	}
+	// the view table, the claim maps and the neighbour lists with their round-local target bases
+	std::vector<FuseDevView> dv(nViews);
+	std::vector<size_t> claimOff(nViews, 0), nbOff(nViews+1, 0);
+	size_t claimBytes = 0;
+	for (int i = 0; i < nViews; ++i) {
+		const b200mvs_fuse_view& v = views[i];
+		FuseDevView& d = dv[i];
+		d.depth = v.depth; d.normal = v.normal; d.conf = v.conf; d.color = v.color; d.claim = nullptr;
+		d.w = v.depth ? v.width : 0; d.h = v.depth ? v.height : 0;
+		compose(v.K, v.R, v.C, d.cam);
+		claimOff[i] = claimBytes; claimBytes += (size_t)d.w*d.h;
+		nbOff[i+1] = nbOff[i] + v.nNeighbors;
+	}
+	std::vector<int> nbIds(nbOff[nViews]);
+	std::vector<uint32_t> nbBase(nbOff[nViews]);
+	for (int i = 0; i < nViews; ++i) {
+		const b200mvs_fuse_view& v = views[i];
+		uint64_t base = 0;
+		for (int k = 0; k < v.nNeighbors; ++k) {
+			nbIds[nbOff[i]+k] = (int)v.neighbors[k];
+			nbBase[nbOff[i]+k] = (uint32_t)base;
+			base += (uint64_t)dv[v.neighbors[k]].w*dv[v.neighbors[k]].h;
+		}
+		if (v.depth && (base >= 0xFFFFFFFFull || (uint64_t)v.width*v.height*(uint64_t)std::max(v.nNeighbors, 1) >= 0x7FFFFFFFull))
+			return fail(ctx, B200MVS_ERR_ARG, "fuse: the maps of an image and its neighbours are too large for one round");
+	}
+	const auto t0 = std::chrono::steady_clock::now();
+	cudaStream_t s = stream_of(ctx, stream);
+	ctx->launches = 0;
+	ctx->fsRounds.clear();
+	const size_t nNbAll = std::max<size_t>(nbIds.size(), 1);
+	CK(ctx->fsClaim.reserve(std::max<size_t>(claimBytes, 1)));
+	for (int i = 0; i < nViews; ++i) if (views[i].depth) dv[i].claim = ctx->fsClaim.as<uint8_t>() + claimOff[i];
+	CK(ctx->fsViews.reserve(sizeof(FuseDevView)*nViews));
+	CK(ctx->fsNb.reserve(nNbAll*8));
+	CK(ctx->fsAny.reserve(sizeof(int)*nViews));
+	CK(ctx->fsCount.reserve(sizeof(FuseCounters)));
+	int* dNb = ctx->fsNb.as<int>();
+	uint32_t* dBase = (uint32_t*)(dNb + nNbAll);
+	FuseCounters* cnt = ctx->fsCount.as<FuseCounters>();
+	CK(cudaEventRecord(ctx->ev0, s));
+	CK(cudaMemcpyAsync(ctx->fsViews.p, dv.data(), sizeof(FuseDevView)*nViews, cudaMemcpyHostToDevice, s));
+	if (!nbIds.empty()) {
+		CK(cudaMemcpyAsync(dNb, nbIds.data(), nbIds.size()*4, cudaMemcpyHostToDevice, s));
+		CK(cudaMemcpyAsync(dBase, nbBase.data(), nbBase.size()*4, cudaMemcpyHostToDevice, s));
+	}
+	if (claimBytes) CK(cudaMemsetAsync(ctx->fsClaim.p, 0, claimBytes, s));
+	CK(cudaMemsetAsync(ctx->fsAny.p, 0, sizeof(int)*nViews, s));
+	CK(cudaMemsetAsync(cnt, 0, sizeof(FuseCounters), s));
+	// which images have a depth > 0 (the host form's validity test), then the same order of the images as the host form
+	for (int i = 0; i < nViews; ++i)
+		if (views[i].depth && views[i].nSceneNeighbors > 0) {
+			CK(fuse_launch_any_positive(views[i].depth, (size_t)views[i].width*views[i].height, ctx->fsAny.as<int>()+i, s));
+			++ctx->launches;
+		}
+	std::vector<int> anyI(nViews);
+	CK(cudaMemcpyAsync(anyI.data(), ctx->fsAny.p, sizeof(int)*nViews, cudaMemcpyDeviceToHost, s));
+	CK(cudaStreamSynchronize(s));
+	uint64_t d2h = sizeof(int)*nViews;
+	const FusePlan plan = fuse_plan(views, nViews, prm, std::vector<char>(anyI.begin(), anyI.end()));
+
+	struct Events {
+		cudaEvent_t b = nullptr, e = nullptr;
+		~Events() { if (b) cudaEventDestroy(b); if (e) cudaEventDestroy(e); }
+	} ev;
+	CK(cudaEventCreate(&ev.b)); CK(cudaEventCreate(&ev.e));
+	// the outputs grow with the rounds: points, normals, colors, offsets (per point), views, weights, projs (per view)
+	DevBuf* O = ctx->fsOut;
+	const size_t perPoint[4] = {12, 12, 3, 4}, perView[3] = {4, 4, 4};
+	uint64_t nPts = 0, nVw = 0, nCol = 0, shared = 0;
+	size_t need = 0;
+	// a CUB call: query its temporary storage, then run it
+#define FUSE_CUB(call) do { need = 0; { void* tmp = nullptr; CK(call); } \
+		CK(ctx->fsCub.reserve(std::max<size_t>(need, 1))); { void* tmp = ctx->fsCub.p; CK(call); } } while (0)
+	for (const int a: plan.order) {
+		const b200mvs_fuse_view& A = views[a];
+		const size_t np = (size_t)A.width*A.height;
+		const int nNb = A.nNeighbors;
+		FuseRound R;
+		R.views = ctx->fsViews.as<FuseDevView>(); R.a = a; R.nNb = nNb; R.nb = dNb + nbOff[a]; R.base = dBase + nbOff[a];
+		R.bNormalMap = plan.bNormalMap; R.bColor = plan.bColor; R.bNormal = plan.bNormal;
+		R.nMin = plan.nMin; R.thDepth = plan.thDepth; R.normalError = plan.normalError;
+		b200mvs_ctx::FuseRoundStat st{a, 0, 0, 0, 0, 0.f};
+		CK(cudaEventRecord(ev.b, s));
+		// the candidates: pixels with a depth and no claim, in raster order
+		CK(ctx->fsFlags.reserve(np)); CK(ctx->fsCand.reserve(np*4));
+		uint8_t* flags = ctx->fsFlags.as<uint8_t>();
+		uint32_t* cand = ctx->fsCand.as<uint32_t>();
+		CK(fuse_launch_candidates(A.depth, dv[a].claim, np, flags, &cnt->nDepths, s));
+		FUSE_CUB(fuse_select(tmp, need, flags, cand, &cnt->nCand, np, s));
+		ctx->launches += 2;
+		uint32_t nCand = 0, nEdges = 0;
+		CK(cudaMemcpyAsync(&nCand, &cnt->nCand, 4, cudaMemcpyDeviceToHost, s));
+		CK(cudaStreamSynchronize(s));
+		d2h += 4;
+		st.candidates = nCand;
+		if (nCand > 0) {
+			const size_t ne = (size_t)nCand*nNb;
+			CK(ctx->fsAcc.reserve(nCand)); CK(ctx->fsIsPt.reserve(nCand*4)); CK(ctx->fsPtId.reserve(nCand*4));
+			CK(ctx->fsNv.reserve(nCand*4)); CK(ctx->fsVOff.reserve(nCand*4));
+			CK(ctx->fsTyp.reserve(std::max<size_t>(ne, 1))); CK(ctx->fsStatus.reserve(std::max<size_t>(ne, 1)));
+			CK(ctx->fsTgt.reserve(std::max<size_t>(ne, 1)*4));
+			uint8_t* acc = ctx->fsAcc.as<uint8_t>();
+			uint8_t* typ = ctx->fsTyp.as<uint8_t>();
+			uint8_t* status = ctx->fsStatus.as<uint8_t>();
+			uint32_t* tgt = ctx->fsTgt.as<uint32_t>();
+			uint32_t *keys = nullptr, *edges = nullptr;
+			CK(cudaMemsetAsync(acc, 0, nCand, s));
+			if (ne > 0) {
+				// the edges: type and target from the maps at the start of the round; the claim and zero edges, grouped by target in
+				// raster order of their owners (the radix sort is stable and its input is in edge order)
+				CK(ctx->fsEdge.reserve(ne*4)); CK(ctx->fsEdge2.reserve(ne*4)); CK(ctx->fsKeys.reserve(ne*4)); CK(ctx->fsKeys2.reserve(ne*4));
+				uint32_t* e1 = ctx->fsEdge.as<uint32_t>();
+				CK(fuse_launch_classify(R, cand, nCand, typ, tgt, s));
+				FUSE_CUB(fuse_select(tmp, need, typ, e1, &cnt->nEdges, ne, s));
+				ctx->launches += 2;
+				CK(cudaMemcpyAsync(&nEdges, &cnt->nEdges, 4, cudaMemcpyDeviceToHost, s));
+				CK(cudaStreamSynchronize(s));
+				d2h += 4;
+				if (nEdges > 0) {
+					uint32_t* k1 = ctx->fsKeys.as<uint32_t>();
+					keys = ctx->fsKeys2.as<uint32_t>(); edges = ctx->fsEdge2.as<uint32_t>();
+					int endBit = 1;
+					while (endBit < 32 && (1ull << endBit) < (uint64_t)nbBase[nbOff[a]+nNb-1] + (uint64_t)dv[nbIds[nbOff[a]+nNb-1]].w*dv[nbIds[nbOff[a]+nNb-1]].h)
+						++endBit;
+					CK(fuse_launch_gather_keys(tgt, e1, nEdges, k1, s));
+					FUSE_CUB(fuse_sort(tmp, need, k1, keys, e1, edges, nEdges, endBit, s));
+					CK(fuse_launch_shared(keys, nEdges, &cnt->shared, s));
+					ctx->launches += 3;
+				}
+			}
+			// the fixed point: every iteration decides at least the earliest undecided candidate
+			for (uint32_t undecided = nCand, last = nCand + 1; undecided > 0; ) {
+				if (undecided >= last) return fail(ctx, B200MVS_ERR_CUDA, "fuse: the acceptance fixed point made no progress");
+				last = undecided;
+				CK(cudaMemsetAsync(&cnt->undecided, 0, 4, s));
+				if (nEdges > 0) { CK(fuse_launch_walk(keys, edges, nEdges, nNb, acc, status, s)); ++ctx->launches; }
+				CK(fuse_launch_decide(R, nCand, typ, status, acc, &cnt->undecided, s));
+				++ctx->launches;
+				CK(cudaMemcpyAsync(&undecided, &cnt->undecided, 4, cudaMemcpyDeviceToHost, s));
+				CK(cudaStreamSynchronize(s));
+				d2h += 4;
+				++st.iterations;
+			}
+			// a candidate can decide while some of its edges are still unknown: one more walk with every candidate decided makes
+			// every edge live or dead, which the views of a point and its zeroed depths need
+			if (nEdges > 0) { CK(fuse_launch_walk(keys, edges, nEdges, nNb, acc, status, s)); ++ctx->launches; }
+			// point IDs and view offsets in raster order, then the points
+			uint32_t *isPt = ctx->fsIsPt.as<uint32_t>(), *ptId = ctx->fsPtId.as<uint32_t>(), *nv = ctx->fsNv.as<uint32_t>(),
+				*vOff = ctx->fsVOff.as<uint32_t>();
+			CK(fuse_launch_count(R, nCand, typ, status, acc, isPt, nv, s));
+			FUSE_CUB(fuse_scan(tmp, need, isPt, ptId, nCand, s));
+			FUSE_CUB(fuse_scan(tmp, need, nv, vOff, nCand, s));
+			CK(fuse_launch_totals(isPt, ptId, nv, vOff, nCand, cnt->totals, s));
+			ctx->launches += 4;
+			FuseCounters hc;
+			CK(cudaMemcpyAsync(&hc, cnt, sizeof(hc), cudaMemcpyDeviceToHost, s));
+			CK(cudaStreamSynchronize(s));
+			d2h += sizeof(hc);
+			const uint64_t nP = hc.totals[0], nV = hc.totals[1];
+			st.edges = nEdges; st.shared = hc.shared - shared; shared = hc.shared;
+			if (nPts + nP + 1 >= 0xFFFFFFFFull || nVw + nV >= 0xFFFFFFFFull)
+				return fail(ctx, B200MVS_ERR_ARG, "fuse: more than 2^32 points or views");
+			const bool colorA = plan.bColor && A.color;
+			if (nP > 0) {
+				for (int i = 0; i < 4; ++i) {
+					if ((i == 1 && !plan.bNormal) || (i == 2 && !colorA)) continue;
+					const uint64_t used = i == 2 ? nCol : nPts;
+					CK(grow_keep(O[i], used*perPoint[i], (used + nP + (i == 3))*perPoint[i], s));
+				}
+				for (int i = 0; i < 3; ++i) CK(grow_keep(O[4+i], nVw*perView[i], (nVw + nV)*perView[i], s));
+				FuseOut fo;
+				fo.points = O[0].as<float>() + 3*nPts; fo.normals = plan.bNormal ? O[1].as<float>() + 3*nPts : nullptr;
+				fo.colors = colorA ? O[2].as<uint8_t>() + 3*nCol : nullptr; fo.offsets = O[3].as<uint32_t>() + nPts;
+				fo.views = O[4].as<uint32_t>(); fo.weights = O[5].as<float>(); fo.projs = O[6].as<uint16_t>(); fo.viewBase = (uint32_t)nVw;
+				CK(fuse_launch_assemble(R, cand, nCand, typ, tgt, status, acc, ptId, vOff, fo, s));
+				++ctx->launches;
+				nPts += nP; nVw += nV; nCol += colorA ? nP : 0;
+			}
+		}
+		CK(cudaEventRecord(ev.e, s));
+		CK(cudaEventSynchronize(ev.e));
+		CK(cudaEventElapsedTime(&st.ms, ev.b, ev.e));
+		ctx->fsRounds.push_back(st);
+	}
+#undef FUSE_CUB
+	CK(cudaEventRecord(ctx->ev1, s));
+	// one read-back of the whole point cloud
+	b200mvs_pointcloud* pc = new (std::nothrow) b200mvs_pointcloud;
+	if (!pc) return fail(ctx, B200MVS_ERR_CUDA, "fuse: out of host memory");
+	struct Owner { b200mvs_pointcloud* p; ~Owner() { delete p; } } own{pc};
+	FuseCounters hc;
+	CK(cudaMemcpyAsync(&hc, cnt, sizeof(hc), cudaMemcpyDeviceToHost, s));
+	pc->points.resize(3*nPts); pc->normals.resize(plan.bNormal ? 3*nPts : 0); pc->colors.resize(3*nCol);
+	pc->offsets.resize(nPts+1); pc->views.resize(nVw); pc->weights.resize(nVw); pc->projs.resize(2*nVw);
+	auto get = [&](void* dst, const DevBuf& src, size_t bytes) {
+		d2h += bytes;
+		return bytes ? cudaMemcpyAsync(dst, src.p, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+	};
+	CK(get(pc->points.data(), O[0], pc->points.size()*4)); CK(get(pc->normals.data(), O[1], pc->normals.size()*4));
+	CK(get(pc->colors.data(), O[2], pc->colors.size())); CK(get(pc->offsets.data(), O[3], nPts*4));
+	CK(get(pc->views.data(), O[4], nVw*4)); CK(get(pc->weights.data(), O[5], nVw*4)); CK(get(pc->projs.data(), O[6], nVw*4));
+	CK(cudaStreamSynchronize(s));
+	d2h += sizeof(hc);
+	pc->offsets[nPts] = (uint32_t)nVw;
+	pc->nDepths = hc.nDepths;
+	if (stats) { const int rc = fill_stats(ctx, stats, t0, 1, 0, d2h); if (rc) return rc; }
+	*out = pc;
+	own.p = nullptr;
+	return B200MVS_OK;
+}
+
+int b200mvs_fuse_round_stats(b200mvs_ctx* ctx, int maxRounds, int* nRounds, int* image, int* iterations, uint64_t* candidates,
+	uint64_t* edges, uint64_t* sharedEdges, float* ms)
+{
+	if (!ctx || maxRounds < 0 || !nRounds) return B200MVS_ERR_ARG;
+	*nRounds = (int)ctx->fsRounds.size();
+	for (int i = 0; i < std::min(maxRounds, *nRounds); ++i) {
+		const b200mvs_ctx::FuseRoundStat& r = ctx->fsRounds[i];
+		if (image) image[i] = r.image;
+		if (iterations) iterations[i] = r.iterations;
+		if (candidates) candidates[i] = r.candidates;
+		if (edges) edges[i] = r.edges;
+		if (sharedEdges) sharedEdges[i] = r.shared;
+		if (ms) ms[i] = r.ms;
+	}
 	return B200MVS_OK;
 }
 

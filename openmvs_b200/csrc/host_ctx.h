@@ -59,6 +59,13 @@ struct b200mvs_ctx {
 	DevBuf fltZ, fltIn, fltOutD, fltOutC;     // FilterDepthMap: z-buffer keys, staged maps (host API), outputs
 	DevBuf ppA, ppB, ppD, ppN, ppC;           // RemoveSmallSegments labels/sizes, GapInterpolation temporaries, staging
 	DevBuf ppK, ppArcs, ppPatch;              // RemoveSmallSegments: seed keys, one-way edges (+ counter), patched segment sizes
+	// FuseDepthMaps (device form): view table, neighbour lists, claim maps, per-round candidate / edge scratch, counters, the growing
+	// point-cloud outputs, and what each round of the last call did (b200mvs_fuse_round_stats)
+	DevBuf fsViews, fsNb, fsClaim, fsAny, fsFlags, fsCand, fsTyp, fsTgt, fsEdge, fsKeys, fsKeys2, fsEdge2, fsStatus, fsAcc;
+	DevBuf fsIsPt, fsPtId, fsNv, fsVOff, fsCub, fsCount;
+	DevBuf fsOut[7];                          // points, normals, colors, offsets, views, weights, projs
+	struct FuseRoundStat { int image, iterations; uint64_t candidates, edges, shared; float ms; };
+	std::vector<FuseRoundStat> fsRounds;
 	b200mvs_debug dbg;                        // diagnostic switches (b200mvs_set_debug); all zero = the shipped kernels
 	const uint8_t* mask = nullptr; int maskW = 0, maskH = 0, maskPitch = 0; // ignore-mask of the reference view (device) or null
 	DevBuf maskBuf, maskLevel;                // staged host mask, mask of the current pyramid level

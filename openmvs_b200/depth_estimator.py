@@ -795,7 +795,15 @@ class SemiGlobalMatcher(_Context):
 		return depth, conf, normal
 
 
-_NORMAL_CTX = {}
+_DEVICE_CTX = {}
+
+
+def _device_context(dev) -> _Context:
+	"""the context kept per device for the module-level device calls (EstimateNormalMap, FuseDepthMaps)"""
+	ctx = _DEVICE_CTX.get(dev.index)
+	if ctx is None:
+		ctx = _DEVICE_CTX[dev.index] = _Context(dev.index)
+	return ctx
 
 
 def EstimateNormalMap(K, depthMap):
@@ -806,9 +814,7 @@ def EstimateNormalMap(K, depthMap):
 	if not (_is_torch(depthMap) and depthMap.is_cuda and depthMap.dtype == torch.float32 and depthMap.dim() == 2 and depthMap.is_contiguous()):
 		raise ValueError("depthMap must be a contiguous 2-D float32 CUDA tensor")
 	dev = depthMap.device
-	ctx = _NORMAL_CTX.get(dev.index)
-	if ctx is None:
-		ctx = _NORMAL_CTX[dev.index] = _Context(dev.index)
+	ctx = _device_context(dev)
 	k = np.ascontiguousarray(K, np.float64).reshape(9)
 	h, w = depthMap.shape
 	normal = torch.empty((h, w, 3), dtype=torch.float32, device=dev)
@@ -830,29 +836,48 @@ class PointCloud:
 
 def FuseDepthMaps(views, nMinViewsFuse: int = 2, fDepthDiffThreshold: float = 0.01, fNormalDiffThreshold: float = 25.0,
 		bEstimateColor: bool = True, bEstimateNormal: bool = True) -> PointCloud:
-	"""DepthMapsData::FuseDepthMaps (libs/MVS/SceneDensify.cpp:1372-1646) through b200mvs_fuse_depth_maps (host arrays, host code:
-	the sequential greedy order is the specification).  views[i] (index = image ID): dict with depth (h, w) float32 — MODIFIED in
-	place like the reference's depth-maps (depths behind an accepted point are zeroed) — or None, normal (h, w, 3) / conf (h, w) /
-	color (h, w, 3) uint8 or None, K R C, neighbors (image IDs, best first) and n_scene_neighbors (the connection score)."""
+	"""DepthMapsData::FuseDepthMaps (libs/MVS/SceneDensify.cpp:1372-1646).  views[i] (index = image ID): dict with depth (h, w)
+	float32 — MODIFIED in place like the reference's depth-maps (depths behind an accepted point are zeroed) — or None, normal
+	(h, w, 3) / conf (h, w) / color (h, w, 3) uint8 or None, K R C, neighbors (image IDs, best first) and n_scene_neighbors (the
+	connection score).
+	numpy maps take b200mvs_fuse_depth_maps (host code: the sequential loop).  CUDA tensors (every map on one device, depth
+	contiguous) take b200mvs_fuse_depth_maps_device on a context kept per device: the same point cloud, bit for bit, with the
+	pixels of each image resolved in parallel; a neighbour list must not repeat an image ID there."""
 	lib = _lib.load()
+	device = any(_is_torch(v.get("depth")) for v in views)
 	n = len(views)
 	arr = (_lib.FuseView*n)()
 	keep = []
+	dev = None
 	for i, v in enumerate(views):
 		o = arr[i]
 		d = v.get("depth")
 		if d is not None:
-			if not (isinstance(d, np.ndarray) and d.dtype == np.float32 and d.flags.c_contiguous and d.flags.writeable):
+			if device:
+				import torch
+				dev = d.device if dev is None else dev
+				if not (_is_torch(d) and d.is_cuda and d.device == dev and d.dtype == torch.float32 and d.dim() == 2 and d.is_contiguous()):
+					raise ValueError("views[%d].depth must be a contiguous 2-D float32 CUDA tensor on the device of the other views" % i)
+			elif not (isinstance(d, np.ndarray) and d.dtype == np.float32 and d.flags.c_contiguous and d.flags.writeable):
 				raise ValueError("views[%d].depth must be a writeable C-contiguous float32 array (it is modified in place)" % i)
 			o.height, o.width = d.shape
-			o.depth = d.ctypes.data
-			for key, dt, shape in (("normal", np.float32, d.shape+(3,)), ("conf", np.float32, d.shape), ("color", np.uint8, d.shape+(3,))):
+			o.depth = d.data_ptr() if device else d.ctypes.data
+			for key, dt, shape in (("normal", np.float32, tuple(d.shape)+(3,)), ("conf", np.float32, tuple(d.shape)),
+					("color", np.uint8, tuple(d.shape)+(3,))):
 				a = v.get(key)
-				if a is not None:
+				if a is None:
+					continue
+				if device:
+					if not (_is_torch(a) and a.device == dev and str(a.dtype) == "torch."+np.dtype(dt).name and tuple(a.shape) == shape):
+						raise ValueError("views[%d].%s must be a %s CUDA tensor of shape %s on the depth's device" % (i, key, np.dtype(dt).name, shape))
+					a = a.contiguous()
+					ptr = a.data_ptr()
+				else:
 					a = np.ascontiguousarray(a, dt)
 					if a.shape != shape:
 						raise ValueError("views[%d].%s has shape %s, expected %s" % (i, key, a.shape, shape))
-					keep.append(a); setattr(o, key, a.ctypes.data)
+					ptr = a.ctypes.data
+				keep.append(a); setattr(o, key, ptr)
 		for name in ("K", "R", "C"):
 			getattr(o, name)[:] = list(np.asarray(v[name], np.float64).ravel())
 		nb = np.ascontiguousarray(v.get("neighbors", []), np.uint32)
@@ -862,23 +887,50 @@ def FuseDepthMaps(views, nMinViewsFuse: int = 2, fDepthDiffThreshold: float = 0.
 		o.nSceneNeighbors = int(v.get("n_scene_neighbors", nb.size))
 	prm = _lib.FuseParams(int(nMinViewsFuse), float(fDepthDiffThreshold), float(fNormalDiffThreshold), int(bool(bEstimateColor)), int(bool(bEstimateNormal)))
 	cloud = C.c_void_p()
-	rc = lib.b200mvs_fuse_depth_maps(arr, n, C.byref(prm), C.byref(cloud))
-	if rc:
-		raise _lib.B200MVSError("b200mvs_fuse_depth_maps failed with status %d (bad view description)" % rc)
+	if device:
+		ctx = _device_context(dev)
+		ctx._call("fuse_depth_maps_device", arr, n, C.byref(prm), C.byref(cloud), _stream_handle(dev), C.byref(ctx.stats))
+	else:
+		rc = lib.b200mvs_fuse_depth_maps(arr, n, C.byref(prm), C.byref(cloud))
+		if rc:
+			raise _lib.B200MVSError("b200mvs_fuse_depth_maps failed with status %d (bad view description)" % rc)
 	try:
-		m = int(lib.b200mvs_pointcloud_size(cloud))
-		def take(fn, count, dt):
-			p = fn(cloud)
-			return np.ctypeslib.as_array(p, shape=(count,)).astype(dt, copy=True) if (count and p) else None
-		off = take(lib.b200mvs_pointcloud_view_offsets, m+1, np.uint32)
-		total = int(off[-1]) if off is not None else 0
-		pts = take(lib.b200mvs_pointcloud_points, 3*m, np.float32)
-		vs = take(lib.b200mvs_pointcloud_views, total, np.uint32); ws = take(lib.b200mvs_pointcloud_weights, total, np.float32)
-		pj = take(lib.b200mvs_pointcloud_projs, 2*total, np.uint16)
-		nr = take(lib.b200mvs_pointcloud_normals, 3*m, np.float32); cl = take(lib.b200mvs_pointcloud_colors, 3*m, np.uint8)
-		return PointCloud(points=pts.reshape(-1, 3) if pts is not None else np.zeros((0, 3), np.float32),
-			pointViews=[vs[off[i]:off[i+1]] for i in range(m)], pointWeights=[ws[off[i]:off[i+1]] for i in range(m)],
-			colors=None if cl is None else cl.reshape(-1, 3), normals=None if nr is None else nr.reshape(-1, 3),
-			projs=[pj[2*off[i]:2*off[i+1]].reshape(-1, 2) for i in range(m)], nDepths=int(lib.b200mvs_pointcloud_depths(cloud)))
+		return _point_cloud(lib, cloud)
 	finally:
 		lib.b200mvs_pointcloud_free(cloud)
+
+
+def _point_cloud(lib, cloud) -> PointCloud:
+	"""copy a b200mvs_pointcloud into a PointCloud"""
+	m = int(lib.b200mvs_pointcloud_size(cloud))
+	def take(fn, count, dt):
+		p = fn(cloud)
+		return np.ctypeslib.as_array(p, shape=(count,)).astype(dt, copy=True) if (count and p) else None
+	off = take(lib.b200mvs_pointcloud_view_offsets, m+1, np.uint32)
+	total = int(off[-1]) if off is not None else 0
+	pts = take(lib.b200mvs_pointcloud_points, 3*m, np.float32)
+	vs = take(lib.b200mvs_pointcloud_views, total, np.uint32); ws = take(lib.b200mvs_pointcloud_weights, total, np.float32)
+	pj = take(lib.b200mvs_pointcloud_projs, 2*total, np.uint16)
+	nr = take(lib.b200mvs_pointcloud_normals, 3*m, np.float32); cl = take(lib.b200mvs_pointcloud_colors, 3*m, np.uint8)
+	return PointCloud(points=pts.reshape(-1, 3) if pts is not None else np.zeros((0, 3), np.float32),
+		pointViews=[vs[off[i]:off[i+1]] for i in range(m)], pointWeights=[ws[off[i]:off[i+1]] for i in range(m)],
+		colors=None if cl is None else cl.reshape(-1, 3), normals=None if nr is None else nr.reshape(-1, 3),
+		projs=[pj[2*off[i]:2*off[i+1]].reshape(-1, 2) for i in range(m)], nDepths=int(lib.b200mvs_pointcloud_depths(cloud)))
+
+
+def FuseRoundStats():
+	"""What each round (image) of the last device FuseDepthMaps call on each device did: {device index: list of dicts with image,
+	iterations (of the acceptance fixed point), candidates, edges (claim and zero), shared (edges whose neighbour pixel another
+	candidate also reaches) and ms (device time)}."""
+	out = {}
+	for index, ctx in _DEVICE_CTX.items():
+		n = C.c_int()
+		ctx._call("fuse_round_stats", 0, C.byref(n), None, None, None, None, None, None)
+		m = n.value
+		img, it = np.zeros(m, np.int32), np.zeros(m, np.int32)
+		cand, edges, shared, ms = np.zeros(m, np.uint64), np.zeros(m, np.uint64), np.zeros(m, np.uint64), np.zeros(m, np.float32)
+		ctx._call("fuse_round_stats", m, C.byref(n), img.ctypes.data_as(C.POINTER(C.c_int)), it.ctypes.data_as(C.POINTER(C.c_int)),
+			cand.ctypes.data, edges.ctypes.data, shared.ctypes.data, ms.ctypes.data)
+		out[index] = [dict(image=int(img[i]), iterations=int(it[i]), candidates=int(cand[i]), edges=int(edges[i]), shared=int(shared[i]),
+			ms=float(ms[i])) for i in range(m)]
+	return out

@@ -152,6 +152,8 @@ PROTOTYPES = {
 	"b200mvs_scale_image_device": (I, [P, P, I, I, I, F, P, IP, P]),
 	"b200mvs_fuse_default_params": (None, [C.POINTER(FuseParams)]),
 	"b200mvs_fuse_depth_maps": (I, [C.POINTER(FuseView), I, C.POINTER(FuseParams), PP]),
+	"b200mvs_fuse_depth_maps_device": (I, [P, C.POINTER(FuseView), I, C.POINTER(FuseParams), PP, P, PStats]),
+	"b200mvs_fuse_round_stats": (I, [P, I, IP, IP, IP, P, P, P, P]),
 	"b200mvs_pointcloud_size": (U64, [P]),
 	"b200mvs_pointcloud_depths": (U64, [P]),
 	"b200mvs_pointcloud_points": (C.POINTER(F), [P]),
