@@ -30,7 +30,9 @@ struct SegArc { int src, dst, srcSize, dstSize, srcKey, dstKey; };
 
 cudaError_t flt_launch_filter(const FltParams& P, int maxNbrPixels, bool adjust, cudaStream_t s);
 cudaError_t flt_launch_resolve(const unsigned long long* z, const float* nbrConf, size_t np, float* depth, float* conf, cudaStream_t s);
-cudaError_t seg_launch_label(const float* depth, int W, int H, float th, int* labels, int* sizes, int* minKey, void* arcs, int* count, int cap, cudaStream_t s);
+// the two RemoveSmallSegments launchers add the number of kernels they start to `launches`
+cudaError_t seg_launch_label(const float* depth, int W, int H, float th, int* labels, int* sizes, int* minKey, void* arcs, int* count, int cap,
+	int& launches, cudaStream_t s);
 cudaError_t seg_launch_remove(float* depth, float* normal, float* conf, int W, int H, unsigned speckle, const int* labels, int* sizes,
-	const int* patch, int nPatch, cudaStream_t s);
+	const int* patch, int nPatch, int& launches, cudaStream_t s);
 cudaError_t gap_launch(float* depth, float* normal, float* conf, float* tDepth, float* tNormal, float* tConf, int W, int H, float th, int gap, cudaStream_t s);

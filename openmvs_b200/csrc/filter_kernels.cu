@@ -15,6 +15,7 @@
 // HBM-bound integer/float work: per reference pixel the vote reads 8 B x N keys + 8 B and
 // writes 8 B; the splat reads 4 B and issues <= 4 atomics per neighbour pixel.
 #include "filter_common.cuh"
+#include "label_common.cuh"
 
 namespace {
 
@@ -178,73 +179,13 @@ __global__ void flt_resolve_kernel(const unsigned long long* z, const float* nbr
 //   3. replay the reference's loop on that condensed graph on the host — components in seed order, a segment = every
 //      not-yet-visited component reachable along arcs — and patch the sizes of the components involved;
 //   4. remove the pixels whose segment is smaller than nSpeckleSize.
-// Labelling: every pixel first links to its left (else upper) connected neighbour — a region that is
-// reasonably convex becomes one tree: row runs hang on their first pixel, which hangs on the row above —
-// pointer jumping flattens these chains in ceil(log2(W+H)) rounds, the upper edges the links did not
-// take are merged by an atomicMin union on the flat trees (mostly "same root already"), and a second
-// series of jumps flattens whatever chains of roots the unions built.
-__device__ __forceinline__ bool seg_edge(float a, float b, float th) {
-	return b > 0 && depth_similar(a, b, th) && depth_similar(b, a, th);
-}
-__device__ __forceinline__ int uf_find(int* L, int i) {
-	int p;
-	while ((p = ((volatile int*)L)[i]) != i) i = p;
-	return i;
-}
-__device__ void uf_union(int* L, int a, int b) {
-	bool done;
-	do {
-		a = uf_find(L, a); b = uf_find(L, b);
-		if (a < b) { const int old = atomicMin(L+b, a); done = (old == b); b = old; }
-		else if (b < a) { const int old = atomicMin(L+a, b); done = (old == a); a = old; }
-		else done = true;
-	} while (!done);
-}
-__global__ void seg_init_kernel(const float* __restrict__ depth, int* L, int* size, int* minKey, int W, int H, float th) {
-	const int x = blockIdx.x*blockDim.x+threadIdx.x, y = blockIdx.y*blockDim.y+threadIdx.y;
-	if (x >= W || y >= H) return;
-	const int i = y*W+x;
-	const float a = depth[i];
-	int l = -1;
-	if (a > 0) {
-		l = i;
-		if (x > 0 && seg_edge(a, depth[i-1], th)) l = i-1;
-		else if (y > 0 && seg_edge(a, depth[i-W], th)) l = i-W;
-	}
-	L[i] = l;
-	size[i] = 0;
-	minKey[i] = 0x7FFFFFFF;
-}
-__global__ void seg_jump_kernel(int* L, int n) {
-	const int i = blockIdx.x*blockDim.x+threadIdx.x;
-	if (i >= n) return;
-	const int p = L[i];
-	if (p >= 0 && p != i) L[i] = ((volatile int*)L)[p]; // labels only ever move towards the root: safe in place
-}
-__global__ void seg_merge_kernel(const float* __restrict__ depth, int* L, int W, int H, float th) {
-	const int x = blockIdx.x*blockDim.x+threadIdx.x, y = blockIdx.y*blockDim.y+threadIdx.y;
-	if (x < 1 || x >= W || y < 1 || y >= H) return;
-	const int i = y*W+x;
-	const float a = depth[i];
-	if (!(a > 0)) return;
-	// the link went left; the upper edge is still open
-	if (seg_edge(a, depth[i-1], th) && seg_edge(a, depth[i-W], th)) uf_union(L, i, i-W);
-}
-// sizes of the components and their first pixel in the reference's seed order (x outer, y inner: key = x*H + y)
-__global__ void seg_count_kernel(int* L, int* size, int* minKey, int W, int H) {
-	const int n = W*H;
-	const int i = blockIdx.x*blockDim.x+threadIdx.x;
-	int r = -1, key = 0x7FFFFFFF;
-	if (i < n && L[i] >= 0) {
-		r = uf_find(L, i);
-		L[i] = r;                   // roots keep L[r] == r, so concurrent finds stay correct
-		key = (i%W)*H + i/W;
-	}
-	// one atomic per distinct root in the warp (large segments would otherwise serialise on one address)
-	const unsigned peers = __match_any_sync(0xFFFFFFFFu, r);
-	const int kmin = __reduce_min_sync(peers, key);
-	if (r >= 0 && (threadIdx.x&31) == __ffs(peers)-1) { atomicAdd(size+r, __popc(peers)); atomicMin(minKey+r, kmin); }
-}
+// The labelling is label_common.cuh's; the seed keys are its minKey (the reference's seeds are column-major).
+struct SegEdge {
+	const float* depth; float th;
+	__device__ float at(int i) const { return __ldg(depth+i); }
+	__device__ bool valid(float a) const { return a > 0; }
+	__device__ bool edge(float a, float b) const { return b > 0 && depth_similar(a, b, th) && depth_similar(b, a, th); }
+};
 __global__ void seg_arcs_kernel(const float* __restrict__ depth, const int* __restrict__ L, const int* __restrict__ size, const int* __restrict__ minKey,
 	int W, int H, float th, SegArc* arcs, int* count, int cap)
 {
@@ -351,28 +292,22 @@ cudaError_t flt_launch_resolve(const unsigned long long* z, const float* nbrConf
 }
 
 // phase 1: two-way components, their sizes / seed keys, the arcs; *count (device) receives the number of arcs found
-cudaError_t seg_launch_label(const float* depth, int W, int H, float th, int* labels, int* sizes, int* minKey, void* arcs, int* count, int cap, cudaStream_t s) {
-	const int n = W*H;
+cudaError_t seg_launch_label(const float* depth, int W, int H, float th, int* labels, int* sizes, int* minKey, void* arcs, int* count, int cap,
+	int& launches, cudaStream_t s) {
 	const dim3 b2(32, 8), g2((W+31)/32, (H+7)/8);
 	cudaMemsetAsync(count, 0, sizeof(int), s);
-	seg_init_kernel<<<g2, b2, 0, s>>>(depth, labels, sizes, minKey, W, H, th);
-	int rounds = 1;
-	while ((1<<rounds) < W+H) ++rounds;
-	for (int r = 0; r < rounds; ++r)
-		seg_jump_kernel<<<(n+255)/256, 256, 0, s>>>(labels, n);
-	seg_merge_kernel<<<g2, b2, 0, s>>>(depth, labels, W, H, th);
-	for (int r = 0; r < rounds; ++r)
-		seg_jump_kernel<<<(n+255)/256, 256, 0, s>>>(labels, n);
-	seg_count_kernel<<<(n+255)/256, 256, 0, s>>>(labels, sizes, minKey, W, H);
+	launches += label_launch(SegEdge{depth, th}, W, H, labels, sizes, minKey, s);
 	seg_arcs_kernel<<<g2, b2, 0, s>>>(depth, labels, sizes, minKey, W, H, th, (SegArc*)arcs, count, cap);
+	++launches;
 	return cudaGetLastError();
 }
 // phase 2: sizes of the components the arcs join replaced by the sizes of their breadth-first segments, then the removal
 cudaError_t seg_launch_remove(float* depth, float* normal, float* conf, int W, int H, unsigned speckle, const int* labels, int* sizes,
-	const int* patch, int nPatch, cudaStream_t s) {
+	const int* patch, int nPatch, int& launches, cudaStream_t s) {
 	const int n = W*H;
-	if (nPatch > 0) seg_patch_kernel<<<(nPatch+255)/256, 256, 0, s>>>((const int2*)patch, nPatch, sizes);
+	if (nPatch > 0) { seg_patch_kernel<<<(nPatch+255)/256, 256, 0, s>>>((const int2*)patch, nPatch, sizes); ++launches; }
 	seg_remove_kernel<<<(n+255)/256, 256, 0, s>>>(labels, sizes, n, speckle, depth, normal, conf);
+	++launches;
 	return cudaGetLastError();
 }
 

@@ -38,12 +38,12 @@ struct b200mvs_ctx {
 	cudaStream_t stream = nullptr;
 	cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 	// grow-only device scratch
-	std::vector<DevBuf> imgs, dmaps, img8;    // staged images / depth-maps / 8-bit colour images (host API; gray images converted on the device)
+	DevBuf stage;                             // the host forms' staged inputs and outputs (HostCall)
+	std::vector<DevBuf> imgs;                 // gray images converted on the device from 8-bit colour views (toGray)
 	std::vector<DevBuf> pyr;                  // per-view pyramid levels (all levels packed)
 	DevBuf plane, cost, best, prior, lowPlane;
-	DevBuf dDepth, dNormal, dConf, dViews;    // level scratch / staging of the maps (host API)
-	DevBuf mapD, mapN;                        // full-resolution in/out maps (host API)
-	DevBuf sgL, sgC, sgR, sgPx, sgCosts, sgAccums, sgAccums2, sgDisp, sgCost, sgMax; // SGM staging / scratch
+	DevBuf dDepth, dNormal;                   // the initial estimate at the coarsest level
+	DevBuf sgCosts, sgAccums, sgAccums2, sgMax; // SGM scratch
 	// wave-front aggregation: cached schedule of the last (size, mode) and its scratch
 	struct FrontPass { FrontLaunch launch; DevBuf items, need; int nItems = 0; };   // launch.items is emptied once uploaded
 	std::vector<FrontPass> sgFront; int sgFrontKey[6] = {0, 0, 0, 0, 0, 0};
@@ -55,9 +55,9 @@ struct b200mvs_ctx {
 	enum { TS_IMG, TS_MASKL, TS_MASKR, TS_MASKT, TS_DL, TS_DR, TS_DL0, TS_DR0, TS_PXL, TS_PXR, TS_RANGES, TS_SCAN, TS_KEYS, TS_LABELS,
 		TS_SIZES, TS_SMALL, TS_COUNT };
 	DevBuf ts[TS_COUNT];
-	DevBuf sfKeys, sfMaps, sfIn, sfOut;       // SGM fusion: splat keys, per-pair depth / range / conf maps, staged pairs and outputs (host API)
-	DevBuf fltZ, fltIn, fltOutD, fltOutC;     // FilterDepthMap: z-buffer keys, staged maps (host API), outputs
-	DevBuf ppA, ppB, ppD, ppN, ppC;           // RemoveSmallSegments labels/sizes, GapInterpolation temporaries, staging
+	DevBuf sfKeys, sfMaps;                    // SGM fusion: splat keys, per-pair depth / range / conf maps
+	DevBuf fltZ;                              // FilterDepthMap: z-buffer keys
+	DevBuf ppA, ppB, ppN;                     // RemoveSmallSegments labels/sizes, GapInterpolation temporaries
 	DevBuf ppK, ppArcs, ppPatch;              // RemoveSmallSegments: seed keys, one-way edges (+ counter), patched segment sizes
 	// FuseDepthMaps (device form): view table, neighbour lists, claim maps, per-round candidate / edge scratch, counters, the growing
 	// point-cloud outputs, and what each round of the last call did (b200mvs_fuse_round_stats)
@@ -104,3 +104,65 @@ inline int fill_stats(b200mvs_ctx* ctx, b200mvs_stats* stats, std::chrono::stead
 	stats->bytes_h2d = h2d; stats->bytes_d2h = d2h;
 	return B200MVS_OK;
 }
+
+// One call of a host form on ctx->stream: the caller's host buffers are staged in the context's device arena (ctx->stage), the
+// device form runs between ctx->ev0 and ctx->ev1, and the outputs are copied back.  Declare every buffer with in / out / inout,
+// each with the device pointer the call should set; stage() sets them and enqueues the H2D copies; run() then does the rest and
+// waits, or enqueue() leaves it pending for b200mvs_sync.  bytes_h2d / bytes_d2h are the bytes copied.
+struct HostCall {
+	b200mvs_ctx* ctx;
+	const std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
+	uint64_t h2d = 0, d2h = 0;
+	bool formRecordsEvents = false;   // the device form records ev0 / ev1 itself (b200mvs_sgm_match_device with statistics)
+
+	explicit HostCall(b200mvs_ctx* c) : ctx(c) {}
+	// `rows` rows of `row` bytes, `pitch` bytes apart on the host (0: packed); packed on the device
+	template <typename T> void in(T*& dev, const void* host, size_t row, int rows = 1, size_t pitch = 0) {
+		slices.push_back({&dev, host, nullptr, row, pitch ? pitch : row, rows, 0});
+	}
+	template <typename T> void out(T*& dev, void* host, size_t bytes) { slices.push_back({&dev, nullptr, host, bytes, bytes, 1, 0}); }
+	template <typename T> void inout(T*& dev, void* host, size_t bytes) { slices.push_back({&dev, host, host, bytes, bytes, 1, 0}); }
+
+	int stage() {
+		size_t total = 0;
+		for (Slice& s: slices) { s.off = total; total += (s.row*s.rows+255) & ~(size_t)255; }  // 256-byte aligned, as cudaMalloc's
+		CK(ctx->stage.reserve(total));
+		for (Slice& s: slices) {
+			void* p = ctx->stage.as<uint8_t>()+s.off;
+			memcpy(s.dev, &p, sizeof(p));
+			if (!s.src) continue;
+			if (s.pitch == s.row) CK(cudaMemcpyAsync(p, s.src, s.row*s.rows, cudaMemcpyHostToDevice, ctx->stream));
+			else CK(cudaMemcpy2DAsync(p, s.row, s.src, s.pitch, s.row, s.rows, cudaMemcpyHostToDevice, ctx->stream));
+			h2d += s.row*s.rows;
+		}
+		return B200MVS_OK;
+	}
+	// form(stream) is the device form on the staged buffers
+	template <typename F> int run(F&& form, b200mvs_stats* stats) {
+		if (int rc = launch(form)) return rc;
+		CK(cudaStreamSynchronize(ctx->stream));
+		return stats ? fill_stats(ctx, stats, t0, 1, h2d, d2h) : B200MVS_OK;
+	}
+	template <typename F> int enqueue(F&& form, int levels) {
+		if (int rc = launch(form)) return rc;
+		ctx->t0 = t0; ctx->pendH2D = h2d; ctx->pendD2H = d2h; ctx->pendLevels = levels;
+		ctx->pending = true;
+		return B200MVS_OK;
+	}
+
+private:
+	struct Slice { void* dev; const void* src; void* dst; size_t row, pitch; int rows; size_t off; };
+	std::vector<Slice> slices;
+
+	template <typename F> int launch(F& form) {
+		if (!formRecordsEvents) CK(cudaEventRecord(ctx->ev0, ctx->stream));
+		if (int rc = form(ctx->stream)) return rc;
+		if (!formRecordsEvents) CK(cudaEventRecord(ctx->ev1, ctx->stream));
+		for (const Slice& s: slices) {
+			if (!s.dst) continue;
+			CK(cudaMemcpyAsync(s.dst, ctx->stage.as<uint8_t>()+s.off, s.row, cudaMemcpyDeviceToHost, ctx->stream));
+			d2h += s.row;
+		}
+		return B200MVS_OK;
+	}
+};

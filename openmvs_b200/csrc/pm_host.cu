@@ -145,24 +145,11 @@ Rows image_rows(const b200mvs_view& v) {
 }
 Rows depth_rows(const b200mvs_view& v) { return rows_of(v.depth, (size_t)v.dwidth*sizeof(float), v.dstride_bytes, v.dheight); }
 
-enum class Residency { Host, Device };
-
-// The engine's views of the caller's: device float images and depth-maps with their pitch in floats.  Host views are
-// uploaded packed into the context's scratch on stream s (h2d: the bytes copied); an 8-bit colour image is converted to
-// gray on the device (toGray) in either residency; device float images and depth-maps are used in place.
-int stage_views(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, Residency res, cudaStream_t s,
-	std::vector<DView>& dv, uint64_t& h2d)
-{
-	const bool host = res == Residency::Host;
-	auto upload = [&](DevBuf& b, const Rows& r) {
-		cudaError_t e = b.reserve(r.row*r.rows);
-		if (e == cudaSuccess) e = cudaMemcpy2DAsync(b.p, r.row, r.p, r.pitch, r.row, r.rows, cudaMemcpyHostToDevice, s);
-		if (e == cudaSuccess) h2d += r.row*r.rows;
-		return e;
-	};
-	if ((int)ctx->imgs.size() < nViews) { ctx->imgs.resize(nViews); ctx->dmaps.resize(nViews); ctx->img8.resize(nViews); }
+// The engine's views of the caller's device views: float images and depth-maps with their pitch in floats.  Float images and
+// depth-maps are used in place; an 8-bit colour image is converted to gray (toGray) into the context's scratch on stream s.
+int stage_views(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, cudaStream_t s, std::vector<DView>& dv) {
+	if ((int)ctx->imgs.size() < nViews) ctx->imgs.resize(nViews);
 	dv.resize(nViews);
-	h2d = 0;
 	for (int i = 0; i < nViews; ++i) {
 		const b200mvs_view& v = views[i];
 		const Rows im = image_rows(v), dm = depth_rows(v);
@@ -170,27 +157,15 @@ int stage_views(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, Residen
 		d.w = v.width; d.h = v.height; d.dw = v.dwidth; d.dh = v.dheight;
 		memcpy(d.K, v.K, sizeof(d.K)); memcpy(d.R, v.R, sizeof(d.R)); memcpy(d.C, v.C, sizeof(d.C));
 		memcpy(d.Kd, v.Kd, sizeof(d.Kd)); memcpy(d.Rd, v.Rd, sizeof(d.Rd)); memcpy(d.Cd, v.Cd, sizeof(d.Cd));
-		if (v.image && !host) {
+		if (v.image) {
 			d.img = v.image; d.pitch = (int)(im.pitch/sizeof(float));
 		} else {
 			CK(ctx->imgs[i].reserve((size_t)v.width*v.height*sizeof(float)));
 			d.img = ctx->imgs[i].as<float>(); d.pitch = v.width;
-			const void* src = im.p; size_t pitch = im.pitch;
-			if (host) {
-				DevBuf& b = v.image ? ctx->imgs[i] : ctx->img8[i];
-				CK(upload(b, im));
-				src = b.p; pitch = im.row;
-			}
-			if (!v.image) {
-				CK(rs_launch_to_gray((const uint8_t*)src, v.width, v.height, (int)pitch, v.channels8, v.bgr8 != 0, ctx->imgs[i].as<float>(),
-					v.width, s)); ++ctx->launches;
-			}
+			CK(rs_launch_to_gray(v.image8, v.width, v.height, (int)im.pitch, v.channels8, v.bgr8 != 0, ctx->imgs[i].as<float>(), v.width, s));
+			++ctx->launches;
 		}
 		d.dmap = v.depth; d.dpitch = (int)(dm.pitch/sizeof(float));
-		if (v.depth && host) {
-			CK(upload(ctx->dmaps[i], dm));
-			d.dmap = ctx->dmaps[i].as<float>(); d.dpitch = v.dwidth;
-		}
 	}
 	return B200MVS_OK;
 }
@@ -415,9 +390,8 @@ int b200mvs_estimate_device(b200mvs_ctx* ctx, const b200mvs_view* views, int nVi
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t s = stream_of(ctx, stream);
 	std::vector<DView> dv;
-	uint64_t h2d;
 	ctx->launches = 0;
-	rc = stage_views(ctx, views, nViews, Residency::Device, s, dv, h2d);
+	rc = stage_views(ctx, views, nViews, s, dv);
 	if (rc) return rc;
 	const auto t0 = std::chrono::steady_clock::now();
 	ctx->nSweepEv = 0; ctx->timeSweeps = stats != nullptr;
@@ -438,34 +412,28 @@ int b200mvs_estimate_async(b200mvs_ctx* ctx, const b200mvs_view* views, int nVie
 	int rc = check_estimate(ctx, views, nViews, dMin, dMax, depth, normal, conf);
 	if (rc) return rc;
 	CK(cudaSetDevice(ctx->device));
-	cudaStream_t s = ctx->stream;
-	ctx->t0 = std::chrono::steady_clock::now();
-	std::vector<DView> dv;
-	uint64_t h2d, d2h = 0;
-	ctx->launches = 0;
-	rc = stage_views(ctx, views, nViews, Residency::Host, s, dv, h2d);
-	if (rc) return rc;
+	HostCall call(ctx);
+	std::vector<b200mvs_view> dev(views, views+nViews);   // the views with staged, packed images and depth-maps
+	for (b200mvs_view& v: dev) {
+		const Rows im = image_rows(v), dm = depth_rows(v);
+		if (v.image) call.in(v.image, im.p, im.row, im.rows, im.pitch);
+		else call.in(v.image8, im.p, im.row, im.rows, im.pitch);
+		if (v.depth) call.in(v.depth, dm.p, dm.row, dm.rows, dm.pitch);
+		v.stride_bytes = v.stride8_bytes = v.dstride_bytes = 0;
+	}
 	const size_t P0 = (size_t)views[0].width*views[0].height;
-	DevBuf& dD = ctx->mapD; DevBuf& dN = ctx->mapN;
-	CK(dD.reserve(P0*sizeof(float))); CK(dN.reserve(P0*3*sizeof(float)));
-	CK(ctx->dConf.reserve(P0*sizeof(float))); CK(ctx->dViews.reserve(P0*sizeof(uint32_t)));
-	CK(cudaMemcpyAsync(dD.p, depth, P0*sizeof(float), cudaMemcpyHostToDevice, s));
-	CK(cudaMemcpyAsync(dN.p, normal, P0*3*sizeof(float), cudaMemcpyHostToDevice, s));
-	h2d += P0*16;
-	ctx->nSweepEv = 0; ctx->timeSweeps = true;
-	CK(cudaEventRecord(ctx->ev0, s));
-	rc = estimate_on_device(ctx, dv.data(), nViews, dMin, dMax, nGeometricIter, dD.as<float>(), dN.as<float>(),
-		ctx->dConf.as<float>(), ctx->dViews.as<uint32_t>(), s);
+	float *dD, *dN, *dC; uint32_t* dV = nullptr;
+	call.inout(dD, depth, P0*sizeof(float)); call.inout(dN, normal, P0*3*sizeof(float)); call.out(dC, conf, P0*sizeof(float));
+	if (viewsMap) call.out(dV, viewsMap, P0*sizeof(uint32_t));
+	if ((rc = call.stage())) return rc;
+	std::vector<DView> dv;
+	ctx->launches = 0;
+	rc = stage_views(ctx, dev.data(), nViews, ctx->stream, dv);   // toGray runs before ev0, as in b200mvs_estimate_device
 	if (rc) return rc;
-	CK(cudaEventRecord(ctx->ev1, s));
-	CK(cudaMemcpyAsync(depth, dD.p, P0*sizeof(float), cudaMemcpyDeviceToHost, s));
-	CK(cudaMemcpyAsync(normal, dN.p, P0*3*sizeof(float), cudaMemcpyDeviceToHost, s));
-	CK(cudaMemcpyAsync(conf, ctx->dConf.p, P0*sizeof(float), cudaMemcpyDeviceToHost, s));
-	d2h += P0*20;
-	if (viewsMap) { CK(cudaMemcpyAsync(viewsMap, ctx->dViews.p, P0*4, cudaMemcpyDeviceToHost, s)); d2h += P0*4; }
-	ctx->pendH2D = h2d; ctx->pendD2H = d2h; ctx->pendLevels = (nGeometricIter < 0 ? ctx->prm.nSubResolutionLevels : 0)+1;
-	ctx->pending = true;
-	return B200MVS_OK;
+	ctx->nSweepEv = 0; ctx->timeSweeps = true;
+	return call.enqueue([&](cudaStream_t s) {
+		return estimate_on_device(ctx, dv.data(), nViews, dMin, dMax, nGeometricIter, dD, dN, dC, dV, s);
+	}, (nGeometricIter < 0 ? ctx->prm.nSubResolutionLevels : 0)+1);
 }
 
 int b200mvs_sync(b200mvs_ctx* ctx, b200mvs_stats* stats) {
@@ -550,8 +518,7 @@ static int block_params(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews,
 	for (int i = 0; i < nViews; ++i)
 		if (!views[i].image) return fail(ctx, B200MVS_ERR_ARG, "the building blocks take float gray images");
 	std::vector<DView> dv;
-	uint64_t h2d;
-	rc = stage_views(ctx, views, nViews, Residency::Device, s, dv, h2d);
+	rc = stage_views(ctx, views, nViews, s, dv);
 	if (rc) return rc;
 	if (tmap) { rc = prepare_ref_tmap(ctx, dv[0], s); if (rc) return rc; }
 	build_params(ctx->prm, dv.data(), nViews, dMin, dMax, lowres, (float4*)plane4, cost, nullptr, P, geom);

@@ -81,36 +81,21 @@ int b200mvs_filter_depth_map(b200mvs_ctx* ctx, const b200mvs_dmap* ref, const b2
 	if (rc) return rc;
 	if (nNbrs < prm->nMinViews || nNbrs < prm->nMinViewsAdjust) { if (filtered) *filtered = 0; return B200MVS_OK; }
 	CK(cudaSetDevice(ctx->device));
-	cudaStream_t s = ctx->stream;
-	const auto t0 = std::chrono::steady_clock::now();
-	// stage every map once: [ref depth | ref conf | nbr0 depth | nbr0 conf | ...]
-	size_t total = 0;
-	for (int i = -1; i < nNbrs; ++i) { const b200mvs_dmap& m = i < 0 ? *ref : nbrs[i]; total += (size_t)m.width*m.height*2; }
-	const size_t np = (size_t)ref->width*ref->height;
-	CK(ctx->fltIn.reserve(total*4)); CK(ctx->fltOutD.reserve(np*4)); CK(ctx->fltOutC.reserve(np*4));
-	std::vector<b200mvs_dmap> dv(nNbrs+1);
-	float* p = ctx->fltIn.as<float>();
-	uint64_t h2d = 0;
-	for (int i = -1; i < nNbrs; ++i) {
-		const b200mvs_dmap& m = i < 0 ? *ref : nbrs[i];
-		const size_t n = (size_t)m.width*m.height;
-		b200mvs_dmap& d = dv[i+1];
-		d = m;
-		CK(cudaMemcpyAsync(p, m.depth, n*4, cudaMemcpyHostToDevice, s)); d.depth = p; p += n; h2d += n*4;
-		d.conf = nullptr;
-		if (m.conf) { CK(cudaMemcpyAsync(p, m.conf, n*4, cudaMemcpyHostToDevice, s)); d.conf = p; h2d += n*4; }
-		p += n;
+	HostCall call(ctx);
+	std::vector<b200mvs_dmap> dv(ref, ref+1);   // the reference, then the neighbours, with staged maps
+	dv.insert(dv.end(), nbrs, nbrs+nNbrs);
+	for (b200mvs_dmap& d: dv) {
+		const size_t bytes = (size_t)d.width*d.height*sizeof(float);
+		call.in(d.depth, d.depth, bytes);
+		if (d.conf) call.in(d.conf, d.conf, bytes);
 	}
-	CK(cudaEventRecord(ctx->ev0, s));
-	rc = b200mvs_filter_depth_map_device(ctx, &dv[0], dv.data()+1, nNbrs, prm, dMin, dMax, ctx->fltOutD.as<float>(), ctx->fltOutC.as<float>(),
-		nullptr, nullptr, filtered, s);
-	if (rc) return rc;
-	CK(cudaEventRecord(ctx->ev1, s));
-	CK(cudaMemcpyAsync(outDepth, ctx->fltOutD.p, np*4, cudaMemcpyDeviceToHost, s));
-	CK(cudaMemcpyAsync(outConf, ctx->fltOutC.p, np*4, cudaMemcpyDeviceToHost, s));
-	CK(cudaStreamSynchronize(s));
-	if (stats) return fill_stats(ctx, stats, t0, 1, h2d, np*8);
-	return B200MVS_OK;
+	const size_t np = (size_t)ref->width*ref->height;
+	float *dOutD, *dOutC;
+	call.out(dOutD, outDepth, np*sizeof(float)); call.out(dOutC, outConf, np*sizeof(float));
+	if ((rc = call.stage())) return rc;
+	return call.run([&](cudaStream_t s) {
+		return b200mvs_filter_depth_map_device(ctx, &dv[0], dv.data()+1, nNbrs, prm, dMin, dMax, dOutD, dOutC, nullptr, nullptr, filtered, s);
+	}, stats);
 }
 
 int b200mvs_remove_small_segments_device(b200mvs_ctx* ctx, float* depth, float* normal, float* conf, int width, int height,
@@ -128,7 +113,8 @@ int b200mvs_remove_small_segments_device(b200mvs_ctx* ctx, float* depth, float* 
 	CK(ctx->ppArcs.reserve(sizeof(int)*4 + (size_t)cap*sizeof(SegArc)));
 	int* count = ctx->ppArcs.as<int>();
 	SegArc* arcs = (SegArc*)(ctx->ppArcs.as<int>()+4);
-	CK(seg_launch_label(depth, width, height, th, ctx->ppA.as<int>(), ctx->ppB.as<int>(), ctx->ppK.as<int>(), arcs, count, cap, s));
+	int launches = 0;
+	CK(seg_launch_label(depth, width, height, th, ctx->ppA.as<int>(), ctx->ppB.as<int>(), ctx->ppK.as<int>(), arcs, count, cap, launches, s));
 	// the condensed graph is resolved on the host: one small read-back (the call synchronises the stream)
 	int nArcs = 0;
 	CK(cudaMemcpyAsync(&nArcs, count, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -139,35 +125,16 @@ int b200mvs_remove_small_segments_device(b200mvs_ctx* ctx, float* depth, float* 
 		std::vector<SegArc> h(nArcs);
 		CK(cudaMemcpyAsync(h.data(), arcs, (size_t)nArcs*sizeof(SegArc), cudaMemcpyDeviceToHost, s));
 		CK(cudaStreamSynchronize(s));
-		// nodes: the components an arc touches; replay of the reference's loop (SceneDensify.cpp:828-895) on them
+		// nodes: the components an arc touches, sorted by label; replay of the reference's loop (SceneDensify.cpp:828-895) on them
 		struct Node { int label, size, key; std::vector<int> out; int seg = -1; };
 		std::vector<Node> nodes;
-		std::vector<std::pair<int, int>> index; // (label, node)
-		auto node_of = [&](int label, int size, int key) {
-			for (auto& p: index) if (p.first == label) return p.second;  // few nodes: linear search is fine ...
-			index.push_back({label, (int)nodes.size()});
-			Node nd; nd.label = label; nd.size = size; nd.key = key; nodes.push_back(nd);
-			return (int)nodes.size()-1;
+		for (const SegArc& a: h) { nodes.push_back({a.src, a.srcSize, a.srcKey}); nodes.push_back({a.dst, a.dstSize, a.dstKey}); }
+		std::sort(nodes.begin(), nodes.end(), [](const Node& x, const Node& y) { return x.label < y.label; });
+		nodes.erase(std::unique(nodes.begin(), nodes.end(), [](const Node& x, const Node& y) { return x.label == y.label; }), nodes.end());
+		auto node_of = [&](int label) {
+			return (int)(std::lower_bound(nodes.begin(), nodes.end(), label, [](const Node& x, int l) { return x.label < l; })-nodes.begin());
 		};
-		if (nArcs > 4096) {  // ... but not for pathological maps: sort once and search
-			std::sort(h.begin(), h.end(), [](const SegArc& a, const SegArc& b) { return a.src != b.src ? a.src < b.src : a.dst < b.dst; });
-		}
-		std::vector<std::pair<int, int>> sortedIndex;
-		if (nArcs > 4096) {
-			std::vector<std::pair<int, std::pair<int, int>>> all; // label -> (size, key)
-			for (auto& a: h) { all.push_back({a.src, {a.srcSize, a.srcKey}}); all.push_back({a.dst, {a.dstSize, a.dstKey}}); }
-			std::sort(all.begin(), all.end());
-			all.erase(std::unique(all.begin(), all.end(), [](const auto& x, const auto& y) { return x.first == y.first; }), all.end());
-			for (auto& e: all) { Node nd; nd.label = e.first; nd.size = e.second.first; nd.key = e.second.second; sortedIndex.push_back({e.first, (int)nodes.size()}); nodes.push_back(nd); }
-		}
-		auto find_node = [&](int label, int size, int key) {
-			if (sortedIndex.empty()) return node_of(label, size, key);
-			return std::lower_bound(sortedIndex.begin(), sortedIndex.end(), std::make_pair(label, -1))->second;
-		};
-		for (auto& a: h) {
-			const int u = find_node(a.src, a.srcSize, a.srcKey), v = find_node(a.dst, a.dstSize, a.dstKey);
-			nodes[u].out.push_back(v);
-		}
+		for (const SegArc& a: h) nodes[node_of(a.src)].out.push_back(node_of(a.dst));
 		std::vector<int> order(nodes.size());
 		for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
 		std::sort(order.begin(), order.end(), [&](int a, int b) { return nodes[a].key < nodes[b].key; });
@@ -189,8 +156,9 @@ int b200mvs_remove_small_segments_device(b200mvs_ctx* ctx, float* depth, float* 
 		CK(cudaMemcpyAsync(ctx->ppPatch.p, patch.data(), patch.size()*sizeof(int), cudaMemcpyHostToDevice, s));
 		CK(cudaStreamSynchronize(s)); // `patch` is a local
 	}
-	CK(seg_launch_remove(depth, normal, conf, width, height, nSpeckleSize, ctx->ppA.as<int>(), ctx->ppB.as<int>(), ctx->ppPatch.as<int>(), nPatch, s));
-	{ int rounds = 1; while ((1<<rounds) < width+height) ++rounds; ctx->launches = 5+2*rounds+(nPatch > 0 ? 1 : 0); }
+	CK(seg_launch_remove(depth, normal, conf, width, height, nSpeckleSize, ctx->ppA.as<int>(), ctx->ppB.as<int>(), ctx->ppPatch.as<int>(), nPatch,
+		launches, s));
+	ctx->launches = launches;
 	return B200MVS_OK;
 }
 
@@ -210,43 +178,34 @@ int b200mvs_gap_interpolation_device(b200mvs_ctx* ctx, float* depth, float* norm
 	return B200MVS_OK;
 }
 
-// host form of the two in-place passes: stage, run, copy back
-static int pp_host(b200mvs_ctx* ctx, int which, float* depth, float* normal, float* conf, int width, int height, float th, unsigned arg, b200mvs_stats* stats) {
+// host form of the two in-place passes: stage the maps, run the device form on them, copy them back
+typedef int (*PPDeviceForm)(b200mvs_ctx*, float*, float*, float*, int, int, float, unsigned, void*);
+static int pp_host(b200mvs_ctx* ctx, PPDeviceForm form, float* depth, float* normal, float* conf, int width, int height, float th, unsigned arg,
+	b200mvs_stats* stats)
+{
 	if (!ctx) return B200MVS_ERR_ARG;
 	if (!depth || width <= 0 || height <= 0) return fail(ctx, B200MVS_ERR_ARG, "post-processing: invalid argument");
 	CK(cudaSetDevice(ctx->device));
-	cudaStream_t s = ctx->stream;
-	const auto t0 = std::chrono::steady_clock::now();
+	HostCall call(ctx);
 	const size_t n = (size_t)width*height;
-	CK(ctx->ppD.reserve(n*4+n*12)); CK(ctx->ppC.reserve(n*4));
-	float* dD = ctx->ppD.as<float>(); float* dN = normal ? dD+n : nullptr; float* dC = conf ? ctx->ppC.as<float>() : nullptr;
-	CK(cudaMemcpyAsync(dD, depth, n*4, cudaMemcpyHostToDevice, s));
-	if (normal) CK(cudaMemcpyAsync(dN, normal, n*12, cudaMemcpyHostToDevice, s));
-	if (conf) CK(cudaMemcpyAsync(dC, conf, n*4, cudaMemcpyHostToDevice, s));
-	CK(cudaEventRecord(ctx->ev0, s));
-	const int rc = which == 0 ? b200mvs_remove_small_segments_device(ctx, dD, dN, dC, width, height, th, arg, s)
-		: b200mvs_gap_interpolation_device(ctx, dD, dN, dC, width, height, th, arg, s);
-	if (rc) return rc;
-	CK(cudaEventRecord(ctx->ev1, s));
-	CK(cudaMemcpyAsync(depth, dD, n*4, cudaMemcpyDeviceToHost, s));
-	if (normal) CK(cudaMemcpyAsync(normal, dN, n*12, cudaMemcpyDeviceToHost, s));
-	if (conf) CK(cudaMemcpyAsync(conf, dC, n*4, cudaMemcpyDeviceToHost, s));
-	CK(cudaStreamSynchronize(s));
-	const uint64_t b = n*4+(normal ? n*12 : 0)+(conf ? n*4 : 0);
-	if (stats) return fill_stats(ctx, stats, t0, 1, b, b);
-	return B200MVS_OK;
+	float *dD, *dN = nullptr, *dC = nullptr;
+	call.inout(dD, depth, n*sizeof(float));
+	if (normal) call.inout(dN, normal, n*3*sizeof(float));
+	if (conf) call.inout(dC, conf, n*sizeof(float));
+	if (int rc = call.stage()) return rc;
+	return call.run([&](cudaStream_t s) { return form(ctx, dD, dN, dC, width, height, th, arg, s); }, stats);
 }
 
 int b200mvs_remove_small_segments(b200mvs_ctx* ctx, float* depth, float* normal, float* conf, int width, int height,
 	float fDepthDiffThreshold, unsigned nSpeckleSize, b200mvs_stats* stats)
 {
-	return pp_host(ctx, 0, depth, normal, conf, width, height, fDepthDiffThreshold, nSpeckleSize, stats);
+	return pp_host(ctx, b200mvs_remove_small_segments_device, depth, normal, conf, width, height, fDepthDiffThreshold, nSpeckleSize, stats);
 }
 
 int b200mvs_gap_interpolation(b200mvs_ctx* ctx, float* depth, float* normal, float* conf, int width, int height,
 	float fDepthDiffThreshold, unsigned nIpolGapSize, b200mvs_stats* stats)
 {
-	return pp_host(ctx, 1, depth, normal, conf, width, height, fDepthDiffThreshold, nIpolGapSize, stats);
+	return pp_host(ctx, b200mvs_gap_interpolation_device, depth, normal, conf, width, height, fDepthDiffThreshold, nIpolGapSize, stats);
 }
 
 // ---- image preparation (SURVEY §8f rank 3): toGray on the device ----

@@ -248,24 +248,19 @@ int b200mvs_sgm_match(b200mvs_ctx* ctx, const float* leftGray, const uint8_t* le
 	if (!leftGray || !leftBGR || !rightGray || !pixels || !disparity || !cost || width <= 6 || height <= 6)
 		return fail(ctx, B200MVS_ERR_ARG, "sgm: null pointer or image too small");
 	CK(cudaSetDevice(ctx->device));
-	cudaStream_t s = ctx->stream;
-	const auto t0 = std::chrono::steady_clock::now();
+	HostCall call(ctx);
 	const size_t n = (size_t)width*height, nv = (size_t)(width-6)*(height-6);
-	CK(ctx->sgL.reserve(n*4)); CK(ctx->sgR.reserve(n*4)); CK(ctx->sgC.reserve(n*3)); CK(ctx->sgPx.reserve(nv*sizeof(SGMPixel)));
-	CK(ctx->sgDisp.reserve(nv*2)); CK(ctx->sgCost.reserve(nv*2));
-	CK(cudaMemcpyAsync(ctx->sgL.p, leftGray, n*4, cudaMemcpyHostToDevice, s));
-	CK(cudaMemcpyAsync(ctx->sgR.p, rightGray, n*4, cudaMemcpyHostToDevice, s));
-	CK(cudaMemcpyAsync(ctx->sgC.p, leftBGR, n*3, cudaMemcpyHostToDevice, s));
-	CK(cudaMemcpyAsync(ctx->sgPx.p, pixels, nv*sizeof(SGMPixel), cudaMemcpyHostToDevice, s));
-	b200mvs_stats st; // the match records ev0 / ev1 around its kernels only when asked for statistics
-	int rc = b200mvs_sgm_match_device(ctx, ctx->sgL.as<float>(), ctx->sgC.as<uint8_t>(), ctx->sgR.as<float>(), width, height,
-		(const b200mvs_sgm_pixel*)ctx->sgPx.p, numCosts, prm, 7, nullptr, nullptr, ctx->sgDisp.as<int16_t>(), ctx->sgCost.as<uint16_t>(), s, &st);
-	if (rc) return rc;
-	CK(cudaMemcpyAsync(disparity, ctx->sgDisp.p, nv*2, cudaMemcpyDeviceToHost, s));
-	CK(cudaMemcpyAsync(cost, ctx->sgCost.p, nv*2, cudaMemcpyDeviceToHost, s));
-	CK(cudaStreamSynchronize(s));
-	if (stats) return fill_stats(ctx, stats, t0, 1, n*11+nv*sizeof(SGMPixel), nv*4);
-	return B200MVS_OK;
+	const float *dL, *dR; const uint8_t* dC; const b200mvs_sgm_pixel* dPx; int16_t* dDisp; uint16_t* dCost;
+	call.in(dL, leftGray, n*sizeof(float)); call.in(dR, rightGray, n*sizeof(float)); call.in(dC, leftBGR, n*3);
+	call.in(dPx, pixels, nv*sizeof(SGMPixel));
+	call.out(dDisp, disparity, nv*sizeof(int16_t)); call.out(dCost, cost, nv*sizeof(uint16_t));
+	if (int rc = call.stage()) return rc;
+	// with statistics the match records ev0 / ev1 around its kernels and checks the wave-front aggregation's error word
+	call.formRecordsEvents = true;
+	b200mvs_stats st;
+	return call.run([&](cudaStream_t s) {
+		return b200mvs_sgm_match_device(ctx, dL, dC, dR, width, height, dPx, numCosts, prm, 7, nullptr, nullptr, dDisp, dCost, s, &st);
+	}, stats);
 }
 
 int b200mvs_sgm_cross_check_device(b200mvs_ctx* ctx, int16_t* l2r, const int16_t* r2l, int width, int height, int thCross, void* stream) {
@@ -677,43 +672,21 @@ int b200mvs_sgm_fuse(b200mvs_ctx* ctx, const b200mvs_sgm_pair* pairs, int nPairs
 	if (!depth || minViews < 0 || (K && !normal))
 		return fail(ctx, B200MVS_ERR_ARG, "sgm fuse: null depth map, negative minViews, or K without a normal map");
 	CK(cudaSetDevice(ctx->device));
-	cudaStream_t s = ctx->stream;
-	const auto t0 = std::chrono::steady_clock::now();
-	// stage the maps: disparities (and costs) of every pair, 16-byte aligned slices
-	std::vector<b200mvs_sgm_pair> dev(pairs, pairs+nPairs);
-	std::vector<size_t> off(nPairs);
-	size_t total = 0;
-	for (int p = 0; p < nPairs; ++p) {
-		off[p] = total;
-		const size_t m = (size_t)pairs[p].width*pairs[p].height;
-		total += ((m*2+15) & ~(size_t)15)*(pairs[p].cost ? 2 : 1);
-	}
-	CK(ctx->sfIn.reserve(total));
-	uint64_t h2d = 0;
-	for (int p = 0; p < nPairs; ++p) {
-		const size_t m = (size_t)pairs[p].width*pairs[p].height;
-		uint8_t* base = ctx->sfIn.as<uint8_t>()+off[p];
-		CK(cudaMemcpyAsync(base, pairs[p].disparity, m*2, cudaMemcpyHostToDevice, s));
-		dev[p].disparity = (const int16_t*)base; h2d += m*2;
-		if (pairs[p].cost) {
-			uint8_t* cb = base+((m*2+15) & ~(size_t)15);
-			CK(cudaMemcpyAsync(cb, pairs[p].cost, m*2, cudaMemcpyHostToDevice, s));
-			dev[p].cost = (const uint16_t*)cb; h2d += m*2;
-		}
+	HostCall call(ctx);
+	std::vector<b200mvs_sgm_pair> dev(pairs, pairs+nPairs);   // the pairs with staged disparity (and cost) maps
+	for (b200mvs_sgm_pair& q: dev) {
+		const size_t bytes = (size_t)q.width*q.height*sizeof(int16_t);
+		call.in(q.disparity, q.disparity, bytes);
+		if (q.cost) call.in(q.cost, q.cost, bytes);
 	}
 	const size_t n = (size_t)width*height;
-	CK(ctx->sfOut.reserve(n*5*sizeof(float)));
-	float* dD = ctx->sfOut.as<float>(); float* dC = dD+n; float* dN = dC+n;
-	CK(cudaEventRecord(ctx->ev0, s));
-	if (int rc = b200mvs_sgm_fuse_device(ctx, dev.data(), nPairs, width, height, minViews, K, dD, conf ? dC : nullptr, K ? dN : nullptr, s))
-		return rc;
-	CK(cudaEventRecord(ctx->ev1, s));
-	CK(cudaMemcpyAsync(depth, dD, n*4, cudaMemcpyDeviceToHost, s));
-	if (conf) CK(cudaMemcpyAsync(conf, dC, n*4, cudaMemcpyDeviceToHost, s));
-	if (K) CK(cudaMemcpyAsync(normal, dN, n*12, cudaMemcpyDeviceToHost, s));
-	CK(cudaStreamSynchronize(s));
-	if (stats) return fill_stats(ctx, stats, t0, 1, h2d, n*4+(conf ? n*4 : 0)+(K ? n*12 : 0));
-	return B200MVS_OK;
+	float *dD, *dC = nullptr, *dN = nullptr;
+	call.out(dD, depth, n*sizeof(float));
+	if (conf) call.out(dC, conf, n*sizeof(float));
+	if (K) call.out(dN, normal, n*3*sizeof(float));
+	if (int rc = call.stage()) return rc;
+	return call.run([&](cudaStream_t s) { return b200mvs_sgm_fuse_device(ctx, dev.data(), nPairs, width, height, minViews, K, dD, dC, dN, s); },
+		stats);
 }
 
 int b200mvs_estimate_normal_map_device(b200mvs_ctx* ctx, const float* depth, int width, int height, const double* K, float* normal,

@@ -11,6 +11,7 @@
 //                                            SemiGlobalMatcher.h:127-142) at an integer factor
 // All integer work on a few MB; one thread per pixel (per row for ExtractMask).  Every result is bit-exact to the sequential code.
 #include "sgm_common.cuh"
+#include "label_common.cuh"
 #include <cub/device/device_scan.cuh>
 
 namespace {
@@ -157,59 +158,14 @@ __global__ void tsgm_extract_mask_kernel(const int16_t* __restrict__ D, uint8_t*
 }
 
 // cv::filterSpeckles(img, newVal, maxSpeckleSize, maxDiff) on int16: the regions are the connected components of the pixels
-// != newVal under the symmetric 4-neighbour relation |d1 - d2| <= maxDiff, so any labelling gives OpenCV's regions.  Union-find
-// on the device as in RemoveSmallSegments (filter_kernels.cu): link left (else up), pointer jumps, atomicMin unions of the upper
-// edges the links did not take, roots, sizes, removal of the regions of at most maxSpeckleSize pixels.
-__device__ __forceinline__ bool spk_edge(int a, int b, int newVal, int maxDiff) { return b != newVal && abs(a-b) <= maxDiff; }
-__device__ __forceinline__ int spk_find(int* L, int i) {
-	int p;
-	while ((p = ((volatile int*)L)[i]) != i) i = p;
-	return i;
-}
-__device__ void spk_union(int* L, int a, int b) {
-	bool done;
-	do {
-		a = spk_find(L, a); b = spk_find(L, b);
-		if (a < b) { const int old = atomicMin(L+b, a); done = (old == b); b = old; }
-		else if (b < a) { const int old = atomicMin(L+a, b); done = (old == a); a = old; }
-		else done = true;
-	} while (!done);
-}
-__global__ void tsgm_speckle_init_kernel(const int16_t* __restrict__ D, int* L, int* size, int W, int H, int newVal, int maxDiff) {
-	const int x = blockIdx.x*blockDim.x+threadIdx.x, y = blockIdx.y*blockDim.y+threadIdx.y;
-	if (x >= W || y >= H) return;
-	const int i = y*W+x;
-	const int a = D[i];
-	int l = -1;
-	if (a != newVal) {
-		l = i;
-		if (x > 0 && spk_edge(a, D[i-1], newVal, maxDiff)) l = i-1;
-		else if (y > 0 && spk_edge(a, D[i-W], newVal, maxDiff)) l = i-W;
-	}
-	L[i] = l;
-	size[i] = 0;
-}
-__global__ void tsgm_speckle_jump_kernel(int* L, int n) {
-	const int i = blockIdx.x*blockDim.x+threadIdx.x;
-	if (i >= n) return;
-	const int p = L[i];
-	if (p >= 0 && p != i) L[i] = ((volatile int*)L)[p];
-}
-__global__ void tsgm_speckle_merge_kernel(const int16_t* __restrict__ D, int* L, int W, int H, int newVal, int maxDiff) {
-	const int x = blockIdx.x*blockDim.x+threadIdx.x, y = blockIdx.y*blockDim.y+threadIdx.y;
-	if (x < 1 || x >= W || y < 1 || y >= H) return;
-	const int i = y*W+x;
-	const int a = D[i];
-	if (a == newVal) return;
-	if (spk_edge(a, D[i-1], newVal, maxDiff) && spk_edge(a, D[i-W], newVal, maxDiff)) spk_union(L, i, i-W);
-}
-__global__ void tsgm_speckle_count_kernel(int* L, int* size, int n) {
-	const int i = blockIdx.x*blockDim.x+threadIdx.x;
-	int r = -1;
-	if (i < n && L[i] >= 0) { r = spk_find(L, i); L[i] = r; }
-	const unsigned peers = __match_any_sync(0xFFFFFFFFu, r);
-	if (r >= 0 && (threadIdx.x&31) == __ffs(peers)-1) atomicAdd(size+r, __popc(peers));
-}
+// != newVal under the symmetric 4-neighbour relation |d1 - d2| <= maxDiff, so any labelling gives OpenCV's regions: the
+// components of label_common.cuh, then the removal of the regions of at most maxSpeckleSize pixels.
+struct SpeckleEdge {
+	const int16_t* D; int newVal, maxDiff;
+	__device__ int at(int i) const { return __ldg(D+i); }
+	__device__ bool valid(int a) const { return a != newVal; }
+	__device__ bool edge(int a, int b) const { return b != newVal && abs(a-b) <= maxDiff; }
+};
 __global__ void tsgm_speckle_remove_kernel(int16_t* __restrict__ D, const int* __restrict__ L, const int* __restrict__ size, int n,
 	int newVal, int maxSpeckleSize)
 {
@@ -314,14 +270,7 @@ cudaError_t tsgm_launch_extract_mask(const int16_t* D, uint8_t* M, int W, int H,
 // labels / sizes: W x H int scratch each
 cudaError_t tsgm_launch_speckles(int16_t* D, int W, int H, int newVal, int maxSpeckleSize, int maxDiff, int* labels, int* sizes, cudaStream_t s) {
 	const int n = W*H;
-	const dim3 b(32, 8), g = grid2(W, H, b);
-	tsgm_speckle_init_kernel<<<g, b, 0, s>>>(D, labels, sizes, W, H, newVal, maxDiff);
-	int rounds = 1;
-	while ((1<<rounds) < W+H) ++rounds;
-	for (int r = 0; r < rounds; ++r) tsgm_speckle_jump_kernel<<<(n+255)/256, 256, 0, s>>>(labels, n);
-	tsgm_speckle_merge_kernel<<<g, b, 0, s>>>(D, labels, W, H, newVal, maxDiff);
-	for (int r = 0; r < rounds; ++r) tsgm_speckle_jump_kernel<<<(n+255)/256, 256, 0, s>>>(labels, n);
-	tsgm_speckle_count_kernel<<<(n+255)/256, 256, 0, s>>>(labels, sizes, n);
+	label_launch(SpeckleEdge{D, newVal, maxDiff}, W, H, labels, sizes, nullptr, s);
 	tsgm_speckle_remove_kernel<<<(n+255)/256, 256, 0, s>>>(D, labels, sizes, n, newVal, maxSpeckleSize);
 	return cudaGetLastError();
 }
