@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import ctypes as C
 import dataclasses
+import math
 from typing import List, Optional
 
 import numpy as np
@@ -141,11 +142,68 @@ def _is_torch(a) -> bool:
 	return type(a).__module__.startswith("torch")
 
 
-def _layout(a):
-	"""(address, shape, strides in bytes, dtype name) of a numpy array or a torch tensor"""
-	if _is_torch(a):
-		return a.data_ptr(), tuple(a.shape), tuple(s*a.element_size() for s in a.stride()), str(a.dtype)[len("torch."):]
-	return a.ctypes.data, a.shape, a.strides, str(a.dtype)
+def _cuda_index(a) -> int:
+	"""the CUDA device of a tensor, which the module-level device calls run on (0 for anything else: the checks then refuse it)"""
+	return a.device.index if _is_torch(a) and a.is_cuda else 0
+
+
+def _pitch(a) -> int:
+	"""row pitch in bytes of a numpy array or a torch tensor"""
+	return a.stride(0)*a.element_size() if _is_torch(a) else a.strides[0]
+
+
+def _host(a, dtype, device=None):
+	"""a map in the form the host calls take it: a C-contiguous numpy array of dtype, copied only if it has to be.  A map for a
+	device call (device given), a CUDA tensor and None are returned as they are, for _arg to judge."""
+	return a if device is not None or a is None or (_is_torch(a) and a.is_cuda) else np.ascontiguousarray(a, dtype)
+
+
+# a 16-bit volume or cost map: the library reads uint16, which torch callers often hold as int16
+_U16 = ("int16", "uint16")
+
+
+def _arg(where: str, name: str, a, dtype, shape=None, device=None, rows: bool = False, min_size: int = 0):
+	"""Check one buffer argument of a library call -> its address (None for None, the C-ABI's "not given").  A raw pointer carries
+	no size, type or device, so this is the only place that can refuse a buffer the call would overrun, misread or fault on.
+	dtype: a dtype name or a tuple of names; an int: the byte size of the records of a pixel map, whose `shape` then counts records.
+	shape: the exact shape with None for any size and a tuple for a choice of sizes; None: any shape.
+	device: None for a numpy array (host call), else the index of the CUDA device the tensor must be on.
+	rows: every row contiguous, rows may be strided; else C-contiguous.  min_size: the least number of elements (volumes).
+	Raises ValueError naming the method, the argument, what was expected and what was given.  Reads attributes only: no
+	synchronisation, no copy."""
+	if a is None:
+		return None
+	tensor = _is_torch(a)
+	if tensor:
+		kind, item, resident = str(a.dtype)[len("torch."):], a.element_size(), a.is_cuda and a.device.index == device
+		steps = [s*item for s in a.stride()]
+	elif isinstance(a, np.ndarray):
+		kind, item, steps, resident = a.dtype.name, a.itemsize, a.strides, device is None
+	else:
+		kind, item, steps, resident = type(a).__name__, 0, (), False
+	dims = tuple(getattr(a, "shape", ()))
+	size = math.prod(dims)
+	if isinstance(dtype, int):
+		typed, counted = size*item % dtype == 0, (size*item//dtype,)
+	else:
+		typed, counted = kind in ((dtype,) if isinstance(dtype, str) else dtype), dims
+	packed = all(n == 1 or s == item*math.prod(dims[k+1:]) for k, (n, s) in enumerate(zip(dims, steps)) if k or not rows)
+	fits = shape is None or (len(counted) == len(shape) and all(
+		s is None or (n in s if isinstance(s, tuple) else n == s) for n, s in zip(counted, shape)))
+	if resident and typed and packed and fits and size >= min_size:
+		return a.data_ptr() if tensor else a.ctypes.data
+	layout = "row-contiguous" if rows else "contiguous"
+	sizes = lambda s: "(%s)" % ", ".join("*" if n is None else "|".join(map(str, n)) if isinstance(n, tuple) else str(n) for n in s)
+	want = "a %s %s" % (layout, "numpy array" if device is None else "CUDA tensor on cuda:%d" % device)
+	if isinstance(dtype, int):
+		want += " of %s records of %d bytes" % (shape[0], dtype)
+	else:
+		want += " of %s" % "|".join((dtype,) if isinstance(dtype, str) else dtype)
+		want += "" if shape is None else " of shape %s" % sizes(shape)
+	want += " of at least %d elements" % min_size if min_size else ""
+	home = "tensor on %s" % a.device if tensor else "numpy array" if isinstance(a, np.ndarray) else "object"
+	raise ValueError("%s: %s must be %s; got a %s %s of shape %s%s" % (where, name, want, kind, home, sizes(dims),
+		"" if packed else ", not " + layout))
 
 
 def _put_camera(o, cam: Camera, suffix: str = ""):
@@ -153,40 +211,29 @@ def _put_camera(o, cam: Camera, suffix: str = ""):
 		getattr(o, name+suffix)[:] = np.asarray(getattr(cam, name), np.float64).ravel()
 
 
-def _make_views(images: List[ViewData]):
-	"""-> (ctypes View array, keepalive list, on_device flag)"""
+def _make_views(images: List[ViewData], device: Optional[int] = None, where: str = "EstimateDepthMap"):
+	"""-> (ctypes View array, keepalive list, on_device flag).  Tensor views must be CUDA tensors on `device` (None: numpy views only)."""
 	arr = (_lib.View*len(images))()
 	keep = []
 	dev = _is_torch(images[0].image)
-	device = images[0].image.device if dev else None
+	home = device if dev else None
 	for i, v in enumerate(images):
 		o = arr[i]
-		if dev != _is_torch(v.image):
-			raise ValueError("mixing host and device images in one DepthData")
-		img = v.image if dev else np.asarray(v.image)
-		if dev and (not img.is_cuda or img.device != device):
-			raise ValueError("all views of a DepthData must live on the same CUDA device")
-		ptr, shape, strides, dtype = _layout(img)
+		img = v.image if _is_torch(v.image) else np.asarray(v.image)
 		keep.append(img)
-		if dtype == "uint8":
-			# 8-bit colour image: toGray runs on the device inside the call
-			if len(shape) != 3 or shape[2] not in (3, 4) or strides[2] != 1 or strides[1] != shape[2]:
-				raise ValueError("colour image must be a (H, W, 3|4) uint8 array or CUDA tensor with packed pixels (Image8U3)")
-			o.image8 = ptr; o.height, o.width, o.channels8 = shape; o.stride8_bytes = strides[0]; o.bgr8 = int(bool(v.bgr))
+		if str(img.dtype).endswith("uint8"):
+			# 8-bit colour image with packed pixels (Image8U3): toGray runs on the device inside the call
+			o.image8 = _arg(where, "images[%d].image" % i, img, "uint8", (None, None, (3, 4)), home, rows=True)
+			o.height, o.width, o.channels8 = img.shape; o.stride8_bytes = _pitch(img); o.bgr8 = int(bool(v.bgr))
 		else:
-			if dtype != "float32" or len(shape) != 2 or strides[1] != 4:
-				raise ValueError("image must be a 2-D float32 array or CUDA tensor with contiguous rows (Image32F)")
-			o.image = ptr; o.height, o.width = shape; o.stride_bytes = strides[0]
+			o.image = _arg(where, "images[%d].image" % i, img, "float32", (None, None), home, rows=True)
+			o.height, o.width = img.shape; o.stride_bytes = _pitch(img)
 		_put_camera(o, v.camera)
 		if v.depthMap is not None and i > 0:
-			dm = v.depthMap if dev else np.ascontiguousarray(v.depthMap, np.float32)
-			if dev and not (_is_torch(dm) and dm.is_cuda and dm.device == device):
-				raise ValueError("device depth-map must be a CUDA tensor on the images' device")
-			ptr, shape, strides, dtype = _layout(dm)
-			if dtype != "float32" or len(shape) != 2 or strides[1] != 4:
-				raise ValueError("depth-map must be a 2-D float32 array or CUDA tensor with unit column stride")
+			dm = _host(v.depthMap, np.float32, home)
+			o.depth = _arg(where, "images[%d].depthMap" % i, dm, "float32", (None, None), home, rows=True)
 			keep.append(dm)
-			o.depth = ptr; o.dheight, o.dwidth = shape; o.dstride_bytes = strides[0]
+			o.dheight, o.dwidth = dm.shape; o.dstride_bytes = _pitch(dm)
 			_put_camera(o, v.cameraDepthMap or v.camera, "d")
 	return arr, keep, dev
 
@@ -195,41 +242,35 @@ def _make_views(images: List[ViewData]):
 _MAPS = (("depthMap", (), "float32"), ("normalMap", (3,), "float32"), ("confMap", (), "float32"), ("viewsMap", (4,), "uint8"))
 
 
-def _host_maps(dd: DepthData):
-	"""Allocate the missing output maps of dd as zeroed numpy arrays and check the given ones -> their addresses."""
+def _out_maps(dd: DepthData, device: Optional[int] = None, where: str = "EstimateDepthMap"):
+	"""Check the given output maps of dd (converted numpy arrays for a host call, CUDA tensors on `device` for a device call), then
+	allocate the missing ones zeroed -> the four addresses."""
 	h, w = dd.images[0].image.shape[:2]
-	for name, ch, dtype in _MAPS:
-		a = getattr(dd, name)
-		if a is None:
-			a = np.zeros((h, w)+ch, dtype)
-		else:
-			a = np.ascontiguousarray(a, dtype)
-			if a.shape != (h, w)+ch:
-				raise ValueError("map has the wrong shape")
+	maps = [(name, (h, w)+ch, dt, _host(getattr(dd, name), dt, device)) for name, ch, dt in _MAPS]
+	for name, shape, dt, a in maps:
+		_arg(where, name, a, dt, shape, device)
+	ptrs = []
+	for name, shape, dt, a in maps:
+		if a is None and device is None:
+			a = np.zeros(shape, dt)
+		elif a is None:
+			import torch
+			a = torch.zeros(shape, dtype=getattr(torch, dt), device=device)
 		setattr(dd, name, a)
-	return [getattr(dd, name).ctypes.data for name, _, _ in _MAPS]
+		ptrs.append(_arg(where, name, a, dt, shape, device))
+	return ptrs
 
 
-def _device_maps(dd: DepthData):
-	"""Allocate the missing output maps of dd as zeroed CUDA tensors on the images' device and check the given ones -> their
-	addresses."""
-	import torch
-	t0 = dd.images[0].image
-	h, w = t0.shape[:2]
-	for name, ch, dt in _MAPS:
-		a, shape, dtype = getattr(dd, name), (h, w)+ch, getattr(torch, dt)
-		if a is None:
-			a = torch.zeros(shape, dtype=dtype, device=t0.device)
-		elif not _is_torch(a) or tuple(a.shape) != shape or not a.is_contiguous() or a.dtype != dtype or a.device != t0.device:
-			raise ValueError("map must be a contiguous %s CUDA tensor of shape %s on the images' device" % (dtype, shape))
-		setattr(dd, name, a)
-	return [getattr(dd, name).data_ptr() for name, _, _ in _MAPS]
+def _host_maps(dd: DepthData, where: str = "EstimateDepthMap"):
+	"""_out_maps of a host call: numpy output maps -> their addresses"""
+	return _out_maps(dd, None, where)
 
 
 class _Context:
-	"""One engine context (b200mvs_create ... b200mvs_destroy) and the calls made on it."""
+	"""One engine context (b200mvs_create ... b200mvs_destroy) on CUDA device `device`, and the calls made on it."""
 
 	def __init__(self, device: int):
+		self.device = int(device)
 		self._lib = _lib.load()
 		self._ctx = C.c_void_p()
 		rc = self._lib.b200mvs_create(int(device), C.byref(self._ctx))
@@ -271,7 +312,6 @@ class PatchMatchB200(_Context):
 
 	def __init__(self, device: int = 0):
 		super().__init__(device)
-		self.device = int(device)
 		self.bGeomConsistency = False
 
 	def Init(self, bGeomConsistency: bool = False):
@@ -282,11 +322,10 @@ class PatchMatchB200(_Context):
 		"""TImage::toGray(out, COLOR_BGR2GRAY, bNormalize=true) (libs/Common/Types.inl:2377-2431) on the device: uint8 CUDA tensor
 		(H, W, 3|4), channel order B,G,R(,A) as cv::imread delivers (bgr=False: R,G,B) -> float32 gray (H, W) in [0, 1]."""
 		import torch
-		if not (_is_torch(image) and image.is_cuda and image.dtype == torch.uint8 and image.dim() == 3 and image.shape[2] in (3, 4) and image.is_contiguous()):
-			raise ValueError("ToGray needs a contiguous uint8 CUDA tensor of shape (H, W, 3|4)")
+		ptr = _arg("ToGray", "image", image, "uint8", (None, None, (3, 4)), self.device)
 		h, w, ch = (int(v) for v in image.shape)
 		out = torch.empty((h, w), dtype=torch.float32, device=image.device)
-		self._call("to_gray_device", image.data_ptr(), w, h, w*ch, ch, int(bool(bgr)), out.data_ptr(), w*4, _stream_handle(image.device))
+		self._call("to_gray_device", ptr, w, h, w*ch, ch, int(bool(bgr)), out.data_ptr(), w*4, _stream_handle(self.device))
 		return out
 
 	def ScaleImage(self, image, scale: float):
@@ -294,14 +333,12 @@ class PatchMatchB200(_Context):
 		cv::resize(image, Size(), scale, scale, scale > 1 ? INTER_CUBIC : INTER_AREA), or None when |scale - 1| < 0.15
 		(the reference keeps the image then)."""
 		import torch
-		if not (_is_torch(image) and image.is_cuda and image.dtype == torch.float32 and image.dim() == 2 and image.stride(1) == 1):
-			raise ValueError("ScaleImage needs a 2-D float32 CUDA tensor with unit column stride")
+		ptr = _arg("ScaleImage", "image", image, "float32", (None, None), self.device, rows=True)
 		h, w = (int(v) for v in image.shape)
 		dw, dh, ok = C.c_int(), C.c_int(), C.c_int()
 		self._lib.b200mvs_scaled_size(w, h, scale, C.byref(dw), C.byref(dh))
 		out = torch.empty((max(dh.value, 1), max(dw.value, 1)), dtype=torch.float32, device=image.device)
-		self._call("scale_image_device", image.data_ptr(), w, h, image.stride(0)*4, scale, out.data_ptr(), C.byref(ok),
-			_stream_handle(image.device))
+		self._call("scale_image_device", ptr, w, h, _pitch(image), scale, out.data_ptr(), C.byref(ok), _stream_handle(self.device))
 		return out if ok.value else None
 
 	def _set_params(self):
@@ -314,17 +351,13 @@ class PatchMatchB200(_Context):
 		self._mask_keep = None
 		if mask is None:
 			self._call("set_ignore_mask", None, 0, 0, 0, 0)
-		elif _is_torch(mask):
-			import torch
-			if mask.dtype != torch.uint8 or not mask.is_cuda or mask.dim() != 2 or mask.stride(1) != 1:
-				raise ValueError("device mask must be a 2-D uint8 CUDA tensor with unit column stride")
-			self._mask_keep = mask
-			self._call("set_ignore_mask", mask.data_ptr(), int(mask.shape[1]), int(mask.shape[0]), int(mask.stride(0)), 1)
-		else:
-			m = np.ascontiguousarray(mask, np.uint8)
-			if m.ndim != 2:
-				raise ValueError("mask must be 2-D")
-			self._call("set_ignore_mask", m.ctypes.data, m.shape[1], m.shape[0], m.strides[0], 0)
+			return
+		home = self.device if _is_torch(mask) else None
+		m = _host(mask, np.uint8, home)
+		ptr = _arg("SetIgnoreMask", "mask", m, "uint8", (None, None), home, rows=True)
+		if home is not None:
+			self._mask_keep = m
+		self._call("set_ignore_mask", ptr, int(m.shape[1]), int(m.shape[0]), _pitch(m), int(home is not None))
 
 	def EstimateDepthMap(self, depthData: DepthData, nGeometricIter: Optional[int] = None, stream=None, sync: bool = True):
 		"""PatchMatchCUDA::EstimateDepthMap(DepthData&): estimate depthMap/normalMap/confMap/viewsMap
@@ -333,19 +366,19 @@ class PatchMatchB200(_Context):
 			raise ValueError("DepthData needs the reference view and at least one neighbour")
 		if nGeometricIter is None:
 			nGeometricIter = 0 if self.bGeomConsistency else -1
+		arr, keep, dev = _make_views(depthData.images, self.device)
+		maps = _out_maps(depthData, self.device if dev else None)
 		self._set_params()
-		arr, keep, dev = _make_views(depthData.images)
 		job = (arr, len(arr), depthData.dMin, depthData.dMax, int(nGeometricIter))
 		if dev:
-			maps = _device_maps(depthData)
 			if stream is None:
-				stream = _stream_handle(depthData.images[0].image.device)
+				stream = _stream_handle(self.device)
 			self._call("estimate_device", *job, *maps, stream, C.byref(self.stats) if sync else None)
 		elif sync:
-			self._call("estimate", *job, *_host_maps(depthData), C.byref(self.stats))
+			self._call("estimate", *job, *maps, C.byref(self.stats))
 		else:
 			# asynchronous host path: the caller keeps depthData alive and calls Wait() before reading the maps
-			self._call("estimate_async", *job, *_host_maps(depthData))
+			self._call("estimate_async", *job, *maps)
 			self._inflight = (depthData, keep)
 		return depthData
 
@@ -355,45 +388,44 @@ class PatchMatchB200(_Context):
 		self._inflight = None
 
 	# ---- building blocks on device tensors (used by the parity tests) -----------------------
-	def _dev_views(self, images):
-		arr, keep, dev = _make_views(images)
+	def _state(self, where, images, plane4, cost, lowres):
+		"""the device views and the float32 state of their reference image (H, W) -> (views, keepalive, [lowres, plane4, cost addresses])"""
+		arr, keep, dev = _make_views(images, self.device, where)
 		if not dev:
-			raise ValueError("building blocks need device-resident views")
-		return arr, keep
+			raise ValueError("%s: building blocks need device-resident views" % where)
+		h, w = images[0].image.shape[:2]
+		return arr, keep, [_arg(where, name, a, "float32", shape, self.device)
+			for name, a, shape in (("lowres", lowres, (h, w)), ("plane4", plane4, (h, w, 4)), ("cost", cost, (h, w)))]
 
 	def ScoreDepthMap(self, images, dMin, dMax, plane4, cost, lowres=None):
 		"""pass A (ScoreDepthMapTmp) on a packed plane field (H, W, 4) = {nx,ny,nz,depth}."""
+		arr, keep, (lr, p4, c) = self._state("ScoreDepthMap", images, plane4, cost, lowres)
 		self._set_params()
-		arr, keep = self._dev_views(images)
-		self._call("pm_score", arr, len(arr), dMin, dMax, lowres.data_ptr() if lowres is not None else None, plane4.data_ptr(),
-			cost.data_ptr(), _stream_handle(plane4.device))
+		self._call("pm_score", arr, len(arr), dMin, dMax, lr, p4, c, _stream_handle(self.device))
 
 	def SweepDepthMap(self, images, dMin, dMax, plane4, cost, sweep, half=-1, nRandomIters=None, lowres=None):
 		"""pass B: one red-black sweep (both colours, or one if half in {0,1})."""
+		arr, keep, (lr, p4, c) = self._state("SweepDepthMap", images, plane4, cost, lowres)
 		self._set_params()
-		arr, keep = self._dev_views(images)
 		if nRandomIters is None:
 			nRandomIters = OPTDENSE.schedule()[1]
-		self._call("pm_sweep", arr, len(arr), dMin, dMax, lowres.data_ptr() if lowres is not None else None, int(sweep), int(half),
-			int(nRandomIters), plane4.data_ptr(), cost.data_ptr(), _stream_handle(plane4.device))
+		self._call("pm_sweep", arr, len(arr), dMin, dMax, lr, int(sweep), int(half), int(nRandomIters), p4, c, _stream_handle(self.device))
 
 
 def EstimateDepthMapsBatch(arrDepthData: List[DepthData], engines: List["PatchMatchB200"], nGeometricIter: int = -1):
 	"""b200mvs_estimate_batch: estimate every DepthData (host buffers) with the given engines — one per GPU of
 	the box, or two on one GPU — dealt round-robin inside this process."""
 	lib = engines[0]._lib
-	for e in engines:
-		e._set_params()
 	jobs = (_lib.Job*len(arrDepthData))()
 	keep = []
 	for j, dd in enumerate(arrDepthData):
-		arr, k, dev = _make_views(dd.images)
-		if dev:
-			raise ValueError("the batch call takes host buffers")
+		arr, k, _ = _make_views(dd.images, None, "EstimateDepthMapsBatch")   # host buffers only
 		keep.append((arr, k))
 		J = jobs[j]
 		J.views = arr; J.nViews = len(arr); J.dMin = dd.dMin; J.dMax = dd.dMax; J.nGeometricIter = int(nGeometricIter)
-		J.depth, J.normal, J.conf, J.viewsMap = _host_maps(dd)
+		J.depth, J.normal, J.conf, J.viewsMap = _host_maps(dd, "EstimateDepthMapsBatch")
+	for e in engines:
+		e._set_params()
 	ctxs = (C.c_void_p*len(engines))(*[e._ctx for e in engines])
 	rc = lib.b200mvs_estimate_batch(ctxs, len(engines), jobs, len(arrDepthData))
 	if rc != 0:
@@ -419,24 +451,17 @@ class DepthMapsData:
 		return True
 
 	@staticmethod
-	def _ptr(a):
-		return a.data_ptr() if _is_torch(a) else a.ctypes.data
-
-	@staticmethod
-	def _dmap(o: "_lib.DMap", depthData: DepthData, need_conf: bool, keep: list):
-		cam = depthData.images[0].camera
-		d, c = depthData.depthMap, depthData.confMap
-		if not _is_torch(d):
-			d = np.ascontiguousarray(d, np.float32)
-			c = None if c is None else np.ascontiguousarray(c, np.float32)
-		elif not d.is_contiguous() or (c is not None and not c.is_contiguous()):
-			raise ValueError("depth/confidence maps must be contiguous")
+	def _dmap(o: "_lib.DMap", depthData: DepthData, need_conf: bool, keep: list, device: Optional[int], label: str):
+		"""fill o with the depth and confidence maps of depthData: host maps (device None) are converted to float32, device maps
+		must be CUDA tensors on `device` -> the depth map"""
+		d, c = _host(depthData.depthMap, np.float32, device), _host(depthData.confMap, np.float32, device)
 		if need_conf and c is None:
 			raise ValueError("FilterDepthMap needs the confidence map of every view")
+		o.depth = _arg("FilterDepthMap", label+".depthMap", d, "float32", (None, None), device)
+		o.conf = _arg("FilterDepthMap", label+".confMap", c, "float32", tuple(d.shape), device)
 		keep += [d, c]
-		o.depth = DepthMapsData._ptr(d); o.conf = DepthMapsData._ptr(c) if c is not None else None
 		o.height, o.width = int(d.shape[0]), int(d.shape[1])
-		_put_camera(o, cam)
+		_put_camera(o, depthData.images[0].camera)
 		return d
 
 	def FilterDepthMap(self, depthDataRef: DepthData, neighbors: List[DepthData], bAdjust: Optional[bool] = None, projected: bool = False):
@@ -449,12 +474,13 @@ class DepthMapsData:
 			min(OPTDENSE.nMinViewsFilterAdjust, self.nCalibratedImages-1), OPTDENSE.fDepthDiffThreshold, int(bAdjust))
 		arr = (_lib.DMap*(len(neighbors)+1))()
 		keep: list = []
-		dref = self._dmap(arr[0], depthDataRef, True, keep)
+		device = self.pmCUDA.device if _is_torch(depthDataRef.depthMap) else None
+		dref = self._dmap(arr[0], depthDataRef, True, keep, device, "depthDataRef")
 		for i, nb in enumerate(neighbors):
-			self._dmap(arr[i+1], nb, bAdjust, keep)
+			self._dmap(arr[i+1], nb, bAdjust, keep, device, "neighbors[%d]" % i)
 		nbrs = C.cast(C.byref(arr, C.sizeof(_lib.DMap)), C.POINTER(_lib.DMap))
 		ok = C.c_int(0)
-		if _is_torch(dref):
+		if device is not None:
 			import torch
 			od = torch.empty_like(dref); oc = torch.empty_like(dref)
 			pd = pc = None
@@ -463,7 +489,7 @@ class DepthMapsData:
 				pc = torch.zeros_like(pd)
 			self.pmCUDA._call("filter_depth_map_device", C.byref(arr[0]), nbrs, len(neighbors), C.byref(prm), depthDataRef.dMin,
 				depthDataRef.dMax, od.data_ptr(), oc.data_ptr(), pd.data_ptr() if projected else None,
-				pc.data_ptr() if projected and bAdjust else None, C.byref(ok), _stream_handle(dref.device))
+				pc.data_ptr() if projected and bAdjust else None, C.byref(ok), _stream_handle(device))
 			if not ok.value:
 				return None
 			return (od, oc, pd, pc) if projected else (od, oc)
@@ -472,30 +498,27 @@ class DepthMapsData:
 			od.ctypes.data, oc.ctypes.data, C.byref(ok), C.byref(self.stats))
 		return (od, oc) if ok.value else None
 
-	def _post(self, name: str, depthData: DepthData, arg: int) -> bool:
-		d, n, c = depthData.depthMap, depthData.normalMap, depthData.confMap
+	def _post(self, where: str, name: str, depthData: DepthData, arg: int) -> bool:
+		"""one in-place pass over the float32 maps of depthData: numpy arrays (host form) or CUDA tensors on pmCUDA's device"""
+		d = depthData.depthMap
+		device = self.pmCUDA.device if _is_torch(d) else None
+		pd = _arg(where, "depthMap", d, "float32", (None, None), device)
 		h, w = int(d.shape[0]), int(d.shape[1])
-		if _is_torch(d):
-			for a in (d, n, c):
-				if a is not None and not a.is_contiguous():
-					raise ValueError("maps must be contiguous")
-			self.pmCUDA._call(name+"_device", d.data_ptr(), n.data_ptr() if n is not None else None, c.data_ptr() if c is not None else None,
-				w, h, OPTDENSE.fDepthDiffThreshold, int(arg), _stream_handle(d.device))
+		pn = _arg(where, "normalMap", depthData.normalMap, "float32", (h, w, 3), device)
+		pc = _arg(where, "confMap", depthData.confMap, "float32", (h, w), device)
+		if device is not None:
+			self.pmCUDA._call(name+"_device", pd, pn, pc, w, h, OPTDENSE.fDepthDiffThreshold, int(arg), _stream_handle(device))
 		else:
-			for a in (d, n, c):
-				if a is not None and not (a.flags.c_contiguous and a.dtype == np.float32):
-					raise ValueError("maps must be contiguous float32 arrays (processed in place)")
-			self.pmCUDA._call(name, d.ctypes.data, n.ctypes.data if n is not None else None, c.ctypes.data if c is not None else None,
-				w, h, OPTDENSE.fDepthDiffThreshold, int(arg), C.byref(self.stats))
+			self.pmCUDA._call(name, pd, pn, pc, w, h, OPTDENSE.fDepthDiffThreshold, int(arg), C.byref(self.stats))
 		return True
 
 	def RemoveSmallSegments(self, depthData: DepthData) -> bool:
 		"""DepthMapsData::RemoveSmallSegments (SceneDensify.cpp:810-900), depthData's maps in place."""
-		return self._post("remove_small_segments", depthData, OPTDENSE.nSpeckleSize)
+		return self._post("RemoveSmallSegments", "remove_small_segments", depthData, OPTDENSE.nSpeckleSize)
 
 	def GapInterpolation(self, depthData: DepthData) -> bool:
 		"""DepthMapsData::GapInterpolation (SceneDensify.cpp:904-1045), depthData's maps in place."""
-		return self._post("gap_interpolation", depthData, OPTDENSE.nIpolGapSize)
+		return self._post("GapInterpolation", "gap_interpolation", depthData, OPTDENSE.nIpolGapSize)
 
 
 class SemiGlobalMatcher(_Context):
@@ -517,44 +540,51 @@ class SemiGlobalMatcher(_Context):
 	def Match(self, leftGray, leftColor, rightGray, imagePixels, numCosts: int):
 		"""Host path: numpy images (gray float32 HxW, colour uint8 HxWx3 BGR) and the PixelMap
 		(structured array from synth.sgm_pixel_map or any {u8 idx, i2 dmin, i2 dmax, i4} records)."""
-		lg = np.ascontiguousarray(leftGray, np.float32); rg = np.ascontiguousarray(rightGray, np.float32)
-		lc = np.ascontiguousarray(leftColor, np.uint8)
-		h, w = lg.shape
-		if rg.shape != (h, w) or lc.shape != (h, w, 3):
-			raise ValueError("left/right/colour images must share one size")
-		px = np.ascontiguousarray(imagePixels)
-		if px.itemsize != 16 or px.size != (w-6)*(h-6):
-			raise ValueError("PixelMap must hold (w-6)*(h-6) 16-byte records")
+		lg, lc, rg, px = _host(leftGray, np.float32), _host(leftColor, np.uint8), _host(rightGray, np.float32), _host(imagePixels, None)
+		(h, w), (plg, plc, prg, _) = self._images("Match", lg, lc, rg, None, None)
+		ppx = _arg("Match", "imagePixels", px, 16, ((w-6)*(h-6),))
 		disp = np.zeros((h-6, w-6), np.int16); cost = np.zeros((h-6, w-6), np.uint16)
-		self._call("sgm_match", lg.ctypes.data, lc.ctypes.data, rg.ctypes.data, w, h, px.ctypes.data, numCosts, C.byref(self.prm),
-			disp.ctypes.data, cost.ctypes.data, C.byref(self.stats))
+		self._call("sgm_match", plg, plc, prg, w, h, ppx, numCosts, C.byref(self.prm), disp.ctypes.data, cost.ctypes.data, C.byref(self.stats))
 		return disp, cost
+
+	def _images(self, where, leftGray, leftColor, rightGray, rightColor, device):
+		"""check the rectified images of a match: gray float32 (h, w), colour uint8 (h, w, 3) -> ((h, w), their addresses)"""
+		plg = _arg(where, "leftGray", leftGray, "float32", (None, None), device)
+		h, w = (int(n) for n in leftGray.shape)
+		return (h, w), [plg] + [_arg(where, name, a, dt, shape, device) for name, a, dt, shape in (("leftColor", leftColor, "uint8", (h, w, 3)),
+			("rightGray", rightGray, "float32", (h, w)), ("rightColor", rightColor, "uint8", (h, w, 3)))]
 
 	def MatchDevice(self, leftGray, leftColor, rightGray, imagePixels, numCosts: int, stages: int = 7, costs=None, accums=None, sync: bool = True):
 		"""Device-resident path on torch CUDA tensors; costs (uint8) / accums (uint16 viewed as int16)
 		are optional in/out volumes of numCosts entries.  Returns (disparity, cost) int16 tensors
 		(cost holds the uint16 bit pattern)."""
 		import torch
-		h, w = leftGray.shape
+		(h, w), (plg, plc, prg, _) = self._images("MatchDevice", leftGray, leftColor, rightGray, None, self.device)
+		ppx = _arg("MatchDevice", "imagePixels", imagePixels, 16, ((w-6)*(h-6),), self.device)
+		pcv = _arg("MatchDevice", "costs", costs, "uint8", None, self.device, min_size=numCosts)
+		pac = _arg("MatchDevice", "accums", accums, _U16, None, self.device, min_size=numCosts)
 		dev = leftGray.device
 		disp = torch.zeros((h-6, w-6), dtype=torch.int16, device=dev)
 		cost = torch.zeros((h-6, w-6), dtype=torch.int16, device=dev)
-		self._call("sgm_match_device", leftGray.data_ptr(), leftColor.data_ptr(), rightGray.data_ptr(), w, h, imagePixels.data_ptr(),
-			numCosts, C.byref(self.prm), int(stages), costs.data_ptr() if costs is not None else None,
-			accums.data_ptr() if accums is not None else None, disp.data_ptr(), cost.data_ptr(), _stream_handle(dev),
-			C.byref(self.stats) if sync else None)
+		self._call("sgm_match_device", plg, plc, prg, w, h, ppx, numCosts, C.byref(self.prm), int(stages), pcv, pac, disp.data_ptr(),
+			cost.data_ptr(), _stream_handle(self.device), C.byref(self.stats) if sync else None)
 		return disp, cost
 
 	def ConsistencyCrossCheck(self, l2r, r2l, thCross: int = 1):
 		"""SemiGlobalMatcher::ConsistencyCrossCheck on int16 CUDA tensors; l2r is modified in place."""
+		pl = _arg("ConsistencyCrossCheck", "l2r", l2r, "int16", (None, None), self.device)
 		h, w = l2r.shape
-		self._call("sgm_cross_check_device", l2r.data_ptr(), r2l.data_ptr(), w, h, int(thCross), _stream_handle(l2r.device))
+		pr = _arg("ConsistencyCrossCheck", "r2l", r2l, "int16", (h, w), self.device)
+		self._call("sgm_cross_check_device", pl, pr, w, h, int(thCross), _stream_handle(self.device))
 		return l2r
 
 	def RefineDisparityMap(self, disparityMap, imagePixels, accums=None, subpixelSteps: int = 4):
-		"""SemiGlobalMatcher::RefineDisparityMap (LC-blend) on CUDA tensors; disparityMap in place."""
-		self._call("sgm_refine_device", imagePixels.data_ptr(), accums.data_ptr() if accums is not None else None,
-			disparityMap.data_ptr(), disparityMap.numel(), int(subpixelSteps), _stream_handle(disparityMap.device))
+		"""SemiGlobalMatcher::RefineDisparityMap (LC-blend) on CUDA tensors: the int16 disparityMap in place, the pixel map of its
+		pixels and the 16-bit accumulated costs (None: those of the last match with this pixel map on the context)."""
+		pd = _arg("RefineDisparityMap", "disparityMap", disparityMap, "int16", (None, None), self.device)
+		ppx = _arg("RefineDisparityMap", "imagePixels", imagePixels, 16, (disparityMap.numel(),), self.device)
+		pac = _arg("RefineDisparityMap", "accums", accums, _U16, None, self.device)
+		self._call("sgm_refine_device", ppx, pac, pd, disparityMap.numel(), int(subpixelSteps), _stream_handle(self.device))
 		return disparityMap
 
 	def MatchPairDevice(self, leftGray, leftColor, rightGray, rightColor, minDisp: int, maxDisp: int, thCross: int = 1, subpixelSteps: int = 4,
@@ -566,7 +596,7 @@ class SemiGlobalMatcher(_Context):
 		overlap (default): the two matches run on two contexts / streams (they are independent until the cross-check), so the
 		aggregation kernels of the two share the SMs."""
 		import torch
-		h, w = leftGray.shape
+		(h, w), _ = self._images("MatchPairDevice", leftGray, leftColor, rightGray, rightColor, self.device)
 		nv = (w-6)*(h-6)
 		num = int(maxDisp-minDisp)
 		dev = leftGray.device
@@ -592,7 +622,7 @@ class SemiGlobalMatcher(_Context):
 			ldisp, _ = self.MatchDevice(leftGray, leftColor, rightGray, pxl, nv*num)
 		else:
 			if getattr(self, "_peer", None) is None:
-				self._peer = SemiGlobalMatcher(device=dev.index or 0)
+				self._peer = SemiGlobalMatcher(device=self.device)
 				self._peer.prm = self.prm
 				self._side = torch.cuda.Stream(device=dev)
 			main = torch.cuda.current_stream(dev)
@@ -630,19 +660,18 @@ class SemiGlobalMatcher(_Context):
 		Returns (leftDisparity * subpixelSteps, cost, levels) with levels = [{"size": (w, h), "numCosts": (right, left)}, ...];
 		cost holds the uint16 bit pattern in an int16 tensor."""
 		import torch
-		h, w = leftGray.shape
-		dev = leftGray.device
+		where = "MatchPairHierarchicalDevice"
+		(h, w), images = self._images(where, leftGray, leftColor, rightGray, rightColor, self.device)
+		masks = [_arg(where, name, m, "uint8", (h, w), self.device) for name, m in (("leftMask", leftMask), ("rightMask", rightMask))]
 		sizes, (iw, ih) = self.HierarchyLevels(w, h, minResolution)
-		if initDisparity is not None and tuple(initDisparity.shape) != (ih, iw):
-			raise ValueError("initDisparity must be %d x %d (rows x columns)" % (ih, iw))
-		ptr = lambda t: t.data_ptr() if t is not None else None
+		pinit = _arg(where, "initDisparity", initDisparity, "int16", (ih, iw), self.device)
+		dev = leftGray.device
 		disp = torch.empty((h-6, w-6), dtype=torch.int16, device=dev)
 		cost = torch.empty((h-6, w-6), dtype=torch.int16, device=dev)
 		nums = (C.c_uint64*(2*len(sizes)))()
 		speckle = OPTDENSE.nSpeckleSize if nSpeckleSize is None else nSpeckleSize
-		self._call("sgm_match_hierarchical_device", leftGray.data_ptr(), leftColor.data_ptr(), rightGray.data_ptr(), rightColor.data_ptr(),
-			w, h, ptr(initDisparity), iw, ih, ptr(leftMask), ptr(rightMask), int(minResolution), int(speckle), int(thCross),
-			int(subpixelSteps), C.byref(self.prm), disp.data_ptr(), cost.data_ptr(), nums, _stream_handle(dev))
+		self._call("sgm_match_hierarchical_device", *images, w, h, pinit, iw, ih, *masks, int(minResolution), int(speckle), int(thCross),
+			int(subpixelSteps), C.byref(self.prm), disp.data_ptr(), cost.data_ptr(), nums, _stream_handle(self.device))
 		levels = [{"size": sizes[k], "numCosts": (int(nums[2*k]), int(nums[2*k+1]))} for k in range(len(sizes))]
 		return disp, cost, levels
 
@@ -650,63 +679,69 @@ class SemiGlobalMatcher(_Context):
 	def Disparity2RangeMap(self, disparityMap, maskMap, minNumDisp: int = 3, minNumDispInvalid: int = 16):
 		"""-> (PixelMap as a (maskH*maskW, 16) uint8 tensor, numCosts) for the 2x grid of maskMap (int16 / uint8 tensors)"""
 		import torch
+		pd = _arg("Disparity2RangeMap", "disparityMap", disparityMap, "int16", (None, None), self.device)
+		pm = _arg("Disparity2RangeMap", "maskMap", maskMap, "uint8", (None, None), self.device)
 		h, w = disparityMap.shape
 		mh, mw = maskMap.shape
 		px = torch.empty((mh*mw, 16), dtype=torch.uint8, device=disparityMap.device)
 		num = C.c_uint64()
-		self._call("sgm_range_map_device", disparityMap.data_ptr(), w, h, maskMap.data_ptr(), mw, mh, int(minNumDisp),
-			int(minNumDispInvalid), px.data_ptr(), C.byref(num), _stream_handle(disparityMap.device))
+		self._call("sgm_range_map_device", pd, w, h, pm, mw, mh, int(minNumDisp), int(minNumDispInvalid), px.data_ptr(), C.byref(num),
+			_stream_handle(self.device))
 		return px, int(num.value)
 
 	def FlipDirection(self, l2r):
 		"""-> the right->left int16 map of a left->right one"""
 		import torch
+		pl = _arg("FlipDirection", "l2r", l2r, "int16", (None, None), self.device)
 		h, w = l2r.shape
 		r2l = torch.empty_like(l2r)
-		self._call("sgm_flip_direction_device", l2r.data_ptr(), r2l.data_ptr(), w, h, _stream_handle(l2r.device))
+		self._call("sgm_flip_direction_device", pl, r2l.data_ptr(), w, h, _stream_handle(self.device))
 		return r2l
 
 	def UpscaleMask(self, maskMap, size2x):
 		"""-> the uint8 mask of size2x = (width, height)"""
 		import torch
+		pm = _arg("UpscaleMask", "maskMap", maskMap, "uint8", (None, None), self.device)
 		h, w = maskMap.shape
 		out = torch.empty((int(size2x[1]), int(size2x[0])), dtype=torch.uint8, device=maskMap.device)
-		self._call("sgm_upscale_mask_device", maskMap.data_ptr(), w, h, out.data_ptr(), int(size2x[0]), int(size2x[1]),
-			_stream_handle(maskMap.device))
+		self._call("sgm_upscale_mask_device", pm, w, h, out.data_ptr(), int(size2x[0]), int(size2x[1]), _stream_handle(self.device))
 		return out
 
 	def ExtractMask(self, disparityMap, maskMap, thValid: int = 3):
 		"""maskMap (uint8, same size) in place"""
+		pd = _arg("ExtractMask", "disparityMap", disparityMap, "int16", (None, None), self.device)
 		h, w = disparityMap.shape
-		self._call("sgm_extract_mask_device", disparityMap.data_ptr(), maskMap.data_ptr(), w, h, int(thValid),
-			_stream_handle(disparityMap.device))
+		pm = _arg("ExtractMask", "maskMap", maskMap, "uint8", (h, w), self.device)
+		self._call("sgm_extract_mask_device", pd, pm, w, h, int(thValid), _stream_handle(self.device))
 		return maskMap
 
 	def FilterSpeckles(self, disparityMap, newVal: int = NO_DISP, maxSpeckleSize: Optional[int] = None, maxDiff: int = 5):
 		"""cv::filterSpeckles on an int16 tensor, in place; maxSpeckleSize defaults to OPTDENSE.nSpeckleSize"""
+		pd = _arg("FilterSpeckles", "disparityMap", disparityMap, "int16", (None, None), self.device)
 		h, w = disparityMap.shape
 		size = OPTDENSE.nSpeckleSize if maxSpeckleSize is None else maxSpeckleSize
-		self._call("sgm_filter_speckles_device", disparityMap.data_ptr(), w, h, int(newVal), int(size), int(maxDiff),
-			_stream_handle(disparityMap.device))
+		self._call("sgm_filter_speckles_device", pd, w, h, int(newVal), int(size), int(maxDiff), _stream_handle(self.device))
 		return disparityMap
 
 	def ResizeAreaU8(self, image, factor: int):
 		"""cv::resize(image, Size(), 1/factor, 1/factor, INTER_AREA) of a uint8 (H, W[, C]) tensor with 1, 3 or 4 channels"""
 		import torch
+		pi = _arg("ResizeAreaU8", "image", image, "uint8", (None, None) if len(image.shape) == 2 else (None, None, (1, 3, 4)), self.device)
 		h, w = image.shape[:2]
 		cn = 1 if image.dim() == 2 else image.shape[2]
 		dh, dw = int(np.rint(h/float(factor))), int(np.rint(w/float(factor)))
 		out = torch.empty((dh, dw) + tuple(image.shape[2:]), dtype=torch.uint8, device=image.device)
-		self._call("resize_area_u8_device", image.data_ptr(), w, h, int(cn), int(factor), out.data_ptr(), _stream_handle(image.device))
+		self._call("resize_area_u8_device", pi, w, h, int(cn), int(factor), out.data_ptr(), _stream_handle(self.device))
 		return out
 
 	def LevelMask(self, mask, levelSize):
 		"""first level's mask: NEAREST resize of the uint8 mask to levelSize = (w, h), cropped to the valid region"""
 		import torch
+		pm = _arg("LevelMask", "mask", mask, "uint8", (None, None), self.device)
 		h, w = mask.shape
 		lw, lh = int(levelSize[0]), int(levelSize[1])
 		out = torch.empty((lh-6, lw-6), dtype=torch.uint8, device=mask.device)
-		self._call("sgm_level_mask_device", mask.data_ptr(), w, h, lw, lh, out.data_ptr(), _stream_handle(mask.device))
+		self._call("sgm_level_mask_device", pm, w, h, lw, lh, out.data_ptr(), _stream_handle(self.device))
 		return out
 
 	# fusion-mode -2: the disparity maps of the pairs that contain an image, projected into it and fused (SemiGlobalMatcher::Fuse,
@@ -725,31 +760,19 @@ class SemiGlobalMatcher(_Context):
 			raise _lib.B200MVSError("b200mvs_sgm_pair_q failed with status %d (a zero focal length in Kleft)" % rc)
 		return out.reshape(4, 4)
 
-	@staticmethod
-	def _pairs(pairs, device: bool):
-		"""[(disparity, cost or None, Q, subpixelSteps), ...] -> (ctypes b200mvs_sgm_pair array, keepalive list)"""
+	def _pairs(self, pairs, device: bool, where: str = "Fuse"):
+		"""[(disparity, cost or None, Q, subpixelSteps), ...] -> (ctypes b200mvs_sgm_pair array, keepalive list).  Host maps are
+		converted to int16 / uint16; device maps must be CUDA tensors on the context's device."""
 		if not 1 <= len(pairs) <= _lib.SGM_MAX_PAIRS:
-			raise ValueError("between 1 and %d pairs" % _lib.SGM_MAX_PAIRS)
+			raise ValueError("%s: between 1 and %d pairs" % (where, _lib.SGM_MAX_PAIRS))
+		home = self.device if device else None
 		arr = (_lib.SgmPair*len(pairs))()
 		keep = []
-		for o, (disp, cost, Q, steps) in zip(arr, pairs):
-			if device:
-				if not (_is_torch(disp) and disp.is_cuda and str(disp.dtype) == "torch.int16" and disp.is_contiguous()):
-					raise ValueError("disparity must be a contiguous int16 CUDA tensor")
-				if cost is not None and not (_is_torch(cost) and cost.is_cuda and cost.dtype.itemsize == 2 and cost.is_contiguous()
-						and cost.device == disp.device):
-					raise ValueError("cost must be a contiguous 16-bit CUDA tensor on the disparity's device")
-				dptr, cptr = disp.data_ptr(), (cost.data_ptr() if cost is not None else None)
-			else:
-				disp = np.ascontiguousarray(disp, np.int16)
-				cost = None if cost is None else np.ascontiguousarray(cost, np.uint16)
-				dptr, cptr = disp.ctypes.data, (cost.ctypes.data if cost is not None else None)
-			if len(disp.shape) != 2:
-				raise ValueError("disparity must be a 2-D map")
-			if cost is not None and tuple(cost.shape) != tuple(disp.shape):
-				raise ValueError("cost map of shape %s for a disparity map of shape %s" % (tuple(cost.shape), tuple(disp.shape)))
+		for k, (o, (disp, cost, Q, steps)) in enumerate(zip(arr, pairs)):
+			disp, cost = _host(disp, np.int16, home), _host(cost, np.uint16, home)
+			o.disparity = _arg(where, "pairs[%d] disparity" % k, disp, "int16", (None, None), home)
+			o.cost = _arg(where, "pairs[%d] cost" % k, cost, _U16, tuple(disp.shape), home)
 			keep += [disp, cost]
-			o.disparity, o.cost = dptr, cptr
 			o.height, o.width = (int(x) for x in disp.shape)
 			o.subpixelSteps = int(steps)
 			o.Q[:] = list(np.asarray(Q, np.float64).reshape(16))
@@ -761,12 +784,12 @@ class SemiGlobalMatcher(_Context):
 		tensors; rejected pixels are 0 in all three, conf is 0 without a cost map."""
 		import torch
 		W, H = int(size[0]), int(size[1])
-		arr, keep = self._pairs([(disparityMap, costMap, Q, subpixelSteps)], True)
+		arr, keep = self._pairs([(disparityMap, costMap, Q, subpixelSteps)], True, "ProjectDisparity2DepthMap")
 		dev = disparityMap.device
 		depth = torch.empty((H, W), dtype=torch.float32, device=dev)
 		rng = torch.empty((H, W, 2), dtype=torch.float32, device=dev)
 		conf = torch.empty((H, W), dtype=torch.float32, device=dev)
-		self._call("sgm_project_disparity_device", arr, W, H, depth.data_ptr(), rng.data_ptr(), conf.data_ptr(), _stream_handle(dev))
+		self._call("sgm_project_disparity_device", arr, W, H, depth.data_ptr(), rng.data_ptr(), conf.data_ptr(), _stream_handle(self.device))
 		return depth, rng, conf
 
 	def Fuse(self, pairs, size, minViews: int = 2, K=None):
@@ -786,7 +809,7 @@ class SemiGlobalMatcher(_Context):
 			conf = torch.empty((H, W), dtype=torch.float32, device=dev)
 			normal = torch.empty((H, W, 3), dtype=torch.float32, device=dev) if k is not None else None
 			self._call("sgm_fuse_device", arr, len(pairs), W, H, int(minViews), kp, depth.data_ptr(), conf.data_ptr(),
-				normal.data_ptr() if normal is not None else None, _stream_handle(dev))
+				normal.data_ptr() if normal is not None else None, _stream_handle(self.device))
 		else:
 			depth = np.zeros((H, W), np.float32); conf = np.zeros((H, W), np.float32)
 			normal = np.zeros((H, W, 3), np.float32) if k is not None else None
@@ -811,14 +834,12 @@ def EstimateNormalMap(K, depthMap):
 	camera-space normals (0 where undetermined).  K: 3x3, converted to float as the reference's Matrix3x3f argument.  Runs on a
 	context kept per device."""
 	import torch
-	if not (_is_torch(depthMap) and depthMap.is_cuda and depthMap.dtype == torch.float32 and depthMap.dim() == 2 and depthMap.is_contiguous()):
-		raise ValueError("depthMap must be a contiguous 2-D float32 CUDA tensor")
-	dev = depthMap.device
-	ctx = _device_context(dev)
+	ptr = _arg("EstimateNormalMap", "depthMap", depthMap, "float32", (None, None), _cuda_index(depthMap))
+	ctx = _device_context(depthMap.device)
 	k = np.ascontiguousarray(K, np.float64).reshape(9)
 	h, w = depthMap.shape
-	normal = torch.empty((h, w, 3), dtype=torch.float32, device=dev)
-	ctx._call("estimate_normal_map_device", depthMap.data_ptr(), w, h, k.ctypes.data, normal.data_ptr(), _stream_handle(dev))
+	normal = torch.empty((h, w, 3), dtype=torch.float32, device=depthMap.device)
+	ctx._call("estimate_normal_map_device", ptr, w, h, k.ctypes.data, normal.data_ptr(), _stream_handle(ctx.device))
 	return normal
 
 
@@ -844,40 +865,24 @@ def FuseDepthMaps(views, nMinViewsFuse: int = 2, fDepthDiffThreshold: float = 0.
 	contiguous) take b200mvs_fuse_depth_maps_device on a context kept per device: the same point cloud, bit for bit, with the
 	pixels of each image resolved in parallel; a neighbour list must not repeat an image ID there."""
 	lib = _lib.load()
-	device = any(_is_torch(v.get("depth")) for v in views)
+	first = next((v["depth"] for v in views if _is_torch(v.get("depth"))), None)
+	device = None if first is None else _cuda_index(first)
 	n = len(views)
 	arr = (_lib.FuseView*n)()
 	keep = []
-	dev = None
 	for i, v in enumerate(views):
 		o = arr[i]
 		d = v.get("depth")
 		if d is not None:
-			if device:
-				import torch
-				dev = d.device if dev is None else dev
-				if not (_is_torch(d) and d.is_cuda and d.device == dev and d.dtype == torch.float32 and d.dim() == 2 and d.is_contiguous()):
-					raise ValueError("views[%d].depth must be a contiguous 2-D float32 CUDA tensor on the device of the other views" % i)
-			elif not (isinstance(d, np.ndarray) and d.dtype == np.float32 and d.flags.c_contiguous and d.flags.writeable):
-				raise ValueError("views[%d].depth must be a writeable C-contiguous float32 array (it is modified in place)" % i)
+			o.depth = _arg("FuseDepthMaps", "views[%d].depth" % i, d, "float32", (None, None), device)
+			if device is None and not d.flags.writeable:
+				raise ValueError("FuseDepthMaps: views[%d].depth must be writeable (it is modified in place)" % i)
 			o.height, o.width = d.shape
-			o.depth = d.data_ptr() if device else d.ctypes.data
-			for key, dt, shape in (("normal", np.float32, tuple(d.shape)+(3,)), ("conf", np.float32, tuple(d.shape)),
-					("color", np.uint8, tuple(d.shape)+(3,))):
+			for key, dt, ch in (("normal", "float32", (3,)), ("conf", "float32", ()), ("color", "uint8", (3,))):
 				a = v.get(key)
-				if a is None:
-					continue
-				if device:
-					if not (_is_torch(a) and a.device == dev and str(a.dtype) == "torch."+np.dtype(dt).name and tuple(a.shape) == shape):
-						raise ValueError("views[%d].%s must be a %s CUDA tensor of shape %s on the depth's device" % (i, key, np.dtype(dt).name, shape))
-					a = a.contiguous()
-					ptr = a.data_ptr()
-				else:
-					a = np.ascontiguousarray(a, dt)
-					if a.shape != shape:
-						raise ValueError("views[%d].%s has shape %s, expected %s" % (i, key, a.shape, shape))
-					ptr = a.ctypes.data
-				keep.append(a); setattr(o, key, ptr)
+				a = a.contiguous() if _is_torch(a) and a.is_cuda else _host(a, dt, device)
+				keep.append(a)
+				setattr(o, key, _arg("FuseDepthMaps", "views[%d].%s" % (i, key), a, dt, tuple(d.shape)+ch, device))
 		for name in ("K", "R", "C"):
 			getattr(o, name)[:] = list(np.asarray(v[name], np.float64).ravel())
 		nb = np.ascontiguousarray(v.get("neighbors", []), np.uint32)
@@ -887,9 +892,9 @@ def FuseDepthMaps(views, nMinViewsFuse: int = 2, fDepthDiffThreshold: float = 0.
 		o.nSceneNeighbors = int(v.get("n_scene_neighbors", nb.size))
 	prm = _lib.FuseParams(int(nMinViewsFuse), float(fDepthDiffThreshold), float(fNormalDiffThreshold), int(bool(bEstimateColor)), int(bool(bEstimateNormal)))
 	cloud = C.c_void_p()
-	if device:
-		ctx = _device_context(dev)
-		ctx._call("fuse_depth_maps_device", arr, n, C.byref(prm), C.byref(cloud), _stream_handle(dev), C.byref(ctx.stats))
+	if device is not None:
+		ctx = _device_context(first.device)
+		ctx._call("fuse_depth_maps_device", arr, n, C.byref(prm), C.byref(cloud), _stream_handle(ctx.device), C.byref(ctx.stats))
 	else:
 		rc = lib.b200mvs_fuse_depth_maps(arr, n, C.byref(prm), C.byref(cloud))
 		if rc:
