@@ -74,6 +74,7 @@ int b200mvs_destroy(b200mvs_ctx* c) {
 	if (c->ev0) cudaEventDestroy(c->ev0);
 	if (c->ev1) cudaEventDestroy(c->ev1);
 	if (c->stream) cudaStreamDestroy(c->stream);
+	if (c->words) cudaFree(c->words);
 	delete c; // frees the device buffers
 	return B200MVS_OK;
 }

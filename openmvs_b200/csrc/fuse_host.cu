@@ -226,12 +226,6 @@ bool on_device(const b200mvs_ctx* ctx, const void* p) {
 	return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == ctx->device;
 }
 
-// the fixed counters of one call, in device memory
-struct FuseCounters {
-	unsigned long long nDepths, shared;
-	uint32_t nCand, nEdges, undecided, totals[2];
-};
-
 } // namespace
 
 extern "C" {
@@ -280,33 +274,35 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 	cudaStream_t s = stream_of(ctx, stream);
 	ctx->launches = 0;
 	ctx->fsRounds.clear();
-	const size_t nNbAll = std::max<size_t>(nbIds.size(), 1);
-	CK(ctx->fsClaim.reserve(std::max<size_t>(claimBytes, 1)));
-	for (int i = 0; i < nViews; ++i) if (views[i].depth) dv[i].claim = ctx->fsClaim.as<uint8_t>() + claimOff[i];
-	CK(ctx->fsViews.reserve(sizeof(FuseDevView)*nViews));
-	CK(ctx->fsNb.reserve(nNbAll*8));
-	CK(ctx->fsAny.reserve(sizeof(int)*nViews));
-	CK(ctx->fsCount.reserve(sizeof(FuseCounters)));
-	int* dNb = ctx->fsNb.as<int>();
-	uint32_t* dBase = (uint32_t*)(dNb + nNbAll);
-	FuseCounters* cnt = ctx->fsCount.as<FuseCounters>();
+	// the call's scratch: the view table, the neighbour IDs and bases, the claim maps, which images have a depth, and the
+	// candidate flags and list of a round, sized for the largest image a round can fuse
+	size_t maxNp = 0;
+	for (int i = 0; i < nViews; ++i) if (views[i].depth && views[i].nSceneNeighbors > 0) maxNp = std::max(maxNp, (size_t)dv[i].w*dv[i].h);
+	Carve scratch(ctx->fsScratch);
+	FuseDevView* dViews; int *dNb, *dAny; uint32_t *dBase, *cand; uint8_t *claim, *flags;
+	scratch.take(dViews, nViews); scratch.take(dNb, nbIds.size()); scratch.take(dBase, nbBase.size());
+	scratch.take(claim, std::max<size_t>(claimBytes, 1)); scratch.take(dAny, nViews); scratch.take(flags, maxNp); scratch.take(cand, maxNp);
+	CK(scratch.commit());
+	for (int i = 0; i < nViews; ++i) if (views[i].depth) dv[i].claim = claim + claimOff[i];
+	ReadBack* rb; CK(read_back(ctx, rb));
+	FuseCounters* cnt = &rb->fuse;
 	CK(cudaEventRecord(ctx->ev0, s));
-	CK(cudaMemcpyAsync(ctx->fsViews.p, dv.data(), sizeof(FuseDevView)*nViews, cudaMemcpyHostToDevice, s));
+	CK(cudaMemcpyAsync(dViews, dv.data(), sizeof(FuseDevView)*nViews, cudaMemcpyHostToDevice, s));
 	if (!nbIds.empty()) {
 		CK(cudaMemcpyAsync(dNb, nbIds.data(), nbIds.size()*4, cudaMemcpyHostToDevice, s));
 		CK(cudaMemcpyAsync(dBase, nbBase.data(), nbBase.size()*4, cudaMemcpyHostToDevice, s));
 	}
-	if (claimBytes) CK(cudaMemsetAsync(ctx->fsClaim.p, 0, claimBytes, s));
-	CK(cudaMemsetAsync(ctx->fsAny.p, 0, sizeof(int)*nViews, s));
+	if (claimBytes) CK(cudaMemsetAsync(claim, 0, claimBytes, s));
+	CK(cudaMemsetAsync(dAny, 0, sizeof(int)*nViews, s));
 	CK(cudaMemsetAsync(cnt, 0, sizeof(FuseCounters), s));
 	// which images have a depth > 0 (the host form's validity test), then the same order of the images as the host form
 	for (int i = 0; i < nViews; ++i)
 		if (views[i].depth && views[i].nSceneNeighbors > 0) {
-			CK(fuse_launch_any_positive(views[i].depth, (size_t)views[i].width*views[i].height, ctx->fsAny.as<int>()+i, s));
+			CK(fuse_launch_any_positive(views[i].depth, (size_t)views[i].width*views[i].height, dAny+i, s));
 			++ctx->launches;
 		}
 	std::vector<int> anyI(nViews);
-	CK(cudaMemcpyAsync(anyI.data(), ctx->fsAny.p, sizeof(int)*nViews, cudaMemcpyDeviceToHost, s));
+	CK(cudaMemcpyAsync(anyI.data(), dAny, sizeof(int)*nViews, cudaMemcpyDeviceToHost, s));
 	CK(cudaStreamSynchronize(s));
 	uint64_t d2h = sizeof(int)*nViews;
 	const FusePlan plan = fuse_plan(views, nViews, prm, std::vector<char>(anyI.begin(), anyI.end()));
@@ -329,15 +325,12 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 		const size_t np = (size_t)A.width*A.height;
 		const int nNb = A.nNeighbors;
 		FuseRound R;
-		R.views = ctx->fsViews.as<FuseDevView>(); R.a = a; R.nNb = nNb; R.nb = dNb + nbOff[a]; R.base = dBase + nbOff[a];
+		R.views = dViews; R.a = a; R.nNb = nNb; R.nb = dNb + nbOff[a]; R.base = dBase + nbOff[a];
 		R.bNormalMap = plan.bNormalMap; R.bColor = plan.bColor; R.bNormal = plan.bNormal;
 		R.nMin = plan.nMin; R.thDepth = plan.thDepth; R.normalError = plan.normalError;
 		b200mvs_ctx::FuseRoundStat st{a, 0, 0, 0, 0, 0.f};
 		CK(cudaEventRecord(ev.b, s));
 		// the candidates: pixels with a depth and no claim, in raster order
-		CK(ctx->fsFlags.reserve(np)); CK(ctx->fsCand.reserve(np*4));
-		uint8_t* flags = ctx->fsFlags.as<uint8_t>();
-		uint32_t* cand = ctx->fsCand.as<uint32_t>();
 		CK(fuse_launch_candidates(A.depth, dv[a].claim, np, flags, &cnt->nDepths, s));
 		FUSE_CUB(fuse_select(tmp, need, flags, cand, &cnt->nCand, np, s));
 		ctx->launches += 2;
@@ -347,22 +340,20 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 		d2h += 4;
 		st.candidates = nCand;
 		if (nCand > 0) {
+			// the round's scratch, carved again by the next round (this one has finished when its events have): per candidate the
+			// acceptance, the point flag, ID, view count and view offset; per (candidate, neighbour) edge its type, status and
+			// target, the selected edges and their sort keys
 			const size_t ne = (size_t)nCand*nNb;
-			CK(ctx->fsAcc.reserve(nCand)); CK(ctx->fsIsPt.reserve(nCand*4)); CK(ctx->fsPtId.reserve(nCand*4));
-			CK(ctx->fsNv.reserve(nCand*4)); CK(ctx->fsVOff.reserve(nCand*4));
-			CK(ctx->fsTyp.reserve(std::max<size_t>(ne, 1))); CK(ctx->fsStatus.reserve(std::max<size_t>(ne, 1)));
-			CK(ctx->fsTgt.reserve(std::max<size_t>(ne, 1)*4));
-			uint8_t* acc = ctx->fsAcc.as<uint8_t>();
-			uint8_t* typ = ctx->fsTyp.as<uint8_t>();
-			uint8_t* status = ctx->fsStatus.as<uint8_t>();
-			uint32_t* tgt = ctx->fsTgt.as<uint32_t>();
-			uint32_t *keys = nullptr, *edges = nullptr;
+			Carve round(ctx->fsRoundScratch);
+			uint8_t *acc, *typ, *status; uint32_t *isPt, *ptId, *nv, *vOff, *tgt, *e1 = nullptr, *k1 = nullptr, *keys = nullptr, *edges = nullptr;
+			round.take(acc, nCand); round.take(isPt, nCand); round.take(ptId, nCand); round.take(nv, nCand); round.take(vOff, nCand);
+			round.take(typ, std::max<size_t>(ne, 1)); round.take(status, std::max<size_t>(ne, 1)); round.take(tgt, std::max<size_t>(ne, 1));
+			if (ne > 0) { round.take(e1, ne); round.take(edges, ne); round.take(k1, ne); round.take(keys, ne); }
+			CK(round.commit());
 			CK(cudaMemsetAsync(acc, 0, nCand, s));
 			if (ne > 0) {
 				// the edges: type and target from the maps at the start of the round; the claim and zero edges, grouped by target in
 				// raster order of their owners (the radix sort is stable and its input is in edge order)
-				CK(ctx->fsEdge.reserve(ne*4)); CK(ctx->fsEdge2.reserve(ne*4)); CK(ctx->fsKeys.reserve(ne*4)); CK(ctx->fsKeys2.reserve(ne*4));
-				uint32_t* e1 = ctx->fsEdge.as<uint32_t>();
 				CK(fuse_launch_classify(R, cand, nCand, typ, tgt, s));
 				FUSE_CUB(fuse_select(tmp, need, typ, e1, &cnt->nEdges, ne, s));
 				ctx->launches += 2;
@@ -370,8 +361,6 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 				CK(cudaStreamSynchronize(s));
 				d2h += 4;
 				if (nEdges > 0) {
-					uint32_t* k1 = ctx->fsKeys.as<uint32_t>();
-					keys = ctx->fsKeys2.as<uint32_t>(); edges = ctx->fsEdge2.as<uint32_t>();
 					int endBit = 1;
 					while (endBit < 32 && (1ull << endBit) < (uint64_t)nbBase[nbOff[a]+nNb-1] + (uint64_t)dv[nbIds[nbOff[a]+nNb-1]].w*dv[nbIds[nbOff[a]+nNb-1]].h)
 						++endBit;
@@ -398,8 +387,6 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 			// every edge live or dead, which the views of a point and its zeroed depths need
 			if (nEdges > 0) { CK(fuse_launch_walk(keys, edges, nEdges, nNb, acc, status, s)); ++ctx->launches; }
 			// point IDs and view offsets in raster order, then the points
-			uint32_t *isPt = ctx->fsIsPt.as<uint32_t>(), *ptId = ctx->fsPtId.as<uint32_t>(), *nv = ctx->fsNv.as<uint32_t>(),
-				*vOff = ctx->fsVOff.as<uint32_t>();
 			CK(fuse_launch_count(R, nCand, typ, status, acc, isPt, nv, s));
 			FUSE_CUB(fuse_scan(tmp, need, isPt, ptId, nCand, s));
 			FUSE_CUB(fuse_scan(tmp, need, nv, vOff, nCand, s));

@@ -1,8 +1,14 @@
 // host_ctx.h — the engine context behind the C-ABI (b200mvs_ctx) and the helpers shared by its host files: capi.cu (lifecycle
 // and settings), pm_host.cu (PatchMatch), sgm_host.cu (SGM), post_host.cu (post-processing and image preparation).
 // Internal to the library; include/b200mvs.h is the interface.
+//
+// Device scratch is owned by subsystem: the context keeps one arena per subsystem, and each entry point carves all of its
+// temporaries from its arena once, before its first launch (Carve), so no pointer it hands a kernel moves during the call.
+// The few words the host reads back before it can size a carve sit in one small block (ReadBack, read_back); the other
+// device buffers of the context are state that outlives a call.
 #pragma once
 #include "../../include/b200mvs.h"
+#include "sgm_common.cuh"
 #include "sgm_front_sched.h"
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -13,7 +19,7 @@
 #include <string>
 #include <vector>
 
-// Grow-only device scratch that owns its memory: freed when the buffer (and so the context) is destroyed.  Move-only: the
+// Grow-only device memory that owns its allocation: freed when the buffer (and so the context) is destroyed.  Move-only: the
 // move constructor deletes the implicit copies.
 struct DevBuf {
 	void* p = nullptr; size_t cap = 0;
@@ -31,45 +37,74 @@ struct DevBuf {
 	template <typename T> T* as() const { return (T*)p; }
 };
 
+// One call's scratch carved from an arena: take() declares each slice with the pointer it sets, commit() reserves the total
+// once and only then sets the pointers, each 256-byte aligned as cudaMalloc's.  A carve's pointers stay valid until its arena
+// is carved again, so an entry point commits once, before its first launch, and calls that nest carve different arenas.
+struct Carve {
+	explicit Carve(DevBuf& arena) : arena(arena) {}
+	template <typename T> void take(T*& p, size_t n) { take_bytes(&p, n*sizeof(T)); }
+	void take_bytes(void* ptrAddr, size_t bytes) { slices.push_back({ptrAddr, bytes, 0}); }
+	bool empty() const { return slices.empty(); }
+	cudaError_t commit() {
+		size_t total = 0;
+		for (Slice& s: slices) { s.off = total; total += (s.bytes+255) & ~(size_t)255; }
+		const cudaError_t e = arena.reserve(total);
+		if (e != cudaSuccess) return e;
+		for (Slice& s: slices) { void* p = arena.as<uint8_t>()+s.off; memcpy(s.ptrAddr, &p, sizeof(p)); }
+		return cudaSuccess;
+	}
+private:
+	struct Slice { void* ptrAddr; size_t bytes, off; };
+	DevBuf& arena;
+	std::vector<Slice> slices;
+};
+
+// FuseDepthMaps (device form): the counters of one call
+struct FuseCounters {
+	unsigned long long nDepths, shared;
+	uint32_t nCand, nEdges, undecided, totals[2];
+};
+
+// The device words the host reads back before it can size a call's scratch, one field per user (read_back)
+struct ReadBack {
+	SGMMapStats mapStats;                     // SGM match: statistics of the pixel map
+	unsigned long long rangeTotal;            // tSGM range map: the size of the volume
+	int minMax[2];                            // tSGM without levels: the disparity range of the initial map
+	int nArcs;                                // RemoveSmallSegments: one-way edges between segments
+	FuseCounters fuse;                        // FuseDepthMaps (device form)
+};
+
 struct b200mvs_ctx {
 	int device = 0;
 	b200mvs_params prm;
 	std::string err;
 	cudaStream_t stream = nullptr;
 	cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-	// grow-only device scratch
+	// scratch arenas
 	DevBuf stage;                             // the host forms' staged inputs and outputs (HostCall)
-	std::vector<DevBuf> imgs;                 // gray images converted on the device from 8-bit colour views (toGray)
-	std::vector<DevBuf> pyr;                  // per-view pyramid levels (all levels packed)
-	DevBuf plane, cost, best, prior, lowPlane;
-	DevBuf dDepth, dNormal;                   // the initial estimate at the coarsest level
-	DevBuf sgCosts, sgAccums, sgAccums2, sgMax; // SGM scratch
-	// wave-front aggregation: cached schedule of the last (size, mode) and its scratch
+	DevBuf pmScratch;                         // PatchMatch estimate and building blocks
+	DevBuf sgmScratch;                        // SGM match
+	DevBuf tsgmScratch;                       // hierarchical (tSGM) level loop and its building blocks
+	DevBuf sfScratch;                         // SGM fusion and the normal map
+	DevBuf ppScratch;                         // post-processing: filter, small segments, gap interpolation
+	DevBuf fsScratch, fsRoundScratch;         // FuseDepthMaps (device form): the call, and one round of it
+	ReadBack* words = nullptr;                // allocated on first use, never moved
+	// wave-front aggregation: cached schedule of the last (size, mode)
 	struct FrontPass { FrontLaunch launch; DevBuf items, need; int nItems = 0; };   // launch.items is emptied once uploaded
 	std::vector<FrontPass> sgFront; int sgFrontKey[6] = {0, 0, 0, 0, 0, 0};
-	DevBuf sgFrontCtl, sgFrontState, sgFrontMeta;
 	cudaStream_t sgSide[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // side streams of the ragged aggregation
 	cudaEvent_t sgJoin[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}, sgFork = nullptr;
-	const void* sgLastPx = nullptr;           // pixel map of the volume in sgAccums (b200mvs_sgm_refine_device check)
-	// hierarchical matcher: level images, masks, disparity maps, pixel maps, Disparity2RangeMap / FlipDirection / speckle scratch
-	enum { TS_IMG, TS_MASKL, TS_MASKR, TS_MASKT, TS_DL, TS_DR, TS_DL0, TS_DR0, TS_PXL, TS_PXR, TS_RANGES, TS_SCAN, TS_KEYS, TS_LABELS,
-		TS_SIZES, TS_SMALL, TS_COUNT };
-	DevBuf ts[TS_COUNT];
-	DevBuf sfKeys, sfMaps;                    // SGM fusion: splat keys, per-pair depth / range / conf maps
-	DevBuf fltZ;                              // FilterDepthMap: z-buffer keys
-	DevBuf ppA, ppB, ppN;                     // RemoveSmallSegments labels/sizes, GapInterpolation temporaries
-	DevBuf ppK, ppArcs, ppPatch;              // RemoveSmallSegments: seed keys, one-way edges (+ counter), patched segment sizes
-	// FuseDepthMaps (device form): view table, neighbour lists, claim maps, per-round candidate / edge scratch, counters, the growing
-	// point-cloud outputs, and what each round of the last call did (b200mvs_fuse_round_stats)
-	DevBuf fsViews, fsNb, fsClaim, fsAny, fsFlags, fsCand, fsTyp, fsTgt, fsEdge, fsKeys, fsKeys2, fsEdge2, fsStatus, fsAcc;
-	DevBuf fsIsPt, fsPtId, fsNv, fsVOff, fsCub, fsCount;
+	// the accumulated costs of the last SGM match in its own scratch, and their pixel map (b200mvs_sgm_refine_device check)
+	const uint16_t* sgLastAccums = nullptr; const void* sgLastPx = nullptr;
+	// FuseDepthMaps (device form): CUB's temporary storage, the growing point-cloud outputs, and what each round of the last call
+	// did (b200mvs_fuse_round_stats)
+	DevBuf fsCub;
 	DevBuf fsOut[7];                          // points, normals, colors, offsets, views, weights, projs
 	struct FuseRoundStat { int image, iterations; uint64_t candidates, edges, shared; float ms; };
 	std::vector<FuseRoundStat> fsRounds;
 	b200mvs_debug dbg;                        // diagnostic switches (b200mvs_set_debug); all zero = the shipped kernels
 	const uint8_t* mask = nullptr; int maskW = 0, maskH = 0, maskPitch = 0; // ignore-mask of the reference view (device) or null
-	DevBuf maskBuf, maskLevel;                // staged host mask, mask of the current pyramid level
-	DevBuf refPad;                            // 16-byte aligned copy of a reference image whose pitch TMA cannot address
+	DevBuf maskBuf;                           // staged host mask
 	CUtensorMap tmapRef;                      // descriptor of the current level's reference image
 	std::vector<cudaEvent_t> sweepEv;         // event pairs around the sweep launches (stats only)
 	int nSweepEv = 0; bool timeSweeps = false;
@@ -87,6 +122,17 @@ inline int fail(b200mvs_ctx* c, int code, const char* what, cudaError_t e = cuda
 	return code;
 }
 #define CK(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) return fail(ctx, B200MVS_ERR_CUDA, #call, _e); } while (0)
+
+// The context's read-back block, allocated by the first call that needs it (a small allocation takes a page of its own)
+inline cudaError_t read_back(b200mvs_ctx* ctx, ReadBack*& words) {
+	if (!ctx->words) {
+		void* p = nullptr;
+		if (cudaError_t e = cudaMalloc(&p, sizeof(ReadBack))) return e;
+		ctx->words = (ReadBack*)p;
+	}
+	words = ctx->words;
+	return cudaSuccess;
+}
 
 // the caller's stream, or the context's when it passes none
 inline cudaStream_t stream_of(b200mvs_ctx* ctx, void* stream) { return stream ? (cudaStream_t)stream : ctx->stream; }
@@ -115,25 +161,22 @@ struct HostCall {
 	uint64_t h2d = 0, d2h = 0;
 	bool formRecordsEvents = false;   // the device form records ev0 / ev1 itself (b200mvs_sgm_match_device with statistics)
 
-	explicit HostCall(b200mvs_ctx* c) : ctx(c) {}
+	explicit HostCall(b200mvs_ctx* c) : ctx(c), carve(c->stage) {}
 	// `rows` rows of `row` bytes, `pitch` bytes apart on the host (0: packed); packed on the device
 	template <typename T> void in(T*& dev, const void* host, size_t row, int rows = 1, size_t pitch = 0) {
-		slices.push_back({&dev, host, nullptr, row, pitch ? pitch : row, rows, 0});
+		add(&dev, host, nullptr, row, rows, pitch ? pitch : row);
 	}
-	template <typename T> void out(T*& dev, void* host, size_t bytes) { slices.push_back({&dev, nullptr, host, bytes, bytes, 1, 0}); }
-	template <typename T> void inout(T*& dev, void* host, size_t bytes) { slices.push_back({&dev, host, host, bytes, bytes, 1, 0}); }
+	template <typename T> void out(T*& dev, void* host, size_t bytes) { add(&dev, nullptr, host, bytes, 1, bytes); }
+	template <typename T> void inout(T*& dev, void* host, size_t bytes) { add(&dev, host, host, bytes, 1, bytes); }
 
 	int stage() {
-		size_t total = 0;
-		for (Slice& s: slices) { s.off = total; total += (s.row*s.rows+255) & ~(size_t)255; }  // 256-byte aligned, as cudaMalloc's
-		CK(ctx->stage.reserve(total));
-		for (Slice& s: slices) {
-			void* p = ctx->stage.as<uint8_t>()+s.off;
-			memcpy(s.dev, &p, sizeof(p));
-			if (!s.src) continue;
-			if (s.pitch == s.row) CK(cudaMemcpyAsync(p, s.src, s.row*s.rows, cudaMemcpyHostToDevice, ctx->stream));
-			else CK(cudaMemcpy2DAsync(p, s.row, s.src, s.pitch, s.row, s.rows, cudaMemcpyHostToDevice, ctx->stream));
-			h2d += s.row*s.rows;
+		CK(carve.commit());
+		for (Copy& c: copies) {
+			memcpy(&c.p, c.dev, sizeof(c.p));
+			if (!c.src) continue;
+			if (c.pitch == c.row) CK(cudaMemcpyAsync(c.p, c.src, c.row*c.rows, cudaMemcpyHostToDevice, ctx->stream));
+			else CK(cudaMemcpy2DAsync(c.p, c.row, c.src, c.pitch, c.row, c.rows, cudaMemcpyHostToDevice, ctx->stream));
+			h2d += c.row*c.rows;
 		}
 		return B200MVS_OK;
 	}
@@ -151,17 +194,23 @@ struct HostCall {
 	}
 
 private:
-	struct Slice { void* dev; const void* src; void* dst; size_t row, pitch; int rows; size_t off; };
-	std::vector<Slice> slices;
+	// one staged buffer: the caller's device pointer (set by stage(), copied to p) and its host side
+	struct Copy { void* dev; void* p; const void* src; void* dst; size_t row, pitch; int rows; };
+	Carve carve;
+	std::vector<Copy> copies;
 
+	void add(void* dev, const void* src, void* dst, size_t row, int rows, size_t pitch) {
+		carve.take_bytes(dev, row*rows);
+		copies.push_back({dev, nullptr, src, dst, row, pitch, rows});
+	}
 	template <typename F> int launch(F& form) {
 		if (!formRecordsEvents) CK(cudaEventRecord(ctx->ev0, ctx->stream));
 		if (int rc = form(ctx->stream)) return rc;
 		if (!formRecordsEvents) CK(cudaEventRecord(ctx->ev1, ctx->stream));
-		for (const Slice& s: slices) {
-			if (!s.dst) continue;
-			CK(cudaMemcpyAsync(s.dst, ctx->stage.as<uint8_t>()+s.off, s.row, cudaMemcpyDeviceToHost, ctx->stream));
-			d2h += s.row;
+		for (const Copy& c: copies) {
+			if (!c.dst) continue;
+			CK(cudaMemcpyAsync(c.dst, c.p, c.row, cudaMemcpyDeviceToHost, ctx->stream));
+			d2h += c.row;
 		}
 		return B200MVS_OK;
 	}

@@ -146,9 +146,10 @@ Rows image_rows(const b200mvs_view& v) {
 Rows depth_rows(const b200mvs_view& v) { return rows_of(v.depth, (size_t)v.dwidth*sizeof(float), v.dstride_bytes, v.dheight); }
 
 // The engine's views of the caller's device views: float images and depth-maps with their pitch in floats.  Float images and
-// depth-maps are used in place; an 8-bit colour image is converted to gray (toGray) into the context's scratch on stream s.
-int stage_views(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, cudaStream_t s, std::vector<DView>& dv) {
-	if ((int)ctx->imgs.size() < nViews) ctx->imgs.resize(nViews);
+// depth-maps are used in place; an 8-bit colour image is converted to gray (toGray) into gray[i] on stream s.
+int stage_views(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, const std::vector<float*>& gray, cudaStream_t s,
+	std::vector<DView>& dv)
+{
 	dv.resize(nViews);
 	for (int i = 0; i < nViews; ++i) {
 		const b200mvs_view& v = views[i];
@@ -160,9 +161,8 @@ int stage_views(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, cudaStr
 		if (v.image) {
 			d.img = v.image; d.pitch = (int)(im.pitch/sizeof(float));
 		} else {
-			CK(ctx->imgs[i].reserve((size_t)v.width*v.height*sizeof(float)));
-			d.img = ctx->imgs[i].as<float>(); d.pitch = v.width;
-			CK(rs_launch_to_gray(v.image8, v.width, v.height, (int)im.pitch, v.channels8, v.bgr8 != 0, ctx->imgs[i].as<float>(), v.width, s));
+			d.img = gray[i]; d.pitch = v.width;
+			CK(rs_launch_to_gray(v.image8, v.width, v.height, (int)im.pitch, v.channels8, v.bgr8 != 0, gray[i], v.width, s));
 			++ctx->launches;
 		}
 		d.dmap = v.depth; d.dpitch = (int)(dm.pitch/sizeof(float));
@@ -205,20 +205,24 @@ EncodeTiledFn encode_tiled_fn() {
 	return fn;
 }
 
+// TMA needs a 16-byte aligned base and row pitch: the bytes of the aligned copy of a w x h float image at `base`, rows `pitchB`
+// bytes apart, that the sweep reads instead (0: the image is read in place)
+size_t ref_pad_bytes(const void* base, size_t pitchB, int w, int h) {
+	return ((uintptr_t)base & 15) || (pitchB & 15) ? ((((size_t)w*4)+15)&~(size_t)15)*h : 0;
+}
+
 // TMA descriptor of the reference image of one level: 2-D float tensor {W, H}, box = the tile a CTA
-// of the sweep kernel stages (72 x 16; the box may exceed the image, TMA zero-fills the outside).  TMA needs a
-// 16-byte aligned base and row pitch; an image that does not satisfy this (odd width, cv::Mat ROI) is first
-// copied to an aligned scratch image.  The sweep kernel has no other way to read the reference patch, so a
-// missing encoder or a refused descriptor fails the call.
-int prepare_ref_tmap(b200mvs_ctx* ctx, const DView& ref, cudaStream_t s) {
+// of the sweep kernel stages (72 x 16; the box may exceed the image, TMA zero-fills the outside).  An image that TMA cannot
+// address (odd width, cv::Mat ROI) is first copied to `pad`, of ref_pad_bytes.  The sweep kernel has no other way to read the
+// reference patch, so a missing encoder or a refused descriptor fails the call.
+int prepare_ref_tmap(b200mvs_ctx* ctx, const DView& ref, float* pad, cudaStream_t s) {
 	EncodeTiledFn enc = encode_tiled_fn();
 	if (!enc) return fail(ctx, B200MVS_ERR_CUDA, "cuTensorMapEncodeTiled: the driver does not provide the entry point");
 	const float* base = ref.img; size_t pitchB = (size_t)ref.pitch*4;
-	if (((uintptr_t)base & 15) || (pitchB & 15)) {
+	if (ref_pad_bytes(base, pitchB, ref.w, ref.h)) {
 		pitchB = (((size_t)ref.w*4)+15)&~(size_t)15;
-		CK(ctx->refPad.reserve(pitchB*ref.h));
-		CK(cudaMemcpy2DAsync(ctx->refPad.p, pitchB, ref.img, (size_t)ref.pitch*4, (size_t)ref.w*4, ref.h, cudaMemcpyDeviceToDevice, s));
-		base = ctx->refPad.as<float>();
+		CK(cudaMemcpy2DAsync(pad, pitchB, ref.img, (size_t)ref.pitch*4, (size_t)ref.w*4, ref.h, cudaMemcpyDeviceToDevice, s));
+		base = pad;
 	}
 	int bw, bh; pm_tma_box(&bw, &bh);
 	const cuuint64_t dims[2] = {(cuuint64_t)ref.w, (cuuint64_t)ref.h};
@@ -247,10 +251,54 @@ int launch_sweep_timed(b200mvs_ctx* ctx, const PMParams& P, bool geom, cudaStrea
 	return B200MVS_OK;
 }
 
-// The whole EstimateDepthMap on device-resident views.  d_depth/d_normal hold the initial
+// sub-resolution levels of an estimate call: none for a geometric pass
+int scale_levels(const b200mvs_params& o, int nGeometricIter) { return nGeometricIter < 0 ? std::max(0, o.nSubResolutionLevels) : 0; }
+
+// The scratch of an estimate call, carved from the PatchMatch arena: the gray images of 8-bit colour views, the pyramid levels
+// of every view (image, then depth-map), the state of the current and of the coarser level, the initial estimate at the
+// coarsest level, the mask of the current level and the TMA-aligned copy of the reference image
+struct PMScratch {
+	std::vector<float*> gray, pyr;
+	float4 *plane = nullptr, *lowPlane = nullptr;
+	float *cost = nullptr, *prior = nullptr, *dDepth = nullptr, *dNormal = nullptr, *refPad = nullptr;
+	uint32_t* best = nullptr;
+	uint8_t* maskLevel = nullptr;
+};
+int carve_estimate(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews, int nGeometricIter, PMScratch& S) {
+	Carve c(ctx->pmScratch);
+	const int W = views[0].width, H = views[0].height, totalScale = scale_levels(ctx->prm, nGeometricIter);
+	const size_t P0 = (size_t)W*H;
+	S.gray.assign(nViews, nullptr);
+	for (int i = 0; i < nViews; ++i) if (!views[i].image) c.take(S.gray[i], (size_t)views[i].width*views[i].height);
+	c.take(S.plane, P0); c.take(S.cost, P0); c.take(S.best, P0);
+	// the TMA pad of the reference image at level 0 (as stage_views describes it; a gray image is packed in the arena), then of the
+	// packed pyramid levels
+	const size_t pitch0 = views[0].image ? image_rows(views[0]).pitch/sizeof(float)*sizeof(float) : (size_t)W*sizeof(float);
+	size_t pad = ref_pad_bytes(views[0].image, pitch0, W, H);
+	if (totalScale > 0) {
+		c.take(S.prior, P0);
+		c.take(S.lowPlane, (size_t)(W/2+2)*(H/2+2));
+		if (ctx->mask) c.take(S.maskLevel, (size_t)(W/2+2)*(H/2+2));
+		const int wc = level_size(W, totalScale), hc = level_size(H, totalScale);
+		c.take(S.dDepth, (size_t)wc*hc); c.take(S.dNormal, (size_t)wc*hc*3);
+		// level 1 is the largest pyramid level
+		S.pyr.assign(nViews, nullptr);
+		for (int i = 0; i < nViews; ++i)
+			c.take(S.pyr[i], (size_t)level_size(views[i].width, 1)*level_size(views[i].height, 1)*(views[i].depth ? 2 : 1));
+		for (int sc = 1; sc <= totalScale; ++sc) {
+			const int w = level_size(W, sc), h = level_size(H, sc);
+			pad = std::max(pad, ref_pad_bytes(nullptr, (size_t)w*4, w, h));
+		}
+	}
+	if (pad) c.take(S.refPad, pad/sizeof(float));
+	CK(c.commit());
+	return B200MVS_OK;
+}
+
+// The whole EstimateDepthMap on device-resident views, in the scratch of carve_estimate.  d_depth/d_normal hold the initial
 // estimate (full resolution) and receive the result together with d_conf / d_views.
 int estimate_on_device(b200mvs_ctx* ctx, const DView* views, int nViews, float dMin, float dMax, int nGeometricIter,
-	float* d_depth, float* d_normal, float* d_conf, uint32_t* d_views, cudaStream_t s)
+	const PMScratch& S, float* d_depth, float* d_normal, float* d_conf, uint32_t* d_views, cudaStream_t s)
 {
 	const b200mvs_params& o = ctx->prm;
 	const int W = views[0].w, H = views[0].h;
@@ -260,25 +308,13 @@ int estimate_on_device(b200mvs_ctx* ctx, const DView* views, int nViews, float d
 	engine_schedule(o, geometric, nSweeps, nR);
 	// Philox phase of the first sweep of this call: photometric sweeps 0 .. nSweepsPhoto-1, then the geometric passes
 	const int sweepBase = geometric ? nSweepsPhoto + nGeometricIter*nSweeps : 0;
-	const int totalScale = !geometric ? std::max(0, o.nSubResolutionLevels) : 0;
+	const int totalScale = scale_levels(o, nGeometricIter);
 	const size_t P0 = (size_t)W*H;
 	if (ctx->mask && (ctx->maskW != W || ctx->maskH != H))
 		return fail(ctx, B200MVS_ERR_ARG, "ignore-mask size differs from the reference image");
-	CK(ctx->plane.reserve(P0*sizeof(float4)));
-	CK(ctx->cost.reserve(P0*sizeof(float)));
-	CK(ctx->best.reserve(P0*sizeof(uint32_t)));
-	if (totalScale > 0) {
-		CK(ctx->prior.reserve(P0*sizeof(float)));
-		CK(ctx->lowPlane.reserve((size_t)(W/2+2)*(H/2+2)*sizeof(float4)));
-		if (ctx->mask) CK(ctx->maskLevel.reserve((size_t)(W/2+2)*(H/2+2)));
-		if ((int)ctx->pyr.size() < nViews) ctx->pyr.resize(nViews);
-		// level 1 is the largest pyramid level: size the buffers once, so that no level re-allocates mid-stream
-		for (int i = 0; i < nViews; ++i)
-			CK(ctx->pyr[i].reserve((size_t)level_size(views[i].w, 1)*level_size(views[i].h, 1)*sizeof(float)*(views[i].dmap ? 2 : 1)));
-	}
-	float4* plane = ctx->plane.as<float4>();
-	float* cost = ctx->cost.as<float>();
-	uint32_t* best = ctx->best.as<uint32_t>();
+	float4* plane = S.plane;
+	float* cost = S.cost;
+	uint32_t* best = S.best;
 	int lowW = 0, lowH = 0;
 	for (int sc = totalScale; sc >= 0; --sc) {
 		// ScaleDepthData (SceneDensify.cpp:578-601): INTER_AREA images, rescaled K
@@ -289,7 +325,7 @@ int estimate_on_device(b200mvs_ctx* ctx, const DView* views, int nViews, float d
 				const int dw = level_size(views[i].w, sc), dh = level_size(views[i].h, sc);
 				if (dw < 2*PM_HALF+2 || dh < 2*PM_HALF+2)
 					return fail(ctx, B200MVS_ERR_ARG, "image too small for nSubResolutionLevels");
-				float* im = ctx->pyr[i].as<float>();   // sized for level 1 above, the largest
+				float* im = S.pyr[i];
 				CK(rs_launch_area(views[i].img, views[i].w, views[i].h, views[i].pitch, im, dw, dh, inv, inv, s)); ++ctx->launches;
 				lv[i].img = im; lv[i].w = dw; lv[i].h = dh; lv[i].pitch = dw;
 				scaleK(views[i].K, views[i].w, views[i].h, dw, dh, lv[i].K);
@@ -302,22 +338,20 @@ int estimate_on_device(b200mvs_ctx* ctx, const DView* views, int nViews, float d
 			}
 		}
 		const int w = lv[0].w, h = lv[0].h;
-		{ const int rc = prepare_ref_tmap(ctx, lv[0], s); if (rc) return rc; }
+		{ const int rc = prepare_ref_tmap(ctx, lv[0], S.refPad, s); if (rc) return rc; }
 		const float* lowres = nullptr;
 		if (sc != totalScale) {
 			// depth LINEAR / normal NEAREST up-sampling of the coarser level; the up-sampled
 			// depth is also the prior of this level (SceneDensify.cpp:660-664)
-			CK(rs_launch_plane_up(ctx->lowPlane.as<float4>(), lowW, lowH, plane, ctx->prior.as<float>(), w, h, ctx->mask != nullptr, s)); ++ctx->launches;
-			lowres = ctx->prior.as<float>();
+			CK(rs_launch_plane_up(S.lowPlane, lowW, lowH, plane, S.prior, w, h, ctx->mask != nullptr, s)); ++ctx->launches;
+			lowres = S.prior;
 		} else if (sc == 0) {
 			CK(pm_launch_pack((int)P0, d_depth, d_normal, plane, s)); ++ctx->launches;
 		} else {
 			// coarsest level: the caller's initial estimate, NEAREST down-sampled
-			CK(ctx->dDepth.reserve((size_t)w*h*sizeof(float)));
-			CK(ctx->dNormal.reserve((size_t)w*h*3*sizeof(float)));
-			CK(rs_launch_nearest(d_depth, W, H, 1, ctx->dDepth.as<float>(), w, h, (double)(1<<sc), (double)(1<<sc), s));
-			CK(rs_launch_nearest(d_normal, W, H, 3, ctx->dNormal.as<float>(), w, h, (double)(1<<sc), (double)(1<<sc), s));
-			CK(pm_launch_pack(w*h, ctx->dDepth.as<float>(), ctx->dNormal.as<float>(), plane, s)); ctx->launches += 3;
+			CK(rs_launch_nearest(d_depth, W, H, 1, S.dDepth, w, h, (double)(1<<sc), (double)(1<<sc), s));
+			CK(rs_launch_nearest(d_normal, W, H, 3, S.dNormal, w, h, (double)(1<<sc), (double)(1<<sc), s));
+			CK(pm_launch_pack(w*h, S.dDepth, S.dNormal, plane, s)); ctx->launches += 3;
 		}
 		PMParams P; bool geom;
 		build_params(o, lv.data(), nViews, dMin, dMax, lowres, plane, cost, best, P, geom);
@@ -326,8 +360,8 @@ int estimate_on_device(b200mvs_ctx* ctx, const DView* views, int nViews, float d
 		if (ctx->mask) {
 			// the mask of this level: cv::resize(..., INTER_NEAREST) of the full-resolution mask (DepthMap.cpp:309)
 			if (sc > 0) {
-				CK(rs_launch_nearest_u8(ctx->mask, W, H, ctx->maskPitch, ctx->maskLevel.as<uint8_t>(), w, h, s)); ++ctx->launches;
-				P.mask = ctx->maskLevel.as<uint8_t>(); P.maskPitch = w;
+				CK(rs_launch_nearest_u8(ctx->mask, W, H, ctx->maskPitch, S.maskLevel, w, h, s)); ++ctx->launches;
+				P.mask = S.maskLevel; P.maskPitch = w;
 			} else { P.mask = ctx->mask; P.maskPitch = ctx->maskPitch; }
 		}
 		CK(pm_launch_score(P, geom, s)); ++ctx->launches;
@@ -339,7 +373,7 @@ int estimate_on_device(b200mvs_ctx* ctx, const DView* views, int nViews, float d
 			}
 		}
 		if (sc > 0) {
-			CK(cudaMemcpyAsync(ctx->lowPlane.p, plane, (size_t)w*h*sizeof(float4), cudaMemcpyDeviceToDevice, s));
+			CK(cudaMemcpyAsync(S.lowPlane, plane, (size_t)w*h*sizeof(float4), cudaMemcpyDeviceToDevice, s));
 			lowW = w; lowH = h;
 		}
 	}
@@ -389,14 +423,16 @@ int b200mvs_estimate_device(b200mvs_ctx* ctx, const b200mvs_view* views, int nVi
 	if (rc) return rc;
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t s = stream_of(ctx, stream);
+	PMScratch S;
+	if ((rc = carve_estimate(ctx, views, nViews, nGeometricIter, S))) return rc;
 	std::vector<DView> dv;
 	ctx->launches = 0;
-	rc = stage_views(ctx, views, nViews, s, dv);
+	rc = stage_views(ctx, views, nViews, S.gray, s, dv);
 	if (rc) return rc;
 	const auto t0 = std::chrono::steady_clock::now();
 	ctx->nSweepEv = 0; ctx->timeSweeps = stats != nullptr;
 	if (stats) CK(cudaEventRecord(ctx->ev0, s));
-	rc = estimate_on_device(ctx, dv.data(), nViews, dMin, dMax, nGeometricIter, depth, normal, conf, (uint32_t*)viewsMap, s);
+	rc = estimate_on_device(ctx, dv.data(), nViews, dMin, dMax, nGeometricIter, S, depth, normal, conf, (uint32_t*)viewsMap, s);
 	if (rc) return rc;
 	if (stats) {
 		CK(cudaEventRecord(ctx->ev1, s));
@@ -426,13 +462,15 @@ int b200mvs_estimate_async(b200mvs_ctx* ctx, const b200mvs_view* views, int nVie
 	call.inout(dD, depth, P0*sizeof(float)); call.inout(dN, normal, P0*3*sizeof(float)); call.out(dC, conf, P0*sizeof(float));
 	if (viewsMap) call.out(dV, viewsMap, P0*sizeof(uint32_t));
 	if ((rc = call.stage())) return rc;
+	PMScratch S;
+	if ((rc = carve_estimate(ctx, dev.data(), nViews, nGeometricIter, S))) return rc;
 	std::vector<DView> dv;
 	ctx->launches = 0;
-	rc = stage_views(ctx, dev.data(), nViews, ctx->stream, dv);   // toGray runs before ev0, as in b200mvs_estimate_device
+	rc = stage_views(ctx, dev.data(), nViews, S.gray, ctx->stream, dv);   // toGray runs before ev0, as in b200mvs_estimate_device
 	if (rc) return rc;
 	ctx->nSweepEv = 0; ctx->timeSweeps = true;
 	return call.enqueue([&](cudaStream_t s) {
-		return estimate_on_device(ctx, dv.data(), nViews, dMin, dMax, nGeometricIter, dD, dN, dC, dV, s);
+		return estimate_on_device(ctx, dv.data(), nViews, dMin, dMax, nGeometricIter, S, dD, dN, dC, dV, s);
 	}, (nGeometricIter < 0 ? ctx->prm.nSubResolutionLevels : 0)+1);
 }
 
@@ -518,9 +556,15 @@ static int block_params(b200mvs_ctx* ctx, const b200mvs_view* views, int nViews,
 	for (int i = 0; i < nViews; ++i)
 		if (!views[i].image) return fail(ctx, B200MVS_ERR_ARG, "the building blocks take float gray images");
 	std::vector<DView> dv;
-	rc = stage_views(ctx, views, nViews, s, dv);
+	rc = stage_views(ctx, views, nViews, {}, s, dv);
 	if (rc) return rc;
-	if (tmap) { rc = prepare_ref_tmap(ctx, dv[0], s); if (rc) return rc; }
+	if (tmap) {
+		float* pad = nullptr;
+		Carve c(ctx->pmScratch);
+		if (size_t bytes = ref_pad_bytes(dv[0].img, (size_t)dv[0].pitch*4, dv[0].w, dv[0].h)) c.take(pad, bytes/sizeof(float));
+		CK(c.commit());
+		if ((rc = prepare_ref_tmap(ctx, dv[0], pad, s))) return rc;
+	}
 	build_params(ctx->prm, dv.data(), nViews, dMin, dMax, lowres, (float4*)plane4, cost, nullptr, P, geom);
 	return B200MVS_OK;
 }

@@ -50,7 +50,6 @@ int b200mvs_filter_depth_map_device(b200mvs_ctx* ctx, const b200mvs_dmap* ref, c
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t s = stream_of(ctx, stream);
 	const size_t np = (size_t)ref->width*ref->height;
-	CK(ctx->fltZ.reserve(np*8*(size_t)nNbrs));
 	FltParams P;
 	memset(&P, 0, sizeof(P));
 	flt_view(*ref, ref->depth, ref->conf, P.ref);
@@ -62,7 +61,10 @@ int b200mvs_filter_depth_map_device(b200mvs_ctx* ctx, const b200mvs_dmap* ref, c
 	P.N = nNbrs; P.nMinViews = prm->nMinViews; P.nMinViewsAdjust = prm->nMinViewsAdjust;
 	P.thDepthDiff = prm->fDepthDiffThreshold*1.2f; P.thStrict = prm->fDepthDiffThreshold*0.8f;
 	P.dMin = dMin; P.dMax = dMax;
-	P.zbuf = ctx->fltZ.as<unsigned long long>(); P.outDepth = outDepth; P.outConf = outConf;
+	Carve scratch(ctx->ppScratch);
+	scratch.take(P.zbuf, np*nNbrs);   // z-buffer keys
+	CK(scratch.commit());
+	P.outDepth = outDepth; P.outConf = outConf;
 	CK(flt_launch_filter(P, maxPix, prm->bAdjust != 0, s));
 	ctx->launches = 2;
 	if (projDepth) {
@@ -109,12 +111,16 @@ int b200mvs_remove_small_segments_device(b200mvs_ctx* ctx, float* depth, float* 
 	cudaStream_t s = stream_of(ctx, stream);
 	const float th = fDepthDiffThreshold*0.7f;
 	const int cap = 1<<18;   // one-way edges kept (a 1080p map has tens); beyond it the call fails loudly
-	CK(ctx->ppA.reserve(n*4)); CK(ctx->ppB.reserve(n*4)); CK(ctx->ppK.reserve(n*4));
-	CK(ctx->ppArcs.reserve(sizeof(int)*4 + (size_t)cap*sizeof(SegArc)));
-	int* count = ctx->ppArcs.as<int>();
-	SegArc* arcs = (SegArc*)(ctx->ppArcs.as<int>()+4);
+	// labels, segment sizes, seed keys, the one-way edges and the patched segment sizes: (label, size) of each of the at most
+	// 2 cap components the edges touch
+	Carve scratch(ctx->ppScratch);
+	int *labels, *sizes, *keys, *patched; SegArc* arcs;
+	scratch.take(labels, n); scratch.take(sizes, n); scratch.take(keys, n); scratch.take(arcs, cap); scratch.take(patched, 4*(size_t)cap);
+	CK(scratch.commit());
+	ReadBack* rb; CK(read_back(ctx, rb));
+	int* count = &rb->nArcs;
 	int launches = 0;
-	CK(seg_launch_label(depth, width, height, th, ctx->ppA.as<int>(), ctx->ppB.as<int>(), ctx->ppK.as<int>(), arcs, count, cap, launches, s));
+	CK(seg_launch_label(depth, width, height, th, labels, sizes, keys, arcs, count, cap, launches, s));
 	// the condensed graph is resolved on the host: one small read-back (the call synchronises the stream)
 	int nArcs = 0;
 	CK(cudaMemcpyAsync(&nArcs, count, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -152,12 +158,10 @@ int b200mvs_remove_small_segments_device(b200mvs_ctx* ctx, float* depth, float* 
 			for (int u: members) { patch.push_back(nodes[u].label); patch.push_back((int)std::min<long long>(total, 0x7FFFFFFF)); }
 		}
 		nPatch = (int)patch.size()/2;
-		CK(ctx->ppPatch.reserve(patch.size()*sizeof(int)));
-		CK(cudaMemcpyAsync(ctx->ppPatch.p, patch.data(), patch.size()*sizeof(int), cudaMemcpyHostToDevice, s));
+		CK(cudaMemcpyAsync(patched, patch.data(), patch.size()*sizeof(int), cudaMemcpyHostToDevice, s));
 		CK(cudaStreamSynchronize(s)); // `patch` is a local
 	}
-	CK(seg_launch_remove(depth, normal, conf, width, height, nSpeckleSize, ctx->ppA.as<int>(), ctx->ppB.as<int>(), ctx->ppPatch.as<int>(), nPatch,
-		launches, s));
+	CK(seg_launch_remove(depth, normal, conf, width, height, nSpeckleSize, labels, sizes, patched, nPatch, launches, s));
 	ctx->launches = launches;
 	return B200MVS_OK;
 }
@@ -170,10 +174,12 @@ int b200mvs_gap_interpolation_device(b200mvs_ctx* ctx, float* depth, float* norm
 		return fail(ctx, B200MVS_ERR_ARG, "gap_interpolation: invalid argument");
 	CK(cudaSetDevice(ctx->device));
 	const size_t n = (size_t)width*height;
-	CK(ctx->ppA.reserve(n*4)); CK(ctx->ppB.reserve(n*4)); CK(ctx->ppN.reserve(n*12));
+	Carve scratch(ctx->ppScratch);
+	float *tDepth, *tNormal, *tConf;
+	scratch.take(tDepth, n); scratch.take(tNormal, 3*n); scratch.take(tConf, n);
+	CK(scratch.commit());
 	const int gap = (int)std::min<unsigned>(nIpolGapSize, (unsigned)std::max(width, height));
-	CK(gap_launch(depth, normal, conf, ctx->ppA.as<float>(), ctx->ppN.as<float>(), ctx->ppB.as<float>(), width, height,
-		fDepthDiffThreshold*2.5f, gap, stream_of(ctx, stream)));
+	CK(gap_launch(depth, normal, conf, tDepth, tNormal, tConf, width, height, fDepthDiffThreshold*2.5f, gap, stream_of(ctx, stream)));
 	ctx->launches = 2;
 	return B200MVS_OK;
 }

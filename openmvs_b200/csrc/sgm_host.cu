@@ -6,22 +6,28 @@
 
 namespace {
 
+// One wave-front aggregation: the shape of its schedule (sgm_front_schedule) and the scratch of its launches, carved by the match
+struct FrontRun {
+	int layout, FB, maxPaths, maxCtl;
+	int* ctl; uint16_t* state; float2* meta;   // [ticket, error, -, - | progress | cellDone] (4+maxCtl ints), path state, path meta
+};
+
 // SGM path aggregation with the wave-front kernel (sgm_front.cu).  Pass layouts (b200mvs_debug.frontLayout, 0 = auto = 1):
 //   1 two tilted fronts f = +-(x + 2y): {right, right-down, down, left-down} and {left, left-up, up, right-up};
 //   2 four straight fronts: top-down {down, right-down, left-down}, bottom-up {up, right-up, left-up}, left-right, right-left;
 //   3 eight passes of one direction each (the traffic of the per-direction kernels with the new step).
-// With a `second` volume, consecutive passes share a launch: pass 2j accumulates into the caller's volume, pass 2j+1 into
-// `second`, and the caller adds the two (the winner-takes-all kernel does).  Without one, every pass has a launch of its own.
-int sgm_aggregate_fronts(b200mvs_ctx* ctx, const SGMParams& P, int num, uint16_t* second, cudaStream_t s) {
+// With a `second` volume (`concurrent`), consecutive passes share a launch: pass 2j accumulates into the caller's volume, pass
+// 2j+1 into `second`, and the caller adds the two (the winner-takes-all kernel does).  Without one, every pass has a launch of
+// its own.  sgm_front_schedule brings the context's cached schedule (ctx->sgFront) to this size and layout; sgm_aggregate_fronts
+// launches it.
+int sgm_front_schedule(b200mvs_ctx* ctx, int vw, int vh, int num, bool concurrent, cudaStream_t s, FrontRun& F) {
 	const b200mvs_debug& D = ctx->dbg;
 	const int layout = std::min(std::max(D.frontLayout-1, 0), 2);
-	const bool concurrent = second != nullptr;
 	const int FB = D.frontBlock > 0 ? D.frontBlock : 32;   // fronts per block: larger blocks widen the window of the sum volume kept in the L2
 	// frontLag = lag + 1.  The sub-cell dependencies make every lag legal.  A larger lag lets more blocks be in flight at once, but
 	// the window of blocks between a block's first and last phase then outgrows the L2 and the sums go to DRAM and back; lag 0
 	// leaves the resident warps all holding items of one block, waiting for each other.  Default: lag 1.
 	const int lag = D.frontLag > 0 ? D.frontLag-1 : 1;
-	const int vw = P.vw, vh = P.vh;
 	// sub-cell width: one lane polls one counter, and a band at an image corner can span the whole width: at most 30 sub-cell columns
 	const int SW = std::max(D.frontSubCell >= 16 ? D.frontSubCell : FRONT_SW, (vw+29)/30);
 	const int key[6] = {vw, vh, layout, FB, lag | (SW<<8), concurrent ? 2 : 1};
@@ -43,19 +49,21 @@ int sgm_aggregate_fronts(b200mvs_ctx* ctx, const SGMParams& P, int num, uint16_t
 		CK(cudaStreamSynchronize(s)); // the pageable source vectors die with `plan`
 		memcpy(ctx->sgFrontKey, key, sizeof(key));
 	}
-	const int maxPaths = vw+vh+8;
-	int maxCtl = 0;
-	for (auto& fp: ctx->sgFront) maxCtl = std::max(maxCtl, fp.launch.nChains + fp.launch.nCells);
-	CK(ctx->sgFrontCtl.reserve((size_t)(4+maxCtl)*sizeof(int)));
-	CK(ctx->sgFrontState.reserve((size_t)8*maxPaths*num*sizeof(uint16_t)));
-	CK(ctx->sgFrontMeta.reserve((size_t)8*maxPaths*sizeof(float2)));
-	int* ctl = ctx->sgFrontCtl.as<int>();
+	F.layout = layout; F.FB = FB; F.maxPaths = vw+vh+8; F.maxCtl = 0;
+	for (auto& fp: ctx->sgFront) F.maxCtl = std::max(F.maxCtl, fp.launch.nChains + fp.launch.nCells);
+	return B200MVS_OK;
+}
+
+int sgm_aggregate_fronts(b200mvs_ctx* ctx, const SGMParams& P, int num, uint16_t* second, const FrontRun& F, cudaStream_t s) {
+	const b200mvs_debug& D = ctx->dbg;
+	const int maxCtl = F.maxCtl;
+	int* ctl = F.ctl;
 	// resident CTAs: the queue needs no particular number; frontCtas = CTAs per SM, frontDepth = ring slots per warp (8 default, 4)
 	const int pd = D.frontDepth == 4 ? 4 : 8;
 	int sms = 0; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device));
 	const int perSm = std::min(sgm_front_blocks_per_sm(num, pd), D.frontCtas > 0 ? D.frontCtas : 2);
 	const int blocks = sms*perSm;
-	const int FBeff = layout == 2 ? (1<<28) : FB;
+	const int FBeff = F.layout == 2 ? (1<<28) : F.FB;
 	for (size_t i = 0; i < ctx->sgFront.size(); ++i) {
 		b200mvs_ctx::FrontPass& fp = ctx->sgFront[i];
 		const FrontLaunch& L = fp.launch;
@@ -65,7 +73,7 @@ int sgm_aggregate_fronts(b200mvs_ctx* ctx, const SGMParams& P, int num, uint16_t
 		FrontArgs A; memset(&A, 0, sizeof(A));
 		A.items = fp.items.as<FrontItem>(); A.nItems = fp.nItems;
 		A.ticket = ctl; A.error = ctl+1; A.progress = ctl+4; A.cellDone = ctl+4+L.nChains; A.cellNeed = fp.need.as<int>();
-		A.state = ctx->sgFrontState.as<uint16_t>(); A.meta = ctx->sgFrontMeta.as<float2>(); A.maxPaths = maxPaths;
+		A.state = F.state; A.meta = F.meta; A.maxPaths = F.maxPaths;
 		A.FB = FBeff; A.num = num;
 		for (int p = 0; p < L.nPasses; ++p) {
 			A.fa[p] = L.pass[p].fa; A.fb[p] = L.pass[p].fb; A.fc[p] = L.fc[p];
@@ -144,18 +152,15 @@ int b200mvs_sgm_match_device(b200mvs_ctx* ctx, const float* leftGray, const uint
 	}
 	if (prm->P1 < 0 || prm->P1 > minP2)
 		return fail(ctx, B200MVS_ERR_ARG, "sgm: needs 0 <= P1 <= min(P2s)");
-	if (!costs) { CK(ctx->sgCosts.reserve(numCosts)); costs = ctx->sgCosts.as<uint8_t>(); }
-	if (!accums) { CK(ctx->sgAccums.reserve(numCosts*sizeof(uint16_t))); accums = ctx->sgAccums.as<uint16_t>(); }
-	P.costs = costs; P.accums = accums;
 	const auto t0 = std::chrono::steady_clock::now();
 	ctx->launches = 0;
 	SGMMapStats st = {};
 	SGMPlan plan = {};
 	if (stats) CK(cudaEventRecord(ctx->ev0, s));
 	if (stages & 7) {
-		CK(ctx->sgMax.reserve(sizeof(SGMMapStats)));
-		CK(sgm_launch_map_stats(P.px, P.vw*P.vh, numCosts, ctx->sgMax.as<SGMMapStats>(), s)); ctx->launches += 2;
-		CK(cudaMemcpyAsync(&st, ctx->sgMax.p, sizeof(st), cudaMemcpyDeviceToHost, s));
+		ReadBack* rb; CK(read_back(ctx, rb));
+		CK(sgm_launch_map_stats(P.px, P.vw*P.vh, numCosts, &rb->mapStats, s)); ctx->launches += 2;
+		CK(cudaMemcpyAsync(&st, &rb->mapStats, sizeof(st), cudaMemcpyDeviceToHost, s));
 		CK(cudaStreamSynchronize(s));
 		if (st.overflow)
 			return fail(ctx, B200MVS_ERR_ARG, "sgm: a pixel's slice [idx, idx+dmax-dmin) ends beyond numCosts");
@@ -163,33 +168,45 @@ int b200mvs_sgm_match_device(b200mvs_ctx* ctx, const float* leftGray, const uint
 		if (st.maxNum > SGM_MAX_DISP)
 			return fail(ctx, B200MVS_ERR_ARG, "sgm: more than 256 disparities per pixel");
 		P.maxNumDisp = st.maxNum;
-		plan = sgm_plan(st, ctx->dbg, !((uintptr_t)P.costs & 15), !((uintptr_t)P.accums & 15), maxP2, numCosts);
+		// a volume the caller does not pass (null here) is carved below, 256-byte aligned
+		plan = sgm_plan(st, ctx->dbg, !((uintptr_t)costs & 15), !((uintptr_t)accums & 15), maxP2, numCosts);
 		if (ctx->dbg.sgmAggregation == 4 && plan.agg != SGMPlan::FRONTS)
 			return fail(ctx, B200MVS_ERR_ARG, "sgm: the wave-front kernel needs a dense volume with one range of 64, 128 or 256 disparities");
 	}
+	// the sum volumes the winner-takes-all adds: accums, then nVol-1 more at `more`
+	const int nVol = (stages & 2) ? plan.volumes : 1;
+	const bool fronts = (stages & 2) && plan.agg == SGMPlan::FRONTS, streams = (stages & 2) && plan.agg == SGMPlan::RAGGED_STREAMS;
+	FrontRun F = {};
+	if (fronts) { const int rc = sgm_front_schedule(ctx, P.vw, P.vh, st.maxNum, nVol == 2, s, F); if (rc) return rc; }
+	// the match's scratch: the volumes the caller does not pass, the second sum volume(s) and the wave-front state
+	Carve scratch(ctx->sgmScratch);
+	const bool ownAccums = !accums;
+	if (ownAccums) scratch.take(accums, numCosts);
+	if (!costs) scratch.take(costs, numCosts);
+	uint16_t* more = nullptr;
+	if (fronts && nVol == 2) scratch.take(more, (size_t)P.vw*P.vh*st.maxNum);
+	if (streams) scratch.take(more, (size_t)7*numCosts);
+	if (fronts) { scratch.take(F.ctl, 4+F.maxCtl); scratch.take(F.state, (size_t)8*F.maxPaths*st.maxNum); scratch.take(F.meta, 8*F.maxPaths); }
+	CK(scratch.commit());
+	P.costs = costs; P.accums = accums;
+	// b200mvs_sgm_refine_device(accums = NULL) reads the last match's own sum volume, for the pixel map it aggregated
+	if (ownAccums) ctx->sgLastAccums = accums;
+	else if (!scratch.empty()) { ctx->sgLastAccums = nullptr; ctx->sgLastPx = nullptr; }   // the carve may have moved them
+	if (stages & 2) ctx->sgLastPx = ownAccums ? (const void*)pixels : nullptr;
 	if (stages & 1) {
 		if (ctx->dbg.sgmCost == 2 && !plan.tcCost)
 			return fail(ctx, B200MVS_ERR_ARG, "sgm: the tensor-core cost kernel needs a dense volume with one range of 64, 128, 192 or 256 disparities");
 		if (plan.tcCost) { CK(sgm_cost_tc_launch(P, st.dminLo, st.maxNum, s)); ctx->launches += (st.maxNum+127)/128; }
 		else { CK(sgm_launch_cost(P, s)); ++ctx->launches; }
 	}
-	// the sum volumes the winner-takes-all adds: accums, then nVol-1 more at `more` (ctx->sgAccums2)
-	const int nVol = (stages & 2) ? plan.volumes : 1;
-	uint16_t* more = nullptr;
-	if ((stages & 2) && plan.agg == SGMPlan::FRONTS) {
-		if (nVol == 2) {
-			CK(ctx->sgAccums2.reserve((size_t)P.vw*P.vh*st.maxNum*sizeof(uint16_t)));
-			more = ctx->sgAccums2.as<uint16_t>();
-		}
-		const int rc = sgm_aggregate_fronts(ctx, P, st.maxNum, more, s);
+	if (fronts) {
+		const int rc = sgm_aggregate_fronts(ctx, P, st.maxNum, more, F, s);
 		if (rc) return rc;
 	} else
-	if ((stages & 2) && plan.agg == SGMPlan::RAGGED_STREAMS) {
+	if (streams) {
 		// ragged (tSGM) ranges: a direction has only 1000-3000 scanlines, one warp each — far too few to fill the GPU.  The eight
 		// directions run side by side on eight streams, each STORING its path costs into a volume of its own (no memset, no
 		// read-modify-write, no races); the winner-takes-all kernel adds the volumes.
-		CK(ctx->sgAccums2.reserve((size_t)7*numCosts*sizeof(uint16_t)));
-		more = ctx->sgAccums2.as<uint16_t>();
 		if (!ctx->sgSide[0]) {
 			for (int i = 0; i < 7; ++i) { CK(cudaStreamCreateWithFlags(&ctx->sgSide[i], cudaStreamNonBlocking)); CK(cudaEventCreateWithFlags(&ctx->sgJoin[i], cudaEventDisableTiming)); }
 			CK(cudaEventCreateWithFlags(&ctx->sgFork, cudaEventDisableTiming));
@@ -216,7 +233,6 @@ int b200mvs_sgm_match_device(b200mvs_ctx* ctx, const float* leftGray, const uint
 			++ctx->launches;
 		}
 	}
-	if (stages & 2) ctx->sgLastPx = (accums == ctx->sgAccums.as<uint16_t>()) ? (const void*)pixels : nullptr;
 	// the winner-takes-all; without stage 4, several volumes are still added into accums (no disparity / cost maps)
 	if ((stages & 4) || nVol > 1) {
 		int16_t* d = (stages & 4) ? disparity : nullptr;
@@ -230,10 +246,10 @@ int b200mvs_sgm_match_device(b200mvs_ctx* ctx, const float* leftGray, const uint
 		CK(cudaStreamSynchronize(s));
 		const int rc = fill_stats(ctx, stats, t0, 1);
 		if (rc) return rc;
-		if ((stages & 2) && plan.agg == SGMPlan::FRONTS) {
+		if (fronts) {
 			// the wave-front kernel flags a dependency wait that timed out (never in a correct schedule): the stream is idle here
 			int err = 0;
-			CK(cudaMemcpy(&err, ctx->sgFrontCtl.as<int>()+1, sizeof(int), cudaMemcpyDeviceToHost));
+			CK(cudaMemcpy(&err, F.ctl+1, sizeof(int), cudaMemcpyDeviceToHost));
 			if (err) return fail(ctx, B200MVS_ERR_CUDA, "sgm: the wave-front aggregation timed out waiting for a predecessor");
 		}
 	}
@@ -276,7 +292,7 @@ int b200mvs_sgm_refine_device(b200mvs_ctx* ctx, const b200mvs_sgm_pixel* pixels,
 	if (!ctx || !pixels || !disparity || nPixels <= 0) return B200MVS_ERR_ARG;
 	if (!accums) {
 		// the accumulated costs of the last match on this context: only valid for the pixel map they were computed for
-		accums = ctx->sgAccums.as<uint16_t>();
+		accums = ctx->sgLastAccums;
 		if (!accums || ctx->sgLastPx != (const void*)pixels)
 			return fail(ctx, B200MVS_ERR_ARG, "sgm refine: no accumulated costs of a match with this pixel map on the context");
 	}
@@ -326,16 +342,15 @@ int b200mvs_sgm_levels(int width, int height, int minResolution, int* numLevels,
 	return B200MVS_OK;
 }
 
+// Disparity2RangeMap of a width x height map onto the mw x mh grid.  ranges: width x height, scan: tsgm_range_map_scratch(mw x mh)
+// bytes, from the caller's carve.
 static int tsgm_range_map(b200mvs_ctx* ctx, const int16_t* disparity, int width, int height, const uint8_t* mask, int mw, int mh,
-	int minNumDisp, int minNumDispInvalid, b200mvs_sgm_pixel* pixels, uint64_t* numCosts, cudaStream_t s)
+	int minNumDisp, int minNumDispInvalid, short2* ranges, uint8_t* scan, b200mvs_sgm_pixel* pixels, uint64_t* numCosts, cudaStream_t s)
 {
-	const size_t n2 = (size_t)mw*mh;
-	CK(ctx->ts[b200mvs_ctx::TS_RANGES].reserve((size_t)width*height*sizeof(short2)));
-	CK(ctx->ts[b200mvs_ctx::TS_SCAN].reserve(tsgm_range_map_scratch(n2)));
-	CK(ctx->ts[b200mvs_ctx::TS_SMALL].reserve(64));
-	unsigned long long* total = ctx->ts[b200mvs_ctx::TS_SMALL].as<unsigned long long>();
-	CK(tsgm_launch_range_map(disparity, width, height, mask, mw, mh, minNumDisp, minNumDispInvalid,
-		ctx->ts[b200mvs_ctx::TS_RANGES].as<short2>(), (SGMPixel*)pixels, ctx->ts[b200mvs_ctx::TS_SCAN].p, total, s));
+	ReadBack* rb; CK(read_back(ctx, rb));
+	unsigned long long* total = &rb->rangeTotal;
+	CK(tsgm_launch_range_map(disparity, width, height, mask, mw, mh, minNumDisp, minNumDispInvalid, ranges, (SGMPixel*)pixels, scan,
+		total, s));
 	// the size of the volume: one 8-byte read per pixel map (the match that follows sizes its scratch with it)
 	unsigned long long num = 0;
 	CK(cudaMemcpyAsync(&num, total, sizeof(num), cudaMemcpyDeviceToHost, s));
@@ -353,8 +368,12 @@ int b200mvs_sgm_range_map_device(b200mvs_ctx* ctx, const int16_t* disparity, int
 	if (maskWidth <= 2*width+3 || maskHeight <= 2*height+1 || (size_t)maskWidth*maskHeight >= (1u<<31))
 		return fail(ctx, B200MVS_ERR_ARG, "range map: the 2x grid must extend beyond (2 width + 3, 2 height + 1)");
 	CK(cudaSetDevice(ctx->device));
-	return tsgm_range_map(ctx, disparity, width, height, mask, maskWidth, maskHeight, minNumDisp, minNumDispInvalid, pixels, numCosts,
-		stream_of(ctx, stream));
+	Carve scratch(ctx->tsgmScratch);
+	short2* ranges; uint8_t* scan;
+	scratch.take(ranges, (size_t)width*height); scratch.take(scan, tsgm_range_map_scratch((size_t)maskWidth*maskHeight));
+	CK(scratch.commit());
+	return tsgm_range_map(ctx, disparity, width, height, mask, maskWidth, maskHeight, minNumDisp, minNumDispInvalid, ranges, scan,
+		pixels, numCosts, stream_of(ctx, stream));
 }
 
 int b200mvs_sgm_flip_direction_device(b200mvs_ctx* ctx, const int16_t* l2r, int16_t* r2l, int width, int height, void* stream) {
@@ -362,8 +381,11 @@ int b200mvs_sgm_flip_direction_device(b200mvs_ctx* ctx, const int16_t* l2r, int1
 	if (!l2r || !r2l || l2r == r2l || width <= 0 || height <= 0 || width >= 65535)
 		return fail(ctx, B200MVS_ERR_ARG, "flip direction: null or aliased maps, or a width outside [1, 65534]");
 	CK(cudaSetDevice(ctx->device));
-	CK(ctx->ts[b200mvs_ctx::TS_KEYS].reserve((size_t)width*height*sizeof(unsigned)));
-	CK(tsgm_launch_flip(l2r, r2l, width, height, ctx->ts[b200mvs_ctx::TS_KEYS].as<unsigned>(), stream_of(ctx, stream)));
+	Carve scratch(ctx->tsgmScratch);
+	unsigned* keys;
+	scratch.take(keys, (size_t)width*height);
+	CK(scratch.commit());
+	CK(tsgm_launch_flip(l2r, r2l, width, height, keys, stream_of(ctx, stream)));
 	return B200MVS_OK;
 }
 
@@ -393,9 +415,11 @@ int b200mvs_sgm_filter_speckles_device(b200mvs_ctx* ctx, int16_t* disparity, int
 		return fail(ctx, B200MVS_ERR_ARG, "filter speckles: null map, bad size or negative limits");
 	CK(cudaSetDevice(ctx->device));
 	const size_t n = (size_t)width*height;
-	CK(ctx->ts[b200mvs_ctx::TS_LABELS].reserve(n*sizeof(int))); CK(ctx->ts[b200mvs_ctx::TS_SIZES].reserve(n*sizeof(int)));
-	CK(tsgm_launch_speckles(disparity, width, height, newVal, maxSpeckleSize, maxDiff, ctx->ts[b200mvs_ctx::TS_LABELS].as<int>(),
-		ctx->ts[b200mvs_ctx::TS_SIZES].as<int>(), stream_of(ctx, stream)));
+	Carve scratch(ctx->tsgmScratch);
+	int *labels, *sizes;
+	scratch.take(labels, n); scratch.take(sizes, n);
+	CK(scratch.commit());
+	CK(tsgm_launch_speckles(disparity, width, height, newVal, maxSpeckleSize, maxDiff, labels, sizes, stream_of(ctx, stream)));
 	return B200MVS_OK;
 }
 
@@ -410,11 +434,12 @@ int b200mvs_resize_area_u8_device(b200mvs_ctx* ctx, const uint8_t* src, int widt
 	return B200MVS_OK;
 }
 
-static int tsgm_level_mask(b200mvs_ctx* ctx, const uint8_t* mask, int width, int height, int lw, int lh, uint8_t* valid, cudaStream_t s) {
-	DevBuf& t = ctx->ts[b200mvs_ctx::TS_MASKT];
-	CK(t.reserve((size_t)lw*lh));
-	CK(rs_launch_nearest_u8(mask, width, height, width, t.as<uint8_t>(), lw, lh, s));
-	CK(cudaMemcpy2DAsync(valid, lw-6, t.as<uint8_t>()+3*lw+3, lw, lw-6, lh-6, cudaMemcpyDeviceToDevice, s));
+// the mask of an lw x lh level, cropped to its valid region; t: lw x lh bytes from the caller's carve
+static int tsgm_level_mask(b200mvs_ctx* ctx, const uint8_t* mask, int width, int height, int lw, int lh, uint8_t* t, uint8_t* valid,
+	cudaStream_t s)
+{
+	CK(rs_launch_nearest_u8(mask, width, height, width, t, lw, lh, s));
+	CK(cudaMemcpy2DAsync(valid, lw-6, t+3*lw+3, lw, lw-6, lh-6, cudaMemcpyDeviceToDevice, s));
 	return B200MVS_OK;
 }
 
@@ -425,7 +450,11 @@ int b200mvs_sgm_level_mask_device(b200mvs_ctx* ctx, const uint8_t* mask, int wid
 	if (!mask || !validMask || width <= 0 || height <= 0 || levelWidth <= 6 || levelHeight <= 6)
 		return fail(ctx, B200MVS_ERR_ARG, "level mask: null pointer or a level of at most 6 pixels");
 	CK(cudaSetDevice(ctx->device));
-	return tsgm_level_mask(ctx, mask, width, height, levelWidth, levelHeight, validMask, stream_of(ctx, stream));
+	Carve scratch(ctx->tsgmScratch);
+	uint8_t* t;
+	scratch.take(t, (size_t)levelWidth*levelHeight);
+	CK(scratch.commit());
+	return tsgm_level_mask(ctx, mask, width, height, levelWidth, levelHeight, t, validMask, stream_of(ctx, stream));
 }
 
 int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
@@ -434,7 +463,6 @@ int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
 	int minResolution, int nSpeckleSize, int thCross, int subpixelSteps, const b200mvs_sgm_params* prm,
 	int16_t* outDisparity, uint16_t* outCost, uint64_t* numCostsPerLevel, void* stream)
 {
-	typedef b200mvs_ctx X;
 	if (!ctx) return B200MVS_ERR_ARG;
 	if (!leftGray || !leftBGR || !rightGray || !rightBGR || !outDisparity || !outCost)
 		return fail(ctx, B200MVS_ERR_ARG, "hierarchical sgm: null image or output map");
@@ -449,21 +477,20 @@ int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
 	cudaStream_t s = stream_of(ctx, stream);
 	const bool tsgm = minResolution > 0;
 	const size_t n = (size_t)width*height, nv = (size_t)(width-6)*(height-6);
-	// grow-only scratch, sized for the full-resolution level up front (nothing is reallocated while kernels use it)
+	// the scratch of every level, sized for the largest: the level images (gray, then BGR, of the left and the right image; the
+	// last level reads the caller's), the valid masks, the disparity maps of the previous level (dL / dR: pw x ph; first level:
+	// the initial map) and of this one (nL / nR), the pixel maps, and the Disparity2RangeMap / FlipDirection / speckle scratch
 	const size_t nImg = nl > 1 ? (size_t)lw[nl-2]*lh[nl-2] : 0;
-	CK(ctx->ts[X::TS_IMG].reserve(nImg*14+64));
-	CK(ctx->ts[X::TS_MASKL].reserve(nv)); CK(ctx->ts[X::TS_MASKR].reserve(nv)); CK(ctx->ts[X::TS_MASKT].reserve(n));
-	for (int b: {X::TS_DL, X::TS_DR, X::TS_DL0, X::TS_DR0}) CK(ctx->ts[b].reserve(nv*sizeof(int16_t)));
-	CK(ctx->ts[X::TS_PXL].reserve(nv*sizeof(SGMPixel))); CK(ctx->ts[X::TS_PXR].reserve(nv*sizeof(SGMPixel)));
-	CK(ctx->ts[X::TS_RANGES].reserve(nv*sizeof(short2))); CK(ctx->ts[X::TS_SCAN].reserve(tsgm_range_map_scratch(nv)));
-	CK(ctx->ts[X::TS_KEYS].reserve(nv*sizeof(unsigned))); CK(ctx->ts[X::TS_LABELS].reserve(nv*sizeof(int)));
-	CK(ctx->ts[X::TS_SIZES].reserve(nv*sizeof(int))); CK(ctx->ts[X::TS_SMALL].reserve(64));
-	uint8_t* maskL = ctx->ts[X::TS_MASKL].as<uint8_t>(); uint8_t* maskR = ctx->ts[X::TS_MASKR].as<uint8_t>();
-	uint8_t* maskT = ctx->ts[X::TS_MASKT].as<uint8_t>();
-	b200mvs_sgm_pixel* pxL = ctx->ts[X::TS_PXL].as<b200mvs_sgm_pixel>(); b200mvs_sgm_pixel* pxR = ctx->ts[X::TS_PXR].as<b200mvs_sgm_pixel>();
-	// dL / dR: the maps of the previous level (pw x ph; first level: the initial map), nL / nR: the maps of this level
-	int16_t *dL = ctx->ts[X::TS_DL0].as<int16_t>(), *dR = ctx->ts[X::TS_DR0].as<int16_t>();
-	int16_t *nL = ctx->ts[X::TS_DL].as<int16_t>(), *nR = ctx->ts[X::TS_DR].as<int16_t>();
+	Carve scratch(ctx->tsgmScratch);
+	float *grayL, *grayR; uint8_t *bgrL, *bgrR, *maskL, *maskR, *maskT, *scan;
+	int16_t *dL, *dR, *nL, *nR; b200mvs_sgm_pixel *pxL, *pxR; short2* ranges; unsigned* keys; int *labels, *sizes;
+	scratch.take(grayL, nImg); scratch.take(grayR, nImg); scratch.take(bgrL, 3*nImg); scratch.take(bgrR, 3*nImg);
+	scratch.take(maskL, nv); scratch.take(maskR, nv); scratch.take(maskT, n);
+	for (int16_t** d: {&dL, &dR, &nL, &nR}) scratch.take(*d, nv);
+	scratch.take(pxL, nv); scratch.take(pxR, nv);
+	scratch.take(ranges, nv); scratch.take(scan, tsgm_range_map_scratch(nv));
+	scratch.take(keys, nv); scratch.take(labels, nv); scratch.take(sizes, nv);
+	CK(scratch.commit());
 	int pw = iw, ph = ih;
 	if (initDisparity) CK(cudaMemcpyAsync(dL, initDisparity, (size_t)iw*ih*sizeof(int16_t), cudaMemcpyDeviceToDevice, s));
 	else CK(tsgm_launch_fill(dL, (size_t)iw*ih, (int16_t)SGM_NO_DISP, s));
@@ -471,7 +498,8 @@ int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
 	if (!tsgm) {
 		// the global range of the initial map (SemiGlobalMatcher.cpp:643-668) over its valid values
 		int mm[2] = {0, 0};
-		int* dmm = (int*)(ctx->ts[X::TS_SMALL].as<unsigned long long>()+1);
+		ReadBack* rb; CK(read_back(ctx, rb));
+		int* dmm = rb->minMax;
 		CK(tsgm_launch_minmax(dL, (size_t)iw*ih, dmm, s));
 		CK(cudaMemcpyAsync(mm, dmm, sizeof(mm), cudaMemcpyDeviceToHost, s));
 		CK(cudaStreamSynchronize(s));
@@ -499,19 +527,17 @@ int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
 		const float *lg = leftGray, *rg = rightGray; const uint8_t *lc = leftBGR, *rcol = rightBGR;
 		if (lev+1 < nl) {
 			const int f = 1 << (nl-1-lev);
-			const size_t m = (size_t)w*h;
-			float* g = (float*)ctx->ts[X::TS_IMG].p; uint8_t* c = (uint8_t*)(g+2*m);
-			CK(rs_launch_area(leftGray, width, height, width, g, w, h, f, f, s));
-			CK(rs_launch_area(rightGray, width, height, width, g+m, w, h, f, f, s));
-			CK(tsgm_launch_area_u8(leftBGR, width, height, 3, c, w, h, f, s));
-			CK(tsgm_launch_area_u8(rightBGR, width, height, 3, c+3*m, w, h, f, s));
-			lg = g; rg = g+m; lc = c; rcol = c+3*m;
+			CK(rs_launch_area(leftGray, width, height, width, grayL, w, h, f, f, s));
+			CK(rs_launch_area(rightGray, width, height, width, grayR, w, h, f, f, s));
+			CK(tsgm_launch_area_u8(leftBGR, width, height, 3, bgrL, w, h, f, s));
+			CK(tsgm_launch_area_u8(rightBGR, width, height, 3, bgrR, w, h, f, s));
+			lg = grayL; rg = grayR; lc = bgrL; rcol = bgrR;
 		}
 		if (first) {
 			// masks: NEAREST to the level size, cropped to the valid region (SemiGlobalMatcher.cpp:627-631)
-			if (leftMask) { if ((rc = tsgm_level_mask(ctx, leftMask, width, height, w, h, maskL, s))) return rc; }
+			if (leftMask) { if ((rc = tsgm_level_mask(ctx, leftMask, width, height, w, h, maskT, maskL, s))) return rc; }
 			else CK(cudaMemsetAsync(maskL, 0xFF, (size_t)vw*vh, s));
-			if (rightMask) { if ((rc = tsgm_level_mask(ctx, rightMask, width, height, w, h, maskR, s))) return rc; }
+			if (rightMask) { if ((rc = tsgm_level_mask(ctx, rightMask, width, height, w, h, maskT, maskR, s))) return rc; }
 			else CK(cudaMemsetAsync(maskR, 0xFF, (size_t)vw*vh, s));
 		} else {
 			for (uint8_t* m: {maskL, maskR}) {
@@ -521,15 +547,15 @@ int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
 		}
 		uint64_t numR = 0, numL = 0;
 		if (tsgm) {
-			CK(tsgm_launch_flip(dL, dR, pw, ph, ctx->ts[X::TS_KEYS].as<unsigned>(), s));
-			if ((rc = tsgm_range_map(ctx, dR, pw, ph, maskR, vw, vh, first ? 11 : 5, first ? 33 : 7, pxR, &numR, s))) return rc;
+			CK(tsgm_launch_flip(dL, dR, pw, ph, keys, s));
+			if ((rc = tsgm_range_map(ctx, dR, pw, ph, maskR, vw, vh, first ? 11 : 5, first ? 33 : 7, ranges, scan, pxR, &numR, s))) return rc;
 		} else {
 			numR = (uint64_t)nv*(uint64_t)(fixHi-fixLo);
 			CK(tsgm_launch_dense_map((SGMPixel*)pxR, nv, fixLo, fixHi, s));
 		}
 		if ((rc = match(rg, rcol, lg, w, h, pxR, numR, nR, outCost))) return rc;
 		if (tsgm) {
-			if ((rc = tsgm_range_map(ctx, dL, pw, ph, maskL, vw, vh, first ? 11 : 5, first ? 33 : 7, pxL, &numL, s))) return rc;
+			if ((rc = tsgm_range_map(ctx, dL, pw, ph, maskL, vw, vh, first ? 11 : 5, first ? 33 : 7, ranges, scan, pxL, &numL, s))) return rc;
 		} else {
 			numL = numR;
 			CK(tsgm_launch_dense_map((SGMPixel*)pxL, nv, -fixHi, -fixLo, s));
@@ -541,7 +567,7 @@ int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
 			CK(sgm_launch_cross_check(nL, nR, vw, vh, thCross, s));
 			CK(sgm_launch_cross_check(nR, nL, vw, vh, thCross, s));
 			for (int16_t* d: {nL, nR})
-				CK(tsgm_launch_speckles(d, vw, vh, SGM_NO_DISP, nSpeckleSize, 5, ctx->ts[X::TS_LABELS].as<int>(), ctx->ts[X::TS_SIZES].as<int>(), s));
+				CK(tsgm_launch_speckles(d, vw, vh, SGM_NO_DISP, nSpeckleSize, 5, labels, sizes, s));
 			CK(tsgm_launch_extract_mask(nL, maskL, vw, vh, 3, s));
 			CK(tsgm_launch_extract_mask(nR, maskR, vw, vh, 3, s));
 		} else {
@@ -551,10 +577,10 @@ int b200mvs_sgm_match_hierarchical_device(b200mvs_ctx* ctx,
 		pw = vw; ph = vh;
 	}
 	// RefineDisparityMap(left) with the accumulated costs of the last left match (SemiGlobalMatcher.cpp:718)
-	if (subpixelSteps > 1 && ctx->sgAccums.p)
-		CK(sgm_launch_refine((const SGMPixel*)pxL, ctx->sgAccums.as<uint16_t>(), dL, (int)nv, subpixelSteps, s));
+	if (subpixelSteps > 1 && ctx->sgLastAccums)
+		CK(sgm_launch_refine((const SGMPixel*)pxL, ctx->sgLastAccums, dL, (int)nv, subpixelSteps, s));
 	CK(cudaMemcpyAsync(outDisparity, dL, nv*sizeof(int16_t), cudaMemcpyDeviceToDevice, s));
-	// the pixel maps of the hierarchy are internal: no later refine call may take sgAccums for its own map
+	// the pixel maps of the hierarchy are internal: no later refine call may take the last match's sums for its own map
 	ctx->sgLastPx = nullptr;
 	CK(cudaStreamSynchronize(s));
 	return B200MVS_OK;
@@ -625,9 +651,12 @@ int b200mvs_sgm_project_disparity_device(b200mvs_ctx* ctx, const b200mvs_sgm_pai
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t s = stream_of(ctx, stream);
 	const size_t n = (size_t)width*height;
-	CK(ctx->sfKeys.reserve(4*n*sizeof(unsigned long long)));
-	CK(sgmf_launch_project(A, width, height, ctx->sfKeys.as<unsigned long long>(), s));
-	CK(sgmf_launch_gather(A, width, height, ctx->sfKeys.as<unsigned long long>(), depth, (float2*)depthRange, conf, n, s));
+	Carve scratch(ctx->sfScratch);
+	unsigned long long* keys;
+	scratch.take(keys, 4*n);
+	CK(scratch.commit());
+	CK(sgmf_launch_project(A, width, height, keys, s));
+	CK(sgmf_launch_gather(A, width, height, keys, depth, (float2*)depthRange, conf, n, s));
 	ctx->launches = 2;
 	return B200MVS_OK;
 }
@@ -649,11 +678,13 @@ int b200mvs_sgm_fuse_device(b200mvs_ctx* ctx, const b200mvs_sgm_pair* pairs, int
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t s = stream_of(ctx, stream);
 	const size_t n = (size_t)width*height, np = (size_t)nPairs*n;
-	CK(ctx->sfKeys.reserve(4*np*sizeof(unsigned long long)));
-	CK(ctx->sfMaps.reserve(np*4*sizeof(float)));
-	float2* range = ctx->sfMaps.as<float2>(); float* pd = (float*)(range+np); float* pc = pd+np;
-	CK(sgmf_launch_project(A, width, height, ctx->sfKeys.as<unsigned long long>(), s));
-	CK(sgmf_launch_gather(A, width, height, ctx->sfKeys.as<unsigned long long>(), pd, range, pc, n, s));
+	// the splat keys, then every pair's range, depth and confidence maps (pair p at p x n)
+	Carve scratch(ctx->sfScratch);
+	unsigned long long* keys; float2* range; float *pd, *pc;
+	scratch.take(keys, 4*np); scratch.take(range, np); scratch.take(pd, np); scratch.take(pc, np);
+	CK(scratch.commit());
+	CK(sgmf_launch_project(A, width, height, keys, s));
+	CK(sgmf_launch_gather(A, width, height, keys, pd, range, pc, n, s));
 	CK(sgmf_launch_fuse(nPairs, width, height, pd, range, pc, n, minViews, depth, conf, s));
 	ctx->launches = 3;
 	if (K) {
