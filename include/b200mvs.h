@@ -489,6 +489,43 @@ const float* b200mvs_pointcloud_weights(const b200mvs_pointcloud* cloud);
 const uint16_t* b200mvs_pointcloud_projs(const b200mvs_pointcloud* cloud);         /* pixel (x, y) of every view of every point */
 void b200mvs_pointcloud_free(b200mvs_pointcloud* cloud);
 
+/* ---- the point cloud without fusion, its colours and its normals ---------------------------------
+ * DepthMapsData::MergeDepthMaps (libs/MVS/SceneDensify.cpp:1305-1366), the branch DenseReconstruction takes when nMinViewsFuse < 2:
+ * images in index order, pixels in raster order; every pixel of a depth-map (depth != NULL) whose depth is not 0 becomes one point
+ * seen by its own image, at projection (x, y).  The same view table as the fusion; only depth, normal, color, width, height, K, R
+ * and C are read, and from prm only bEstimateColor (the colour map's pixel) and bEstimateNormal (R^T of the normal map's normal);
+ * NULL prm: the defaults.  An image with a depth-map and no colour map (normal map) while bEstimateColor (bEstimateNormal) is set
+ * is refused (B200MVS_ERR_ARG).  nDepths is the number of points; there are no weights (b200mvs_pointcloud_weights gives NULL).
+ * The host form is host code over HOST maps; the device form takes DEVICE maps on the context's device (the table stays on the
+ * host), runs on `stream`, waits for it and returns the same cloud bit for bit. */
+int b200mvs_merge_depth_maps(const b200mvs_fuse_view* views, int nViews, const b200mvs_fuse_params* prm, b200mvs_pointcloud** cloud);
+int b200mvs_merge_depth_maps_device(b200mvs_ctx* ctx, const b200mvs_fuse_view* views, int nViews, const b200mvs_fuse_params* prm,
+	b200mvs_pointcloud** cloud, void* stream, b200mvs_stats* stats);
+/* EstimatePointColors (libs/MVS/DepthMap.cpp:1429-1465) into colors (3 bytes per point).  The cloud in the layout of the
+ * b200mvs_pointcloud accessors: points (3 floats per point), viewOffsets (nPoints + 1 entries from 0), views (image IDs below
+ * nImages).  images: the scene images; color (3 bytes per pixel, NULL: the image is empty), width, height, K, R and C are read.
+ * A point takes the colour of its view of least depth, sampled bilinearly with the reference's uint8 truncations; white when it
+ * has no view with an image or projects outside the 1-pixel border.  The host form stages HOST buffers (and colour maps); the
+ * _device form takes DEVICE points / viewOffsets / views / colors / images[i].color and a host `images` table, runs on `stream`
+ * and waits for it. */
+int b200mvs_estimate_point_colors(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
+	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, uint8_t* colors, b200mvs_stats* stats);
+int b200mvs_estimate_point_colors_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
+	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, uint8_t* colors, void* stream);
+/* EstimatePointNormals (libs/MVS/DepthMap.cpp:1469-1519) into normals (3 floats per point): the unit eigenvector of the smallest
+ * eigenvalue of the scatter matrix of the point's min(numNeighbors, nPoints) nearest points (itself included; ties to the lower
+ * index; double), cast to float and turned towards the camera centre of the point's first view.  1 <= numNeighbors <= 32 (the
+ * reference's default is 16); every point needs a view, and every coordinate must be finite (B200MVS_ERR_ARG otherwise, before
+ * any grid is built); at most 2^31 - 1 points.  Same buffers as the colour calls (only C of images is read). */
+#define B200MVS_MAX_POINT_NEIGHBORS 32
+int b200mvs_estimate_point_normals(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
+	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int numNeighbors, float* normals, b200mvs_stats* stats);
+int b200mvs_estimate_point_normals_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
+	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int numNeighbors, float* normals, void* stream);
+/* The exact neighbour search of the normals: per point the min(numNeighbors, nPoints) nearest points, ascending by (squared distance
+ * in double, index), into indices (nPoints x min(numNeighbors, nPoints), DEVICE).  points: DEVICE, finite. */
+int b200mvs_point_knn_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, int numNeighbors, uint32_t* indices, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

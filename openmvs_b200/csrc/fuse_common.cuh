@@ -75,10 +75,13 @@ FUSE_HD void normal_to_world(const Cam& c, const float* n, float out[3]) {
 // Conf2Weight (SceneDensify.cpp:120-122)
 FUSE_HD float conf2weight(float conf, float depth) { return div_f(1.f, mul_f(mul_f(fmaxf(sub_f(1.f, conf), 0.03f), depth), depth)); }
 
-// Camera::ProjectPointP3<float> (Camera.h:308-314): double sums, float components
-FUSE_HD float project_row(const double* P, const float pt[3]) {
-	return (float)add_d(add_d(add_d(mul_d(P[0], (double)pt[0]), mul_d(P[1], (double)pt[1])), mul_d(P[2], (double)pt[2])), P[3]);
+// one row of P applied to a float point widened to double; row 2 is Camera::PointDepth (libs/MVS/Camera.cpp:112-115)
+FUSE_HD double project_row_d(const double* P, const float pt[3]) {
+	return add_d(add_d(add_d(mul_d(P[0], (double)pt[0]), mul_d(P[1], (double)pt[1])), mul_d(P[2], (double)pt[2])), P[3]);
 }
+
+// Camera::ProjectPointP3<float> (Camera.h:308-314): double sums, float components
+FUSE_HD float project_row(const double* P, const float pt[3]) { return (float)project_row_d(P, pt); }
 
 // The pixel of neighbour B a point falls on: false when it is behind B (pz <= 0) or outside its w x h map.  ROUND2INT
 // (libs/Common/Types.h:947-953) is floor(v + 0.5); the range test is made on the rounded float, so a value beyond int (or NaN)

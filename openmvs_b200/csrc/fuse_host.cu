@@ -77,14 +77,6 @@ FusePlan fuse_plan(const b200mvs_fuse_view* views, int nViews, const b200mvs_fus
 
 } // namespace
 
-struct b200mvs_pointcloud {
-	std::vector<float> points, normals, weights;
-	std::vector<uint8_t> colors;
-	std::vector<uint32_t> views, offsets;   // views / weights of point i: [offsets[i], offsets[i+1])
-	std::vector<uint16_t> projs;            // pixel (x, y) of every view of every point, parallel to `views`
-	uint64_t nDepths = 0;
-};
-
 extern "C" {
 
 void b200mvs_fuse_default_params(b200mvs_fuse_params* p) {
@@ -216,14 +208,6 @@ cudaError_t grow_keep(DevBuf& b, size_t used, size_t need, cudaStream_t s) {
 	e = cudaStreamSynchronize(s);
 	std::swap(b.p, n.p); std::swap(b.cap, n.cap);
 	return e;
-}
-
-// map pointers of the device form must be device (or managed) memory of the context's device
-bool on_device(const b200mvs_ctx* ctx, const void* p) {
-	if (!p) return true;
-	cudaPointerAttributes a;
-	if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-	return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == ctx->device;
 }
 
 } // namespace

@@ -1,5 +1,6 @@
 // host_ctx.h — the engine context behind the C-ABI (b200mvs_ctx) and the helpers shared by its host files: capi.cu (lifecycle
-// and settings), pm_host.cu (PatchMatch), sgm_host.cu (SGM), post_host.cu (post-processing and image preparation).
+// and settings), pm_host.cu (PatchMatch), sgm_host.cu (SGM), post_host.cu (post-processing and image preparation), fuse_host.cu
+// (FuseDepthMaps), cloud_host.cu (MergeDepthMaps, point colours and normals).
 // Internal to the library; include/b200mvs.h is the interface.
 //
 // Device scratch is owned by subsystem: the context keeps one arena per subsystem, and each entry point carves all of its
@@ -72,6 +73,19 @@ struct ReadBack {
 	int minMax[2];                            // tSGM without levels: the disparity range of the initial map
 	int nArcs;                                // RemoveSmallSegments: one-way edges between segments
 	FuseCounters fuse;                        // FuseDepthMaps (device form)
+	unsigned long long mergePoints;           // MergeDepthMaps (device form): the number of points
+	int cloudBad;                             // point colours / normals / k-NN: what the checks found (CLOUD_* bits)
+	unsigned cloudBox[6];                     // point normals / k-NN: bounding box as ordered keys (box_key, cloud_common.cuh)
+	float cloudSample[3*1024];                // point normals / k-NN: the points the grid's extent is estimated from (CLOUD_SAMPLE)
+};
+
+// PointCloud as the fusion and the merge return it (b200mvs_pointcloud accessors)
+struct b200mvs_pointcloud {
+	std::vector<float> points, normals, weights;
+	std::vector<uint8_t> colors;
+	std::vector<uint32_t> views, offsets;   // views / weights of point i: [offsets[i], offsets[i+1])
+	std::vector<uint16_t> projs;            // pixel (x, y) of every view of every point, parallel to `views`
+	uint64_t nDepths = 0;
 };
 
 struct b200mvs_ctx {
@@ -88,6 +102,8 @@ struct b200mvs_ctx {
 	DevBuf sfScratch;                         // SGM fusion and the normal map
 	DevBuf ppScratch;                         // post-processing: filter, small segments, gap interpolation
 	DevBuf fsScratch, fsRoundScratch;         // FuseDepthMaps (device form): the call, and one round of it
+	DevBuf pcScratch, pcCub;                  // MergeDepthMaps, point colours / normals, k-NN: the call, and CUB's temporary storage
+	DevBuf pcOut;                             // MergeDepthMaps (device form): the point cloud before its read-back
 	ReadBack* words = nullptr;                // allocated on first use, never moved
 	// wave-front aggregation: cached schedule of the last (size, mode)
 	struct FrontPass { FrontLaunch launch; DevBuf items, need; int nItems = 0; };   // launch.items is emptied once uploaded
@@ -132,6 +148,14 @@ inline cudaError_t read_back(b200mvs_ctx* ctx, ReadBack*& words) {
 	}
 	words = ctx->words;
 	return cudaSuccess;
+}
+
+// map pointers of a device form must be device (or managed) memory of the context's device
+inline bool on_device(const b200mvs_ctx* ctx, const void* p) {
+	if (!p) return true;
+	cudaPointerAttributes a;
+	if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+	return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == ctx->device;
 }
 
 // the caller's stream, or the context's when it passes none

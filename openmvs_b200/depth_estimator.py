@@ -822,10 +822,12 @@ _DEVICE_CTX = {}
 
 
 def _device_context(dev) -> _Context:
-	"""the context kept per device for the module-level device calls (EstimateNormalMap, FuseDepthMaps)"""
-	ctx = _DEVICE_CTX.get(dev.index)
+	"""the context kept per device (a torch device or an index) for the module-level calls (EstimateNormalMap, FuseDepthMaps, the
+	point-cloud calls; their host-buffer forms use device 0's)"""
+	index = dev if isinstance(dev, int) else dev.index
+	ctx = _DEVICE_CTX.get(index)
 	if ctx is None:
-		ctx = _DEVICE_CTX[dev.index] = _Context(dev.index)
+		ctx = _DEVICE_CTX[index] = _Context(index)
 	return ctx
 
 
@@ -905,8 +907,8 @@ def FuseDepthMaps(views, nMinViewsFuse: int = 2, fDepthDiffThreshold: float = 0.
 		lib.b200mvs_pointcloud_free(cloud)
 
 
-def _point_cloud(lib, cloud) -> PointCloud:
-	"""copy a b200mvs_pointcloud into a PointCloud"""
+def _point_cloud(lib, cloud, weights: bool = True) -> PointCloud:
+	"""copy a b200mvs_pointcloud into a PointCloud; weights=False: a cloud without weights (MergeDepthMaps), pointWeights None"""
 	m = int(lib.b200mvs_pointcloud_size(cloud))
 	def take(fn, count, dt):
 		p = fn(cloud)
@@ -918,7 +920,7 @@ def _point_cloud(lib, cloud) -> PointCloud:
 	pj = take(lib.b200mvs_pointcloud_projs, 2*total, np.uint16)
 	nr = take(lib.b200mvs_pointcloud_normals, 3*m, np.float32); cl = take(lib.b200mvs_pointcloud_colors, 3*m, np.uint8)
 	return PointCloud(points=pts.reshape(-1, 3) if pts is not None else np.zeros((0, 3), np.float32),
-		pointViews=[vs[off[i]:off[i+1]] for i in range(m)], pointWeights=[ws[off[i]:off[i+1]] for i in range(m)],
+		pointViews=[vs[off[i]:off[i+1]] for i in range(m)], pointWeights=[ws[off[i]:off[i+1]] for i in range(m)] if weights else None,
 		colors=None if cl is None else cl.reshape(-1, 3), normals=None if nr is None else nr.reshape(-1, 3),
 		projs=[pj[2*off[i]:2*off[i+1]].reshape(-1, 2) for i in range(m)], nDepths=int(lib.b200mvs_pointcloud_depths(cloud)))
 
@@ -939,3 +941,16 @@ def FuseRoundStats():
 		out[index] = [dict(image=int(img[i]), iterations=int(it[i]), candidates=int(cand[i]), edges=int(edges[i]), shared=int(shared[i]),
 			ms=float(ms[i])) for i in range(m)]
 	return out
+
+
+
+# The point-cloud calls after the fusion live in point_cloud.py, which builds on this module; they are re-exported here on first
+# use, so that either module can be imported first.
+_POINT_CLOUD_CALLS = ("MergeDepthMaps", "EstimatePointColors", "EstimatePointNormals", "PointKNN")
+
+
+def __getattr__(name):
+	if name in _POINT_CLOUD_CALLS:
+		from . import point_cloud
+		return getattr(point_cloud, name)
+	raise AttributeError("module %r has no attribute %r" % (__name__, name))

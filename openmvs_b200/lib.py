@@ -10,6 +10,7 @@ from . import build as _build
 ABI_VERSION = 7  # B200MVS_ABI_VERSION of include/b200mvs.h these structs mirror
 SGM_MAX_LEVELS = 9  # B200MVS_SGM_MAX_LEVELS: entries of the level-size arrays of b200mvs_sgm_levels
 SGM_MAX_PAIRS = 32  # B200MVS_SGM_MAX_PAIRS: pairs one b200mvs_sgm_fuse call takes
+MAX_POINT_NEIGHBORS = 32  # B200MVS_MAX_POINT_NEIGHBORS: the largest numNeighbors of the point-normal and k-NN calls
 
 
 class View(C.Structure):
@@ -164,6 +165,13 @@ PROTOTYPES = {
 	"b200mvs_pointcloud_weights": (C.POINTER(F), [P]),
 	"b200mvs_pointcloud_projs": (C.POINTER(C.c_uint16), [P]),
 	"b200mvs_pointcloud_free": (None, [P]),
+	"b200mvs_merge_depth_maps": (I, [C.POINTER(FuseView), I, C.POINTER(FuseParams), PP]),
+	"b200mvs_merge_depth_maps_device": (I, [P, C.POINTER(FuseView), I, C.POINTER(FuseParams), PP, P, PStats]),
+	"b200mvs_estimate_point_colors": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, P, PStats]),
+	"b200mvs_estimate_point_colors_device": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, P, P]),
+	"b200mvs_estimate_point_normals": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, I, P, PStats]),
+	"b200mvs_estimate_point_normals_device": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, I, P, P]),
+	"b200mvs_point_knn_device": (I, [P, P, U64, I, P, P]),
 }
 SYMBOLS = list(PROTOTYPES)
 

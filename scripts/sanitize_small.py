@@ -52,3 +52,13 @@ p = DepthData([], 0, 0, fd.copy(), np.ascontiguousarray(sc.views[1].normal_gt*(f
 dm.RemoveSmallSegments(p); print("segments kept", (p.depthMap > 0).mean())
 dm.GapInterpolation(p); print("gaps filled to", (p.depthMap > 0).mean())
 dm.pmCUDA.Release()
+# the point-cloud tail: merge (both forms), colours and normals (host-buffer and device forms), k-NN
+from openmvs_b200.depth_estimator import EstimatePointColors, EstimatePointNormals, MergeDepthMaps, PointKNN
+pv = [dict(depth=maps[i][0].copy(), normal=np.ascontiguousarray(sc.views[i].normal_gt), K=sc.views[i].K, R=sc.views[i].R, C=sc.views[i].C,
+	color=(np.clip(sc.views[i].image, 0, 1)[..., None]*255).astype(np.uint8).repeat(3, -1)) for i in range(3)]
+MergeDepthMaps(pv)
+pc = MergeDepthMaps([dict(v, **{k: torch.from_numpy(np.ascontiguousarray(v[k])).cuda() for k in ("depth", "normal", "color")}) for v in pv])
+EstimatePointColors(pv, pc); EstimatePointNormals(pv, pc)
+pc.points = torch.from_numpy(pc.points).cuda()
+EstimatePointColors([dict(v, color=torch.from_numpy(v["color"]).cuda()) for v in pv], pc); EstimatePointNormals(pv, pc, 32)
+print("point cloud", len(pc.points), "knn", tuple(PointKNN(pc.points, 16).shape))
