@@ -89,7 +89,8 @@ typedef struct {
 } b200mvs_params;
 
 /* Diagnostic switches (all zero = the shipped kernels); replaces the environment variables of round 1.  The PatchMatch kernels
- * have none: reserved0..2 hold the places of three retired switches and are ignored. */
+ * have none: reserved0..2 hold the places of three retired switches and are ignored.  The wave-front SGM aggregation has one
+ * schedule: reserved3..9 hold the places of its seven retired tuning switches and are ignored. */
 typedef struct {
 	int reserved0;       /* ignored */
 	int reserved1;       /* ignored */
@@ -98,15 +99,13 @@ typedef struct {
 	int sgmCost;         /* 0 auto (tensor-core kernel for dense volumes with one range of 64 / 128 / 192 / 256 disparities, SIMT otherwise);
 	                        1 SIMT cost kernel; 2 tensor-core (wgmma) cost kernel or an error */
 	int reserved2;       /* ignored */
-	int frontLayout;     /* wave-front aggregation: 0 auto; 1 two tilted fronts +-(x+2y), four directions each; 2 four straight
-	                        fronts; 3 eight passes of one direction */
-	int frontSerial;     /* 1: one pass per launch into one sum volume (default: two passes share a launch, each with its own
-	                        volume, added by the winner-takes-all kernel) */
-	int frontBlock;      /* fronts per work item (0: default) */
-	int frontLag;        /* 1 + queue distance, in blocks, between the directions of a pass (0: default = distance 1) */
-	int frontCtas;       /* resident CTAs per SM (0: default) */
-	int frontDepth;      /* steps whose loads are in flight: 4 or 8 (0: default) */
-	int frontSubCell;    /* columns per sub-cell of the phase dependencies (0: default 64; never fewer than width / 30) */
+	int reserved3;       /* ignored */
+	int reserved4;       /* ignored */
+	int reserved5;       /* ignored */
+	int reserved6;       /* ignored */
+	int reserved7;       /* ignored */
+	int reserved8;       /* ignored */
+	int reserved9;       /* ignored */
 	int reserved[4];
 } b200mvs_debug;
 

@@ -105,9 +105,9 @@ struct b200mvs_ctx {
 	DevBuf pcScratch, pcCub;                  // MergeDepthMaps, point colours / normals, k-NN: the call, and CUB's temporary storage
 	DevBuf pcOut;                             // MergeDepthMaps (device form): the point cloud before its read-back
 	ReadBack* words = nullptr;                // allocated on first use, never moved
-	// wave-front aggregation: cached schedule of the last (size, mode)
-	struct FrontPass { FrontLaunch launch; DevBuf items, need; int nItems = 0; };   // launch.items is emptied once uploaded
-	std::vector<FrontPass> sgFront; int sgFrontKey[6] = {0, 0, 0, 0, 0, 0};
+	// wave-front aggregation: the schedule of the last valid-region size vw x vh, uploaded (launch.items is emptied then)
+	struct FrontSchedule { int vw = 0, vh = 0; FrontLaunch launch; DevBuf items, need; int nItems = 0; };
+	FrontSchedule sgFront;
 	cudaStream_t sgSide[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // side streams of the ragged aggregation
 	cudaEvent_t sgJoin[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}, sgFork = nullptr;
 	// the accumulated costs of the last SGM match in its own scratch, and their pixel map (b200mvs_sgm_refine_device check)

@@ -53,8 +53,8 @@ bool sgm_cost_tc_supports(int num);
 cudaError_t sgm_cost_tc_launch(const SGMParams& P, int dmin, int num, cudaStream_t s);
 // sgm_front.cu (FrontArgs: sgm_front_sched.h)
 struct FrontArgs;
-cudaError_t sgm_front_launch(const SGMParams& P, const FrontArgs& A, int blocks, int pd, cudaStream_t s);
-int sgm_front_blocks_per_sm(int num, int pd);
+cudaError_t sgm_front_launch(const SGMParams& P, const FrontArgs& A, int blocks, cudaStream_t s);
+int sgm_front_blocks_per_sm(int num);
 bool sgm_front_supports(int num);
 // sgm_tsgm.cu
 size_t tsgm_range_map_scratch(size_t n);

@@ -38,6 +38,7 @@
 namespace {
 
 constexpr int FRONT_WARPS = 4;
+constexpr int PD = 8;   // ring slots per warp: steps whose loads are in flight (DESIGN §5.3)
 
 __device__ __forceinline__ uint4 ldcg4(const void* p) { return __ldcg((const uint4*)p); }
 __device__ __forceinline__ void stcg4(void* p, uint4 v) { __stcg((uint4*)p, v); }
@@ -62,12 +63,11 @@ template <int NW> struct FrontSlot {
 	static constexpr int BYTES = IOFF+128;
 };
 
-// NW words per lane (2*NW disparities), 8 lanes per pixel, 4 pixels (adjacent paths) per warp; PD = ring slots = steps whose
-// loads are in flight.  Dense volumes only: every pixel of the valid region is valid, owns `num` = 16*NW entries at
-// idx = (y*vw + x)*num (checked by the caller).  Per-item overhead is kept off the critical path: the ticket of the item after
+// NW words per lane (2*NW disparities), 8 lanes per pixel, 4 pixels (adjacent paths) per warp.  Dense volumes only: every pixel
+// of the valid region is valid, owns `num` = 16*NW entries at idx = (y*vw + x)*num (checked by the caller).  Per-item overhead is kept off the critical path: the ticket of the item after
 // next and the record of the next item are requested while the current item runs; the copies of the first steps' read-only
 // inputs (costs, intensities) are issued before the dependency wait; the wait polls with relaxed loads and fences once.
-template <int NW, int PD>
+template <int NW>
 __global__ void __launch_bounds__(FRONT_WARPS*32)
 sgm_front_kernel(const __grid_constant__ SGMParams P, const __grid_constant__ FrontArgs A)
 {
@@ -104,7 +104,7 @@ sgm_front_kernel(const __grid_constant__ SGMParams P, const __grid_constant__ Fr
 		const int s0 = min(n, front_first_step(fblk*A.FB, f0, df)), s1 = min(n, front_first_step((fblk+1)*A.FB, f0, df));
 		const int cnt = s1-s0;
 		const int maxcnt = __reduce_max_sync(0xFFFFFFFFu, cnt);
-		const bool add = __any_sync(0xFFFFFFFFu, !(A.storePhase0[pass] && ph == 0));   // item-wide, and known to be warp-uniform
+		const bool add = ph != 0;   // phase 0 stores the sum
 		uint16_t* const sum = A.sum[pass];
 		// Step k of this lane's segment lies at base + min(k, last)*stride: every lane takes part in every copy (lanes whose
 		// segment is shorter re-read their last step, lanes without steps the first slice of the volume).
@@ -276,37 +276,36 @@ sgm_front_kernel(const __grid_constant__ SGMParams P, const __grid_constant__ Fr
 	}
 }
 
-template <int NW, int PD> cudaError_t front_launch(const SGMParams& P, const FrontArgs& A, int blocks, cudaStream_t s) {
+template <int NW> cudaError_t front_launch(const SGMParams& P, const FrontArgs& A, int blocks, cudaStream_t s) {
 	const int smem = FRONT_WARPS*PD*FrontSlot<NW>::BYTES;
-	cudaError_t e = cudaFuncSetAttribute(sgm_front_kernel<NW, PD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+	cudaError_t e = cudaFuncSetAttribute(sgm_front_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
 	if (e != cudaSuccess) return e;
-	sgm_front_kernel<NW, PD><<<blocks, FRONT_WARPS*32, smem, s>>>(P, A);
+	sgm_front_kernel<NW><<<blocks, FRONT_WARPS*32, smem, s>>>(P, A);
 	return cudaGetLastError();
 }
-template <int NW, int PD> int front_blocks_per_sm() {
+template <int NW> int front_blocks_per_sm() {
 	int per = 1;
 	const int smem = FRONT_WARPS*PD*FrontSlot<NW>::BYTES;
-	cudaFuncSetAttribute(sgm_front_kernel<NW, PD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-	cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, sgm_front_kernel<NW, PD>, FRONT_WARPS*32, smem);
+	cudaFuncSetAttribute(sgm_front_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+	cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, sgm_front_kernel<NW>, FRONT_WARPS*32, smem);
 	return std::max(1, per);
 }
 
 } // namespace
 
-// pd: ring slots per warp (4 or 8 steps in flight)
-cudaError_t sgm_front_launch(const SGMParams& P, const FrontArgs& A, int blocks, int pd, cudaStream_t s) {
+cudaError_t sgm_front_launch(const SGMParams& P, const FrontArgs& A, int blocks, cudaStream_t s) {
 	const int NW = A.num/16;
-	if (NW == 8) return pd == 4 ? front_launch<8, 4>(P, A, blocks, s) : front_launch<8, 8>(P, A, blocks, s);
-	if (NW == 4) return pd == 4 ? front_launch<4, 4>(P, A, blocks, s) : front_launch<4, 8>(P, A, blocks, s);
-	if (NW == 16) return pd == 4 ? front_launch<16, 4>(P, A, blocks, s) : front_launch<16, 8>(P, A, blocks, s);
+	if (NW == 8) return front_launch<8>(P, A, blocks, s);
+	if (NW == 4) return front_launch<4>(P, A, blocks, s);
+	if (NW == 16) return front_launch<16>(P, A, blocks, s);
 	return cudaErrorInvalidValue;
 }
 // resident CTAs of the kernel per SM on the current device
-int sgm_front_blocks_per_sm(int num, int pd) {
+int sgm_front_blocks_per_sm(int num) {
 	const int NW = num/16;
-	if (NW == 8) return pd == 4 ? front_blocks_per_sm<8, 4>() : front_blocks_per_sm<8, 8>();
-	if (NW == 4) return pd == 4 ? front_blocks_per_sm<4, 4>() : front_blocks_per_sm<4, 8>();
-	if (NW == 16) return pd == 4 ? front_blocks_per_sm<16, 4>() : front_blocks_per_sm<16, 8>();
+	if (NW == 8) return front_blocks_per_sm<8>();
+	if (NW == 4) return front_blocks_per_sm<4>();
+	if (NW == 16) return front_blocks_per_sm<16>();
 	return 1;
 }
 bool sgm_front_supports(int num) { return num == 64 || num == 128 || num == 256; }

@@ -37,9 +37,8 @@ struct FrontArgs {
 	int maxPaths;        // paths per phase slot in state / meta
 	int FB;              // fronts per block
 	int num;             // disparities per pixel (16 * NW)
-	// the (up to two) passes that share the launch's queue; each accumulates into its own sum volume
+	// the two passes that share the launch's queue; each accumulates into its own sum volume, which its phase 0 stores
 	int fa[2], fb[2], fc[2];   // front f(x,y) = fa*x + fb*y + fc >= 0
-	int storePhase0[2];        // 1: phase 0 stores the sum instead of adding to it (the volume's first pass)
 	uint16_t* sum[2];
 };
 
@@ -76,14 +75,25 @@ FRONT_HD inline int front_first_step(int lo, int f0, int df) {
 }
 
 // ---- host side: schedule --------------------------------------------------------------------------------------------
-struct FrontPassDesc { int fa, fb; int nDirs; int dirs[4]; };
+// A pass: the front f = fa*x + fb*y and its four directions, in phase order
+struct FrontPassDesc { int fa, fb; int dirs[4]; };
+// The two tilted passes f = +-(x + 2y): {right, right-down, down, left-down} then {left, left-up, up, right-up}
+constexpr FrontPassDesc FRONT_PASSES[2] = {{1, 2, {1, 4, 0, 5}}, {-1, -2, {3, 7, 2, 6}}};
 
-// Phase dependencies are tracked per SUB-CELL: a front block cut into column ranges of SW (default FRONT_SW) pixels.  An item touches the one
+// Phase dependencies are tracked per SUB-CELL: a front block cut into column ranges of SW pixels.  An item touches the one
 // to three sub-cells its pixels fall into (its paths are adjacent and its segment is at most a block long); it waits until every
 // item of the previous phase that touches one of them is complete, and bumps the counters of its own when it is done.  With
 // dependencies this local the phases of a block can follow each other directly in the queue (lag 0): the slice of the sum
 // volume a block owns is read-modify-written by its four directions while it sits in the L2.
-constexpr int FRONT_SW = 64;    // default width; b200mvs_debug.frontSubCell overrides it (the driver keeps at most 30 columns of sub-cells)
+//
+// The schedule the driver runs: 32 fronts per block, lag 1, sub-cells of FRONT_SW columns (DESIGN §5.3 records the measurements
+// that chose them).  The sub-cell dependencies make every lag legal.  A larger lag lets more blocks be in flight at once, but the
+// window of blocks between a block's first and last phase then outgrows the L2 and the sums go to DRAM and back; lag 0 leaves the
+// resident warps all holding items of one block, waiting for each other.  sgm_front_build takes block size, lag and sub-cell
+// width as arguments so that the CPU simulation of the schedule can also test small blocks and other lags.
+constexpr int FRONT_FB = 32, FRONT_LAG = 1, FRONT_SW = 64;
+// One lane polls one counter, and a band at an image corner can span the whole width: at most 30 sub-cell columns
+inline int sgm_front_sub_cell(int vw) { return std::max(FRONT_SW, (vw+29)/30); }
 
 // Work items of one pass in queue order; returns the number of front blocks, bands and sub-cell columns through nFB / maxBands /
 // nSX, and the number of items touching each sub-cell through cellCount (index (ph*nFB + fb)*nSX + sx).
@@ -99,11 +109,10 @@ inline void sgm_front_build(int vw, int vh, const FrontPassDesc& pd, int FB, int
 	nFB = (fmax-fmin)/FB + 1;
 	maxBands = (vw+vh+3)/4 + 1;
 	nSX = (vw+SW-1)/SW;
-	const bool phases = pd.nDirs > 1;      // a pass of one direction has no phase dependencies: no counters
 	items.clear();
 	std::vector<int> xkey;                // first column of every item: position along the front
-	cellCount.assign((size_t)pd.nDirs*nFB*nSX, 0);
-	for (int ph = 0; ph < pd.nDirs; ++ph) {
+	cellCount.assign((size_t)4*nFB*nSX, 0);
+	for (int ph = 0; ph < 4; ++ph) {
 		const int dir = pd.dirs[ph];
 		const int nPaths = front_path_count(dir, vw, vh);
 		for (int band = 0; band*4 < nPaths; ++band) {
@@ -130,7 +139,7 @@ inline void sgm_front_build(int vw, int vh, const FrontPassDesc& pd, int FB, int
 					xlo = std::min(xlo, std::min(xa, xb)); xhi = std::max(xhi, std::max(xa, xb));
 				}
 				if (xhi < 0) continue;
-				const int sx0 = xlo/SW, nsx = phases ? xhi/SW-sx0+1 : 0;
+				const int sx0 = xlo/SW, nsx = xhi/SW-sx0+1;
 				FrontItem it;
 				it.k0 = band*4; it.dir = (short)dir; it.ph = (short)ph; it.fb = fb; it.seq = seq++;
 				it.chain = ph*maxBands + band;
@@ -160,26 +169,23 @@ inline void sgm_front_build(int vw, int vh, const FrontPassDesc& pd, int FB, int
 	items.swap(sorted);
 }
 
-
-// One kernel launch: one pass, or two passes whose items share one queue (interleaved, each pass in its own order).  Two
-// passes never touch the same sum volume, so they are independent chains of dependencies: while an item of one waits for
-// its predecessors the warps find ready work in the other.
+// The launch: the two passes' items share one queue (interleaved, each pass in its own order).  The two passes never touch the
+// same sum volume, so they are independent chains of dependencies: while an item of one waits for its predecessors the warps
+// find ready work in the other.  Pass p accumulates into sum volume p; the winner-takes-all kernel adds the two.
 struct FrontLaunch {
-	int nPasses; FrontPassDesc pass[2];
 	int fc[2], nFB[2], maxBands;
 	int nChains, nCells;           // sizes of progress[] / cellDone[]
-	int subCell;                   // width of a sub-cell in columns
+	int FB, subCell;               // fronts per block, width of a sub-cell in columns
 	std::vector<FrontItem> items;
 	std::vector<int> cellNeed;     // items touching each sub-cell (nCells entries)
 };
-inline void sgm_front_build_launch(int vw, int vh, const FrontPassDesc* pds, int nPasses, int FB, int lag, int SW, FrontLaunch& L) {
-	L.subCell = SW;
-	L.nPasses = nPasses; L.items.clear(); L.cellNeed.clear(); L.nChains = 0; L.nCells = 0; L.maxBands = 0;
+inline void sgm_front_build_launch(int vw, int vh, int FB, int lag, int SW, FrontLaunch& L) {
+	L.FB = FB; L.subCell = SW;
+	L.items.clear(); L.cellNeed.clear(); L.nChains = 0; L.nCells = 0; L.maxBands = 0;
 	std::vector<FrontItem> part[2];
-	for (int p = 0; p < nPasses; ++p) {
-		L.pass[p] = pds[p];
+	for (int p = 0; p < 2; ++p) {
 		int nSX = 0; std::vector<int> cnt;
-		sgm_front_build(vw, vh, pds[p], FB, lag, SW, part[p], L.nFB[p], L.maxBands, L.fc[p], nSX, cnt);
+		sgm_front_build(vw, vh, FRONT_PASSES[p], FB, lag, SW, part[p], L.nFB[p], L.maxBands, L.fc[p], nSX, cnt);
 		for (FrontItem& it: part[p]) {
 			it.dir = (short)(it.dir | (p<<8));
 			it.chain += L.nChains; it.cell += L.nCells;
@@ -188,7 +194,6 @@ inline void sgm_front_build_launch(int vw, int vh, const FrontPassDesc* pds, int
 		L.cellNeed.insert(L.cellNeed.end(), cnt.begin(), cnt.end());
 		L.nChains += 4*L.maxBands; L.nCells += (int)cnt.size();
 	}
-	if (nPasses == 1) { L.items.swap(part[0]); return; }
 	// proportional interleave: both passes reach the end of their queues together
 	const size_t na = part[0].size(), nb = part[1].size();
 	L.items.reserve(na+nb);
@@ -197,38 +202,4 @@ inline void sgm_front_build_launch(int vw, int vh, const FrontPassDesc* pds, int
 		if (ib >= nb || (ia < na && ia*nb <= ib*na)) L.items.push_back(part[0][ia++]);
 		else L.items.push_back(part[1][ib++]);
 	}
-}
-
-// Pass layouts of the wave-front aggregation (b200mvs_debug.frontLayout - 1):
-//   0 (default) two tilted fronts f = +-(x + 2y): {right, right-down, down, left-down} then {left, left-up, up, right-up};
-//   1 four straight fronts: top-down {down, right-down, left-down}, bottom-up {up, right-up, left-up}, left-right, right-left;
-//   2 eight passes of one direction each (the traffic of the per-direction kernels with the new step).
-inline std::vector<FrontPassDesc> sgm_front_layout(int layout) {
-	std::vector<FrontPassDesc> descs;
-	if (layout == 0) {
-		descs.push_back(FrontPassDesc{1, 2, 4, {1, 4, 0, 5}});
-		descs.push_back(FrontPassDesc{-1, -2, 4, {3, 7, 2, 6}});
-	} else if (layout == 1) {
-		descs.push_back(FrontPassDesc{0, 1, 3, {0, 4, 5, 0}});
-		descs.push_back(FrontPassDesc{0, -1, 3, {2, 6, 7, 0}});
-		descs.push_back(FrontPassDesc{1, 0, 1, {1, 0, 0, 0}});
-		descs.push_back(FrontPassDesc{-1, 0, 1, {3, 0, 0, 0}});
-	} else {
-		const int f[8][2] = {{0, 1}, {1, 0}, {0, -1}, {-1, 0}, {1, 1}, {-1, 1}, {1, -1}, {-1, -1}};
-		for (int d = 0; d < 8; ++d) descs.push_back(FrontPassDesc{f[d][0], f[d][1], 1, {d, 0, 0, 0}});
-	}
-	return descs;
-}
-// The launches of a layout: `concurrent` pairs consecutive passes (pass 2j into volume 0, pass 2j+1 into volume 1; the caller adds
-// the two volumes at the end), otherwise one pass per launch, all into volume 0.
-inline std::vector<FrontLaunch> sgm_front_plan(int vw, int vh, int layout, bool concurrent, int FB, int lag, int SW = FRONT_SW) {
-	const std::vector<FrontPassDesc> descs = sgm_front_layout(layout);
-	const int fbSize = layout == 2 ? (1<<28) : FB;   // one-direction passes need no blocks: one item per band walks the whole path
-	std::vector<FrontLaunch> out;
-	const size_t per = concurrent ? 2 : 1;
-	for (size_t i = 0; i < descs.size(); i += per) {
-		out.emplace_back();
-		sgm_front_build_launch(vw, vh, &descs[i], (int)std::min(per, descs.size()-i), fbSize, lag, SW, out.back());
-	}
-	return out;
 }

@@ -6,82 +6,52 @@
 
 namespace {
 
-// One wave-front aggregation: the shape of its schedule (sgm_front_schedule) and the scratch of its launches, carved by the match
+// One wave-front aggregation: the shape of its schedule (sgm_front_schedule) and the scratch of its launch, carved by the match
 struct FrontRun {
-	int layout, FB, maxPaths, maxCtl;
+	int maxPaths, maxCtl;
 	int* ctl; uint16_t* state; float2* meta;   // [ticket, error, -, - | progress | cellDone] (4+maxCtl ints), path state, path meta
 };
 
-// SGM path aggregation with the wave-front kernel (sgm_front.cu).  Pass layouts (b200mvs_debug.frontLayout, 0 = auto = 1):
-//   1 two tilted fronts f = +-(x + 2y): {right, right-down, down, left-down} and {left, left-up, up, right-up};
-//   2 four straight fronts: top-down {down, right-down, left-down}, bottom-up {up, right-up, left-up}, left-right, right-left;
-//   3 eight passes of one direction each (the traffic of the per-direction kernels with the new step).
-// With a `second` volume (`concurrent`), consecutive passes share a launch: pass 2j accumulates into the caller's volume, pass
-// 2j+1 into `second`, and the caller adds the two (the winner-takes-all kernel does).  Without one, every pass has a launch of
-// its own.  sgm_front_schedule brings the context's cached schedule (ctx->sgFront) to this size and layout; sgm_aggregate_fronts
-// launches it.
-int sgm_front_schedule(b200mvs_ctx* ctx, int vw, int vh, int num, bool concurrent, cudaStream_t s, FrontRun& F) {
-	const b200mvs_debug& D = ctx->dbg;
-	const int layout = std::min(std::max(D.frontLayout-1, 0), 2);
-	const int FB = D.frontBlock > 0 ? D.frontBlock : 32;   // fronts per block: larger blocks widen the window of the sum volume kept in the L2
-	// frontLag = lag + 1.  The sub-cell dependencies make every lag legal.  A larger lag lets more blocks be in flight at once, but
-	// the window of blocks between a block's first and last phase then outgrows the L2 and the sums go to DRAM and back; lag 0
-	// leaves the resident warps all holding items of one block, waiting for each other.  Default: lag 1.
-	const int lag = D.frontLag > 0 ? D.frontLag-1 : 1;
-	// sub-cell width: one lane polls one counter, and a band at an image corner can span the whole width: at most 30 sub-cell columns
-	const int SW = std::max(D.frontSubCell >= 16 ? D.frontSubCell : FRONT_SW, (vw+29)/30);
-	const int key[6] = {vw, vh, layout, FB, lag | (SW<<8), concurrent ? 2 : 1};
-	if (memcmp(key, ctx->sgFrontKey, sizeof(key)) != 0) {
-		ctx->sgFront.clear();
-		std::vector<FrontLaunch> plan = sgm_front_plan(vw, vh, layout, concurrent, FB, lag, SW);
-		ctx->sgFront.resize(plan.size());
-		for (size_t i = 0; i < plan.size(); ++i) {
-			b200mvs_ctx::FrontPass& fp = ctx->sgFront[i];
-			CK(fp.items.reserve(plan[i].items.size()*sizeof(FrontItem)));
-			CK(cudaMemcpyAsync(fp.items.p, plan[i].items.data(), plan[i].items.size()*sizeof(FrontItem), cudaMemcpyHostToDevice, s));
-			CK(fp.need.reserve(std::max<size_t>(1, plan[i].cellNeed.size())*sizeof(int)));
-			CK(cudaMemcpyAsync(fp.need.p, plan[i].cellNeed.data(), plan[i].cellNeed.size()*sizeof(int), cudaMemcpyHostToDevice, s));
-			CK(cudaStreamSynchronize(s)); // the pageable source vectors are released below
-			fp.nItems = (int)plan[i].items.size();
-			plan[i].items.clear(); plan[i].items.shrink_to_fit(); plan[i].cellNeed.clear(); plan[i].cellNeed.shrink_to_fit();
-			fp.launch = plan[i];
-		}
-		CK(cudaStreamSynchronize(s)); // the pageable source vectors die with `plan`
-		memcpy(ctx->sgFrontKey, key, sizeof(key));
+// SGM path aggregation with the wave-front kernel (sgm_front.cu): the two tilted passes f = +-(x + 2y) of sgm_front_sched.h share
+// one launch and one queue; pass 0 accumulates into the caller's volume, pass 1 into `second`, and the winner-takes-all kernel
+// adds the two.  The schedule is fixed (32 fronts per block, lag 1, sub-cells of at least 64 columns, DESIGN §5.3) and depends
+// only on the size of the valid region: sgm_front_schedule builds and uploads it when the size changes (ctx->sgFront), and
+// sgm_aggregate_fronts launches it.
+int sgm_front_schedule(b200mvs_ctx* ctx, int vw, int vh, cudaStream_t s, FrontRun& F) {
+	b200mvs_ctx::FrontSchedule& S = ctx->sgFront;
+	if (S.vw != vw || S.vh != vh) {
+		FrontLaunch L;
+		sgm_front_build_launch(vw, vh, FRONT_FB, FRONT_LAG, sgm_front_sub_cell(vw), L);
+		S.vw = S.vh = 0;   // no schedule until the upload has completed
+		CK(S.items.reserve(L.items.size()*sizeof(FrontItem)));
+		CK(cudaMemcpyAsync(S.items.p, L.items.data(), L.items.size()*sizeof(FrontItem), cudaMemcpyHostToDevice, s));
+		CK(S.need.reserve(std::max<size_t>(1, L.cellNeed.size())*sizeof(int)));
+		CK(cudaMemcpyAsync(S.need.p, L.cellNeed.data(), L.cellNeed.size()*sizeof(int), cudaMemcpyHostToDevice, s));
+		CK(cudaStreamSynchronize(s)); // the pageable source vectors are released below
+		S.nItems = (int)L.items.size();
+		L.items.clear(); L.items.shrink_to_fit(); L.cellNeed.clear(); L.cellNeed.shrink_to_fit();
+		S.launch = L; S.vw = vw; S.vh = vh;
 	}
-	F.layout = layout; F.FB = FB; F.maxPaths = vw+vh+8; F.maxCtl = 0;
-	for (auto& fp: ctx->sgFront) F.maxCtl = std::max(F.maxCtl, fp.launch.nChains + fp.launch.nCells);
+	F.maxPaths = vw+vh+8; F.maxCtl = S.launch.nChains + S.launch.nCells;
 	return B200MVS_OK;
 }
 
 int sgm_aggregate_fronts(b200mvs_ctx* ctx, const SGMParams& P, int num, uint16_t* second, const FrontRun& F, cudaStream_t s) {
-	const b200mvs_debug& D = ctx->dbg;
-	const int maxCtl = F.maxCtl;
-	int* ctl = F.ctl;
-	// resident CTAs: the queue needs no particular number; frontCtas = CTAs per SM, frontDepth = ring slots per warp (8 default, 4)
-	const int pd = D.frontDepth == 4 ? 4 : 8;
+	const b200mvs_ctx::FrontSchedule& S = ctx->sgFront;
+	const FrontLaunch& L = S.launch;
+	// resident CTAs: the queue needs no particular number; at most 2 per SM (DESIGN §5.3)
 	int sms = 0; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device));
-	const int perSm = std::min(sgm_front_blocks_per_sm(num, pd), D.frontCtas > 0 ? D.frontCtas : 2);
-	const int blocks = sms*perSm;
-	const int FBeff = F.layout == 2 ? (1<<28) : F.FB;
-	for (size_t i = 0; i < ctx->sgFront.size(); ++i) {
-		b200mvs_ctx::FrontPass& fp = ctx->sgFront[i];
-		const FrontLaunch& L = fp.launch;
-		// [ticket, error, -, - | progress | cellDone]; the error word survives the launches of one call
-		if (i == 0) CK(cudaMemsetAsync(ctl, 0, (size_t)(4+maxCtl)*sizeof(int), s));
-		else { CK(cudaMemsetAsync(ctl, 0, sizeof(int), s)); CK(cudaMemsetAsync(ctl+4, 0, (size_t)maxCtl*sizeof(int), s)); }
-		FrontArgs A; memset(&A, 0, sizeof(A));
-		A.items = fp.items.as<FrontItem>(); A.nItems = fp.nItems;
-		A.ticket = ctl; A.error = ctl+1; A.progress = ctl+4; A.cellDone = ctl+4+L.nChains; A.cellNeed = fp.need.as<int>();
-		A.state = F.state; A.meta = F.meta; A.maxPaths = F.maxPaths;
-		A.FB = FBeff; A.num = num;
-		for (int p = 0; p < L.nPasses; ++p) {
-			A.fa[p] = L.pass[p].fa; A.fb[p] = L.pass[p].fb; A.fc[p] = L.fc[p];
-			A.storePhase0[p] = i == 0 ? 1 : 0;
-			A.sum[p] = p == 0 ? P.accums : second;
-		}
-		CK(sgm_front_launch(P, A, blocks, pd, s)); ++ctx->launches;
-	}
+	const int blocks = sms*std::min(sgm_front_blocks_per_sm(num), 2);
+	// [ticket, error, -, - | progress | cellDone]
+	CK(cudaMemsetAsync(F.ctl, 0, (size_t)(4+F.maxCtl)*sizeof(int), s));
+	FrontArgs A; memset(&A, 0, sizeof(A));
+	A.items = S.items.as<FrontItem>(); A.nItems = S.nItems;
+	A.ticket = F.ctl; A.error = F.ctl+1; A.progress = F.ctl+4; A.cellDone = F.ctl+4+L.nChains; A.cellNeed = S.need.as<int>();
+	A.state = F.state; A.meta = F.meta; A.maxPaths = F.maxPaths;
+	A.FB = L.FB; A.num = num;
+	for (int p = 0; p < 2; ++p) { A.fa[p] = FRONT_PASSES[p].fa; A.fb[p] = FRONT_PASSES[p].fb; A.fc[p] = L.fc[p]; }
+	A.sum[0] = P.accums; A.sum[1] = second;
+	CK(sgm_front_launch(P, A, blocks, s)); ++ctx->launches;
 	return B200MVS_OK;
 }
 
@@ -90,10 +60,10 @@ struct SGMPlan {
 	enum Aggregation { FRONTS, UNIFORM_RING, UNIFORM, RAGGED_STREAMS, RAGGED } agg;
 	bool tcCost;     // the tensor-core cost kernel (sgm_cost_tc.cu), else sgm_cost_kernel
 	bool denseWta;   // sgm_wta_uniform_kernel, else sgm_wta_kernel
-	int volumes;     // sum volumes the aggregation leaves for the winner-takes-all to add: 1, 2 (paired wave-front passes) or 8
+	int volumes;     // sum volumes the aggregation leaves for the winner-takes-all to add: 1, 2 (the wave-front passes) or 8
 };
 
-// Picks the kernels from the pixel map's statistics, the debug switches (b200mvs_debug.sgmAggregation / sgmCost / frontSerial),
+// Picks the kernels from the pixel map's statistics, the debug switches (b200mvs_debug.sgmAggregation / sgmCost),
 // the 16-byte alignment of the cost and sum volumes' base pointers and the largest P2.
 SGMPlan sgm_plan(const SGMMapStats& st, const b200mvs_debug& D, bool costsAligned, bool accumsAligned, int maxP2, uint64_t numCosts) {
 	const int mode = D.sgmAggregation;
@@ -115,8 +85,7 @@ SGMPlan sgm_plan(const SGMMapStats& st, const b200mvs_debug& D, bool costsAligne
 	// dense volume with one range of 64 / 128 / 192 / 256 disparities: the banded-GEMM cost kernel on the tensor cores
 	p.tcCost = dense && costsAligned && sgm_cost_tc_supports(st.maxNum) && D.sgmCost != 1;
 	p.denseWta = dense && accumsAligned;
-	// every wave-front layout has at least two passes, so unless frontSerial is set two of them share a launch
-	p.volumes = front ? (D.frontSerial ? 1 : 2) : p.agg == SGMPlan::RAGGED_STREAMS ? 8 : 1;
+	p.volumes = front ? 2 : p.agg == SGMPlan::RAGGED_STREAMS ? 8 : 1;
 	return p;
 }
 
@@ -177,14 +146,14 @@ int b200mvs_sgm_match_device(b200mvs_ctx* ctx, const float* leftGray, const uint
 	const int nVol = (stages & 2) ? plan.volumes : 1;
 	const bool fronts = (stages & 2) && plan.agg == SGMPlan::FRONTS, streams = (stages & 2) && plan.agg == SGMPlan::RAGGED_STREAMS;
 	FrontRun F = {};
-	if (fronts) { const int rc = sgm_front_schedule(ctx, P.vw, P.vh, st.maxNum, nVol == 2, s, F); if (rc) return rc; }
+	if (fronts) { const int rc = sgm_front_schedule(ctx, P.vw, P.vh, s, F); if (rc) return rc; }
 	// the match's scratch: the volumes the caller does not pass, the second sum volume(s) and the wave-front state
 	Carve scratch(ctx->sgmScratch);
 	const bool ownAccums = !accums;
 	if (ownAccums) scratch.take(accums, numCosts);
 	if (!costs) scratch.take(costs, numCosts);
 	uint16_t* more = nullptr;
-	if (fronts && nVol == 2) scratch.take(more, (size_t)P.vw*P.vh*st.maxNum);
+	if (fronts) scratch.take(more, (size_t)P.vw*P.vh*st.maxNum);
 	if (streams) scratch.take(more, (size_t)7*numCosts);
 	if (fronts) { scratch.take(F.ctl, 4+F.maxCtl); scratch.take(F.state, (size_t)8*F.maxPaths*st.maxNum); scratch.take(F.meta, 8*F.maxPaths); }
 	CK(scratch.commit());

@@ -296,8 +296,8 @@ class _Context:
 
 	def SetDebug(self, **kw):
 		"""b200mvs_set_debug: diagnostic kernel switches, the fields of b200mvs_debug; no arguments = defaults.
-		SGM: sgmAggregation (0 auto, 1 general, 2 register-pipelined uniform, 3 bulk-copy ring, 4 wave fronts), sgmCost,
-		frontLayout / frontSerial / frontBlock / frontLag / frontCtas / frontDepth / frontSubCell.  PatchMatch has no switches.
+		SGM: sgmAggregation (0 auto, 1 general, 2 register-pipelined uniform, 3 bulk-copy ring, 4 wave fronts) and sgmCost
+		(0 auto, 1 SIMT, 2 tensor cores).  PatchMatch has no switches.
 		An unknown or reserved field name raises AttributeError."""
 		d = _lib.Debug()
 		for k, v in kw.items():

@@ -37,8 +37,8 @@ class Params(C.Structure):
 class Debug(C.Structure):
 	"""b200mvs_debug"""
 	_fields_ = [("reserved0", C.c_int), ("reserved1", C.c_int), ("sgmAggregation", C.c_int), ("sgmCost", C.c_int),
-		("reserved2", C.c_int), ("frontLayout", C.c_int), ("frontSerial", C.c_int), ("frontBlock", C.c_int), ("frontLag", C.c_int),
-		("frontCtas", C.c_int), ("frontDepth", C.c_int), ("frontSubCell", C.c_int), ("reserved", C.c_int*4)]
+		("reserved2", C.c_int), ("reserved3", C.c_int), ("reserved4", C.c_int), ("reserved5", C.c_int), ("reserved6", C.c_int),
+		("reserved7", C.c_int), ("reserved8", C.c_int), ("reserved9", C.c_int), ("reserved", C.c_int*4)]
 
 
 class Stats(C.Structure):

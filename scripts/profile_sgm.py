@@ -1,6 +1,6 @@
-"""1080p SGM pair for profiling: per-stage device times of the aggregation variants (b200mvs_debug.sgmAggregation) and of the
-wave-front layouts / block sizes, with an identity check against the register-pipelined kernel.
-usage: profile_sgm.py [D] [default]"""
+"""1080p SGM pair for profiling: per-stage device times of the default kernels and of the aggregation and cost variants
+(b200mvs_debug.sgmAggregation / sgmCost), with an identity check against the register-pipelined kernel.
+usage: profile_sgm.py [D]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -16,41 +16,7 @@ m = SemiGlobalMatcher()
 costs = torch.zeros(n, dtype=torch.uint8, device="cuda"); accums = torch.zeros(n, dtype=torch.int16, device="cuda")
 ref = None
 MODES = [("register pipeline", dict(sgmAggregation=2)), ("bulk-copy ring, 8 launches", dict(sgmAggregation=3)),
-	("wave fronts (default)", dict())]
-for layout, name in ((1, "tilted"), (2, "straight"), (3, "single")):
-	for serial in (0, 1):
-		MODES.append(("fronts %s %s" % (name, "serial" if serial else "paired"), dict(sgmAggregation=4, frontLayout=layout, frontSerial=serial)))
-for layout, name in ((1, "tilted"), (2, "straight")):
-	for fbk in (32, 64):
-		for lag in (0, 1, 2):
-			for ctas in (2, 4):
-				MODES.append(("fronts %s paired FB %d lag %d ctas %d" % (name, fbk, lag, ctas), dict(sgmAggregation=4, frontLayout=layout, frontBlock=fbk, frontLag=lag+1, frontCtas=ctas)))
-MODES += [("fronts tilted paired FB 16 lag 0", dict(sgmAggregation=4, frontBlock=16)), ("fronts tilted paired FB 128 lag 0", dict(sgmAggregation=4, frontBlock=128)),
-	("fronts tilted paired FB 64 lag 0 depth 4", dict(sgmAggregation=4, frontDepth=4)), ("fronts tilted paired FB 64 lag 0 ctas 1", dict(sgmAggregation=4, frontCtas=1)),
-	("fronts tilted paired FB 64 lag 0 ctas 3", dict(sgmAggregation=4, frontCtas=3))]
-MODES.append(("SIMT cost kernel + wave fronts", dict(sgmCost=1)))
-if len(sys.argv) > 2 and sys.argv[2] == "default":
-	MODES = MODES[2:3]
-if len(sys.argv) > 2 and sys.argv[2] == "lag0":
-	MODES = [("fronts FB 32 lag 0", dict(sgmAggregation=4, frontLag=1))]
-if len(sys.argv) > 2 and sys.argv[2] == "lag2":
-	MODES = [("fronts FB 32 lag 2", dict(sgmAggregation=4, frontLag=3))]
-if len(sys.argv) > 2 and sys.argv[2] == "lag1":
-	MODES = [("fronts FB 32 lag 1", dict(sgmAggregation=4, frontLag=2))]
-if len(sys.argv) > 2 and sys.argv[2] == "fb64":
-	MODES = [("fronts FB 64 lag 2", dict(sgmAggregation=4, frontBlock=64))]
-if len(sys.argv) > 2 and sys.argv[2] == "order":
-	MODES = MODES[:1]+[("fronts default (FB 32 lag 1)", dict())]
-	for fbk in (32, 64):
-		for lag in (0, 1, 2):
-			for sw in (128, 64):
-				for ctas in (2, 3):
-					MODES.append(("fronts FB %d lag %d subcell %d ctas %d" % (fbk, lag, sw, ctas), dict(sgmAggregation=4, frontBlock=fbk, frontLag=lag+1, frontSubCell=sw, frontCtas=ctas)))
-	MODES.append(("fronts FB 32 lag 1 subcell 32", dict(sgmAggregation=4, frontLag=2, frontSubCell=32)))
-	MODES.append(("fronts FB 32 lag 1 ctas 1", dict(sgmAggregation=4, frontLag=2, frontCtas=1)))
-	MODES.append(("fronts straight FB 32 lag 1", dict(sgmAggregation=4, frontLayout=2, frontLag=2)))
-if len(sys.argv) > 2 and sys.argv[2] == "tc":
-	MODES = MODES[-1:]
+	("wave fronts (default)", dict()), ("SIMT cost kernel + wave fronts", dict(sgmCost=1))]
 for name, dbg in MODES:
 	m.SetDebug(**dbg)
 	for rep in range(2):

@@ -187,13 +187,16 @@ def test_null_context_and_bad_arguments_return_status_codes():
 
 
 def test_set_debug_refuses_reserved_and_unknown_fields():
-	"""The retired PatchMatch switches are reserved fields of b200mvs_debug: naming one (or an old name) is an error, not a
-	silent no-op.  The check runs before any call into the library."""
+	"""The retired PatchMatch switches and wave-front tuning switches are reserved fields of b200mvs_debug: naming one (or an old
+	name) is an error, not a silent no-op.  The check runs before any call into the library."""
 	from openmvs_b200 import lib
 	from openmvs_b200.depth_estimator import PatchMatchB200
 	names = [f for f, _ in lib.Debug._fields_]
 	assert names[:2] == ["reserved0", "reserved1"] and names[4] == "reserved2"
+	assert names[5:12] == ["reserved%d" % i for i in range(3, 10)]
+	retired = ("noTMA", "scalarTaps", "sweepFourCtas",
+		"frontLayout", "frontSerial", "frontBlock", "frontLag", "frontCtas", "frontDepth", "frontSubCell")
 	pm = PatchMatchB200.__new__(PatchMatchB200)   # no context: SetDebug must refuse the name before using one
-	for k in ("reserved", "reserved0", "reserved1", "reserved2", "noTMA", "scalarTaps", "sweepFourCtas"):
+	for k in ("reserved",) + tuple(names[:2]) + tuple(names[4:12]) + retired:
 		with pytest.raises(AttributeError):
 			pm.SetDebug(**{k: 1})
