@@ -1,4 +1,5 @@
-// sgm_front.cu — SGM path aggregation as wave fronts (sm_90a), the default for uniform disparity ranges.
+// sgm_front.cu — SGM path aggregation as wave fronts (sm_90a), the default for dense volumes with one range of 64, 128 or 256
+// disparities.
 //
 // What it computes: the eight path recursions of SemiGlobalMatcher::Match and their sum
 //   L_r(p,d) = C(p,d) + min(L_r(q,d), L_r(q,d+-1)+P1, min_d' L_r(q,d')+P2) - min_d' L_r(q,d'),  S = sum_r L_r
@@ -26,8 +27,9 @@
 //   * the inputs of a step reach the warp through a ring in shared memory filled by cp.async (no destination registers:
 //     the prefetch distance does not depend on the register allocator), and the whole step is branch-free, so that the warp
 //     never splits (a split warp runs every shuffle through a collective re-synchronisation).
-// Bit-exact against the oracle (tests/test_sgm_parity_gpu.py); the per-direction kernels of sgm_kernels.cu remain for
-// ragged (tSGM) ranges and as debug variants (b200mvs_debug.sgmAggregation).
+// Bit-exact against the oracle (tests/test_sgm_parity_gpu.py).  Every other pixel map runs the per-direction kernels of
+// sgm_kernels.cu (sgm_plan, sgm_host.cu): uniform ranges of other widths, with invalid pixels, unaligned slices or a P2 above
+// 16000, and ragged (tSGM) ranges; b200mvs_debug.sgmAggregation can also select them.
 #include "sgm_common.cuh"
 #include "sgm_front_sched.h"
 #include <string.h>

@@ -112,6 +112,9 @@ constexpr int LPAD = 8;
 constexpr int AGG_PD = 2;           // prefetch distance (steps) of the scanline pipeline (general kernel)
 constexpr int AGG_PD_UNIFORM = 4;   // the packed uniform kernel keeps only 3 registers per stage in flight
 
+// penalty of a path step from intensity Ip to I: P2s[|round(255 (I - Ip))|] (SemiGlobalMatcher.cpp:1009, 518-524)
+__device__ __forceinline__ int path_penalty(const SGMParams& P, float I, float Ip) { return P.P2s[abs((int)floorf(255.f*(I-Ip)+.5f))]; }
+
 // One warp walks one scanline; lane l owns disparities l, l+32, ... (NPL per lane) of every pixel.
 // The scanline is a chain of dependent steps, so it is software-pipelined: the pixel record of
 // step t+PD+1 and the cost / accumulator values of step t+PD are in flight while step t computes.
@@ -176,7 +179,7 @@ sgm_aggregate_kernel(const __grid_constant__ SGMParams P, int dir)
 		if (p.dmin < p.dmax) {
 			// NB: the reference reads the intensity at the valid-region coordinates (no half-window offset)
 			const float I = I0;
-			const int P2 = P.P2s[abs((int)floorf(255.f*(I-Ip)+.5f))];
+			const int P2 = path_penalty(P, I, Ip);
 			Ip = I;
 			const uint16_t* Lp = lines[warp][cur] + LPAD;
 			uint16_t* Ls = lines[warp][cur^1] + LPAD;
@@ -269,111 +272,124 @@ sgm_aggregate_kernel(const __grid_constant__ SGMParams P, int dir)
 	}
 }
 
-// Uniform-range variant (the reference's non-tSGM branch gives every pixel one global range,
-// SemiGlobalMatcher.cpp:643-669): all valid pixels share [dmin, dmax), the count is a multiple of 4 and
-// every pixel's slice of the volume is 4-aligned.  Lane l owns the NPL consecutive disparities
-// [l*NPL, l*NPL+NPL): its costs are one packed 32-bit (NPL=4) or 64-bit (NPL=8) load, its accumulators one
-// 64/128-bit load and store, d-1 / d+1 live in the lane's own registers except at the two ends (one
-// shuffle each), and the line never touches shared memory.
+// Uniform ranges (the reference's non-tSGM branch gives every pixel one global range, SemiGlobalMatcher.cpp:643-669): all valid
+// pixels share [dmin, dmin+num), the count is a multiple of 4 and every pixel's slice of the volume is 4-aligned.  Lane l owns the NPL
+// consecutive disparities [l*NPL, l*NPL+NPL): its costs are one packed 32-bit (NPL=4) or 64-bit (NPL=8) word, its sums one 64/128-bit
+// word, d-1 / d+1 live in the lane's own registers except at the two ends (one shuffle each), and the line never touches shared
+// memory.  The two uniform kernels below differ only in how a step's inputs reach the registers; PackedPath is the rest.
 template <int NPL> struct Pack;
 template <> struct Pack<4> { typedef uint32_t C; typedef uint2 A; };
 template <> struct Pack<8> { typedef uint2 C; typedef uint4 A; };
 
+// One warp's scanline in the packed lane layout: the lane's share of the volume, the path state and the step.
+template <int NPL> struct PackedPath {
+	typedef typename Pack<NPL>::C CW;
+	typedef typename Pack<NPL>::A AW;
+	const int lane;
+	const bool active;   // num % 4 == 0 and NPL in {4, 8}: a lane is all in or all out ...
+	const int nval;      // ... except with NPL = 8 and num % 8 == 4: then the last active lane owns 4 disparities
+	unsigned Lp[NPL];    // the previous line
+	unsigned minLp;      // its minimum over the warp
+	bool havePrev;       // false before the first valid pixel of the scanline
+	float Ip;            // intensity of the previous valid pixel
+
+	__device__ __forceinline__ PackedPath(int l, int num)
+		: lane(l), active(l*NPL < num), nval(min(NPL, max(0, num-l*NPL))), minLp(0xFFFFu), havePrev(false), Ip(0.5f) {
+		#pragma unroll
+		for (int j = 0; j < NPL; ++j) Lp[j] = 0xFFFFu;
+	}
+
+	// The lane's packed costs and sums of a slice (costs / sums: the slice's first entries, 4-byte aligned, in global memory or in
+	// a shared-memory stage); zero when the pixel is not valid or the lane owns no disparity.  Word i holds disparities 4i .. 4i+3.
+	__device__ __forceinline__ void load(bool valid, const uint8_t* costs, const uint16_t* sums, CW& c, AW& a) const {
+		uint32_t cw[NPL/4]; uint2 aw[NPL/4];
+		#pragma unroll
+		for (int i = 0; i < NPL/4; ++i) { cw[i] = 0u; aw[i] = make_uint2(0u, 0u); }
+		if (valid && active) {
+			const uint32_t* cs = (const uint32_t*)costs + lane*(NPL/4);
+			const uint2* as = (const uint2*)sums + lane*(NPL/4);
+			#pragma unroll
+			for (int i = 0; i < NPL/4; ++i)
+				if (i == 0 || nval > 4) { cw[i] = cs[i]; aw[i] = as[i]; }
+		}
+		memcpy(&c, cw, sizeof(c)); memcpy(&a, aw, sizeof(a));
+	}
+
+	// One step at a valid pixel of intensity I with the lane's costs c and sums a: the new line, its sum with a stored to the
+	// pixel's slice `sums`, and the line's minimum over the warp.
+	__device__ __forceinline__ void step(const SGMParams& P, float I, CW c, AW a, uint16_t* sums) {
+		const int P2 = path_penalty(P, I, Ip);
+		Ip = I;
+		uint8_t cb[NPL]; uint16_t ab[NPL];
+		memcpy(cb, &c, NPL); memcpy(ab, &a, 2*NPL);
+		unsigned Ln[NPL];
+		if (!havePrev) {
+			#pragma unroll
+			for (int j = 0; j < NPL; ++j) Ln[j] = j < nval ? (unsigned)(cb[j]+P2) : 0xFFFFu;
+		} else {
+			const unsigned below = __shfl_up_sync(0xFFFFFFFFu, Lp[NPL-1], 1);
+			const unsigned above = __shfl_down_sync(0xFFFFFFFFu, Lp[0], 1);
+			const int far = (int)minLp+P2;
+			#pragma unroll
+			for (int j = 0; j < NPL; ++j) {
+				const int lm = j > 0 ? (int)Lp[j-1] : (lane > 0 ? (int)below : 0xFFFF);
+				const int lq = j < NPL-1 ? (int)Lp[j+1] : (lane < 31 ? (int)above : 0xFFFF);
+				const int best = min(min((int)Lp[j], min(lm, lq)+P.P1), far);
+				Ln[j] = j < nval ? (unsigned)((int)cb[j]+best-(int)minLp) : 0xFFFFu;
+			}
+		}
+		if (active) {
+			#pragma unroll
+			for (int j = 0; j < NPL; ++j) ab[j] = (uint16_t)(ab[j]+(j < nval ? Ln[j] : 0u));
+			uint2* dst = (uint2*)sums + lane*(NPL/4);
+			#pragma unroll
+			for (int i = 0; i < NPL/4; ++i)
+				if (i == 0 || nval > 4) { uint2 w; memcpy(&w, ab+4*i, 8); dst[i] = w; }
+		}
+		unsigned mn = Ln[0];
+		#pragma unroll
+		for (int j = 0; j < NPL; ++j) { Lp[j] = Ln[j]; mn = min(mn, Ln[j]); }
+		minLp = __reduce_min_sync(0xFFFFFFFFu, mn); // redux.sync: one instruction instead of a 5-shuffle chain
+		havePrev = true;
+	}
+};
+
+// Register pipeline: any 4-aligned slices.  The pixel record and intensity of step t+PD+1 and the packed words of step t+PD are in
+// flight while step t computes.
 template <int NPL, int PD>
 __global__ void __launch_bounds__(AGG_WARPS*32)
 sgm_aggregate_uniform_kernel(const __grid_constant__ SGMParams P, int dir, int dmin, int num)
 {
-	typedef typename Pack<NPL>::C CW;
-	typedef typename Pack<NPL>::A AW;
+	typedef PackedPath<NPL> Path;
 	const int warp = threadIdx.x>>5, lane = threadIdx.x&31;
 	const int k = blockIdx.x*AGG_WARPS + warp;
 	int x, y, dx, dy;
 	if (!front_path_start(dir, k, P.vw, P.vh, x, y, dx, dy))
 		return;
-	const bool active = lane*NPL < num;   // num % 4 == 0 and NPL in {4, 8}: a lane is all in or all out ...
-	const int nval = min(NPL, max(0, num-lane*NPL)); // ... except with NPL = 8 and num % 8 == 4
-	auto inside = [&](int xx, int yy) { return xx >= 0 && yy >= 0 && xx < P.vw && yy < P.vh; };
-	auto valid = [&](const SGMPixel& p) { return p.dmin < p.dmax; };
+	const int len = front_path_len(x, y, dx, dy, P.vw, P.vh);
+	Path path(lane, num);
+	auto valid = [](const SGMPixel& p) { return p.dmin < p.dmax; };
 	SGMPixel none; none.idx = 0; none.dmin = 0; none.dmax = 0; none.pad = 0;
 	SGMPixel pr[PD+1]; float Ir[PD+1];
-	CW c[PD]; AW a[PD];
-	auto loadC = [&](const SGMPixel& p) -> CW {
-		CW v; memset(&v, 0, sizeof(v));
-		if (active && valid(p)) {
-			const uint32_t* src = (const uint32_t*)(P.costs + p.idx) + lane*(NPL/4);
-			if (NPL == 4) { uint32_t t = src[0]; memcpy(&v, &t, 4); }
-			else { uint2 t; t.x = src[0]; t.y = nval > 4 ? src[1] : 0u; memcpy(&v, &t, 8); }
-		}
-		return v;
-	};
-	auto loadA = [&](const SGMPixel& p) -> AW {
-		AW v; memset(&v, 0, sizeof(v));
-		if (active && valid(p)) {
-			const uint2* src = (const uint2*)(P.accums + p.idx) + lane*(NPL/4);
-			if (NPL == 4) { uint2 t = src[0]; memcpy(&v, &t, 8); }
-			else { uint4 t; const uint2 lo = src[0]; t.x = lo.x; t.y = lo.y; t.z = t.w = 0u; if (nval > 4) { const uint2 hi = src[1]; t.z = hi.x; t.w = hi.y; } memcpy(&v, &t, 16); }
-		}
-		return v;
-	};
+	typename Path::CW c[PD]; typename Path::AW a[PD];
 	#pragma unroll
 	for (int i = 0; i <= PD; ++i) {
 		pr[i] = none; Ir[i] = 0.f;
 		const int xx = x+i*dx, yy = y+i*dy;
-		if (inside(xx, yy)) { pr[i] = P.px[(size_t)yy*P.vw + xx]; Ir[i] = __ldg(P.lgray + (size_t)yy*P.w + xx); }
+		if (i < len) { pr[i] = P.px[(size_t)yy*P.vw + xx]; Ir[i] = __ldg(P.lgray + (size_t)yy*P.w + xx); }
 	}
 	#pragma unroll
-	for (int i = 0; i < PD; ++i) { c[i] = loadC(pr[i]); a[i] = loadA(pr[i]); }
-	unsigned Lp[NPL];
-	#pragma unroll
-	for (int j = 0; j < NPL; ++j) Lp[j] = 0xFFFFu;
-	unsigned minLp = 0xFFFFu;
-	bool havePrev = false;
-	float Ip = 0.5f;
-	for (; inside(x, y); x += dx, y += dy) {
+	for (int i = 0; i < PD; ++i) path.load(valid(pr[i]), P.costs + pr[i].idx, P.accums + pr[i].idx, c[i], a[i]);
+	for (int t = 0; t < len; ++t, x += dx, y += dy) {
 		SGMPixel pnew = none; float Inew = 0.f;
 		{
 			const int xx = x+(PD+1)*dx, yy = y+(PD+1)*dy;
-			if (inside(xx, yy)) { pnew = P.px[(size_t)yy*P.vw + xx]; Inew = __ldg(P.lgray + (size_t)yy*P.w + xx); }
+			if (t+PD+1 < len) { pnew = P.px[(size_t)yy*P.vw + xx]; Inew = __ldg(P.lgray + (size_t)yy*P.w + xx); }
 		}
-		const CW cn = loadC(pr[PD]);
-		const AW an = loadA(pr[PD]);
-		const SGMPixel p = pr[0];
-		if (valid(p)) {
-			const float I = Ir[0];
-			const int P2 = P.P2s[abs((int)floorf(255.f*(I-Ip)+.5f))];
-			Ip = I;
-			uint8_t cb[NPL]; uint16_t ab[NPL];
-			memcpy(cb, &c[0], NPL); memcpy(ab, &a[0], 2*NPL);
-			unsigned Ln[NPL];
-			if (!havePrev) {
-				#pragma unroll
-				for (int j = 0; j < NPL; ++j) Ln[j] = j < nval ? (unsigned)(cb[j]+P2) : 0xFFFFu;
-			} else {
-				const unsigned below = __shfl_up_sync(0xFFFFFFFFu, Lp[NPL-1], 1);
-				const unsigned above = __shfl_down_sync(0xFFFFFFFFu, Lp[0], 1);
-				const int far = (int)minLp+P2;
-				#pragma unroll
-				for (int j = 0; j < NPL; ++j) {
-					const int lm = j > 0 ? (int)Lp[j-1] : (lane > 0 ? (int)below : 0xFFFF);
-					const int lq = j < NPL-1 ? (int)Lp[j+1] : (lane < 31 ? (int)above : 0xFFFF);
-					const int best = min(min((int)Lp[j], min(lm, lq)+P.P1), far);
-					Ln[j] = j < nval ? (unsigned)((int)cb[j]+best-(int)minLp) : 0xFFFFu;
-				}
-			}
-			if (active) {
-				#pragma unroll
-				for (int j = 0; j < NPL; ++j) ab[j] = (uint16_t)(ab[j]+(j < nval ? Ln[j] : 0u));
-				uint2* dst = (uint2*)(P.accums + p.idx) + lane*(NPL/4);
-				uint2 w0; memcpy(&w0, ab, 8); dst[0] = w0;
-				if (NPL == 8 && nval > 4) { uint2 w1; memcpy(&w1, ab+4, 8); dst[1] = w1; }
-			}
-			unsigned mn = Ln[0];
-			#pragma unroll
-			for (int j = 0; j < NPL; ++j) { Lp[j] = Ln[j]; mn = min(mn, Ln[j]); }
-			mn = __reduce_min_sync(0xFFFFFFFFu, mn); // redux.sync: one instruction instead of a 5-shuffle chain
-			minLp = mn;
-			havePrev = true;
-		}
+		typename Path::CW cn; typename Path::AW an;
+		path.load(valid(pr[PD]), P.costs + pr[PD].idx, P.accums + pr[PD].idx, cn, an);
+		if (valid(pr[0]))
+			path.step(P, Ir[0], c[0], a[0], P.accums + pr[0].idx);
 		#pragma unroll
 		for (int i = 0; i < PD; ++i) { pr[i] = pr[i+1]; Ir[i] = Ir[i+1]; }
 		pr[PD] = pnew; Ir[PD] = Inew;
@@ -383,11 +399,9 @@ sgm_aggregate_uniform_kernel(const __grid_constant__ SGMParams P, int dir, int d
 	}
 }
 
-// Uniform-range variant with a bulk-copy ring (cp.async.bulk + mbarrier) — the default on sm_90a when every
-// slice of the volume is 16-byte aligned (num % 16 == 0, idx % 16 == 0).
-// A scanline is a chain of dependent steps, so its bandwidth is set by the bytes it keeps in flight.  Registers
-// limit the kernel above to PD = 4 steps (about 1.5 KB per warp); here every warp owns a ring of 2E stages in
-// shared memory.  The steps are grouped in epochs of E: while epoch e is computed, the copies of epoch e+1
+// Bulk-copy ring (cp.async.bulk + mbarrier): every slice of the volume 16-byte aligned (num % 16 == 0, idx % 16 == 0).
+// A scanline is a chain of dependent steps, so its bandwidth is set by the bytes it keeps in flight.  Every warp owns a ring of 2E
+// stages in shared memory.  The steps are grouped in epochs of E: while epoch e is computed, the copies of epoch e+1
 // are in flight, and when epoch e is done its E stages are refilled for epoch e+2 — lane l < E reads the
 // pixel record of "its" step, posts the expected byte count on that stage's mbarrier and issues the two bulk
 // copies (num cost bytes + 2*num accumulator bytes) itself, so no lane ever waits for another lane's address.
@@ -405,13 +419,15 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, unsigne
 	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
 		:: "r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
+// shared memory of one warp's ring: 2E stages of num cost bytes and 2*num sum bytes, 2E 16-byte records, 2E mbarriers
+__host__ __device__ constexpr unsigned ring_warp_bytes(int E, int num) { return 2u*E*(3u*num+16u+8u); }
 
 template <int NPL, int E>
 __global__ void __launch_bounds__(AGG_WARPS*32)
 sgm_aggregate_uniform_ring_kernel(const __grid_constant__ SGMParams P, int dir, int dmin, int num)
 {
-	typedef typename Pack<NPL>::C CW;
-	typedef typename Pack<NPL>::A AW;
+	typedef typename PackedPath<NPL>::CW CW;
+	typedef typename PackedPath<NPL>::AW AW;
 	constexpr int RING = 2*E;
 	static_assert(RING <= 32, "one lane per stage");
 	extern __shared__ __align__(128) unsigned char ring_smem[];
@@ -422,8 +438,7 @@ sgm_aggregate_uniform_ring_kernel(const __grid_constant__ SGMParams P, int dir, 
 		return;
 	const int n = front_path_len(x0, y0, dx, dy, P.vw, P.vh);
 	const unsigned stageBytes = 3u*(unsigned)num;                        // costs | accumulators
-	const unsigned warpBytes = RING*(stageBytes+16u+8u);
-	unsigned char* base = ring_smem + (size_t)warp*warpBytes;
+	unsigned char* base = ring_smem + (size_t)warp*ring_warp_bytes(E, num);
 	unsigned char* stages = base;                                        // RING x stageBytes (16-byte aligned: num % 16 == 0)
 	uint4* recs = (uint4*)(base + RING*stageBytes);                      // RING x {idx lo, idx hi, intensity, valid | parity << 1}
 	uint64_t* bars = (uint64_t*)(base + RING*(stageBytes+16u));          // RING mbarriers
@@ -431,8 +446,7 @@ sgm_aggregate_uniform_ring_kernel(const __grid_constant__ SGMParams P, int dir, 
 		asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_addr(bars+lane)) : "memory");
 	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");         // the init is visible to the async proxy
 	__syncwarp();
-	const bool active = lane*NPL < num;
-	const int nval = min(NPL, max(0, num-lane*NPL));
+	PackedPath<NPL> path(lane, num);
 	unsigned phase = 0;                                                  // bit h: completions so far (mod 2) of this lane's stage in half h
 	// producer: lane l < E owns step e*E+l of epoch e, stage (e & 1)*E + l
 	auto issue_epoch = [&](int e) {
@@ -457,7 +471,7 @@ sgm_aggregate_uniform_ring_kernel(const __grid_constant__ SGMParams P, int dir, 
 		}
 		__syncwarp();
 	};
-	// consumer: record, wait, packed loads of step t
+	// consumer: record, wait, packed words of step t
 	auto fetch = [&](int t, uint4& r, CW& c, AW& a) {
 		const int slot = t & (RING-1);
 		r = recs[slot];
@@ -465,28 +479,12 @@ sgm_aggregate_uniform_ring_kernel(const __grid_constant__ SGMParams P, int dir, 
 		if (r.w & 1u) {
 			const uint32_t bar = smem_addr(bars+slot);
 			while (!mbar_try_wait(bar, (r.w>>1)&1u)) {}
-			if (active) {
-				const unsigned char* st = stages+(size_t)slot*stageBytes;
-				const uint32_t* cs = (const uint32_t*)st + lane*(NPL/4);
-				const uint2* as = (const uint2*)(st+num) + lane*(NPL/4);
-				if (NPL == 4) { uint32_t v = cs[0]; memcpy(&c, &v, 4); uint2 w = as[0]; memcpy(&a, &w, 8); }
-				else {
-					uint2 v; v.x = cs[0]; v.y = nval > 4 ? cs[1] : 0u; memcpy(&c, &v, 8);
-					uint4 w; const uint2 lo = as[0]; w.x = lo.x; w.y = lo.y; w.z = w.w = 0u;
-					if (nval > 4) { const uint2 hi = as[1]; w.z = hi.x; w.w = hi.y; }
-					memcpy(&a, &w, 16);
-				}
-			}
+			const unsigned char* st = stages+(size_t)slot*stageBytes;
+			path.load(true, st, (const uint16_t*)(st+num), c, a);
 		}
 	};
 	issue_epoch(0);
 	issue_epoch(1);
-	unsigned Lp[NPL];
-	#pragma unroll
-	for (int j = 0; j < NPL; ++j) Lp[j] = 0xFFFFu;
-	unsigned minLp = 0xFFFFu;
-	bool havePrev = false;
-	float Ip = 0.5f;
 	uint4 rec; CW c; AW a;
 	fetch(0, rec, c, a);
 	#pragma unroll 1
@@ -500,42 +498,8 @@ sgm_aggregate_uniform_ring_kernel(const __grid_constant__ SGMParams P, int dir, 
 		uint4 recN = make_uint4(0u, 0u, 0u, 0u); CW cN; AW aN;
 		memset(&cN, 0, sizeof(cN)); memset(&aN, 0, sizeof(aN));
 		if (t+1 < n) fetch(t+1, recN, cN, aN);
-		if (rec.w & 1u) {
-			const float I = __uint_as_float(rec.z);
-			const int P2 = P.P2s[abs((int)floorf(255.f*(I-Ip)+.5f))];
-			Ip = I;
-			uint8_t cb[NPL]; uint16_t ab[NPL];
-			memcpy(cb, &c, NPL); memcpy(ab, &a, 2*NPL);
-			unsigned Ln[NPL];
-			if (!havePrev) {
-				#pragma unroll
-				for (int j = 0; j < NPL; ++j) Ln[j] = j < nval ? (unsigned)(cb[j]+P2) : 0xFFFFu;
-			} else {
-				const unsigned below = __shfl_up_sync(0xFFFFFFFFu, Lp[NPL-1], 1);
-				const unsigned above = __shfl_down_sync(0xFFFFFFFFu, Lp[0], 1);
-				const int far = (int)minLp+P2;
-				#pragma unroll
-				for (int j = 0; j < NPL; ++j) {
-					const int lm = j > 0 ? (int)Lp[j-1] : (lane > 0 ? (int)below : 0xFFFF);
-					const int lq = j < NPL-1 ? (int)Lp[j+1] : (lane < 31 ? (int)above : 0xFFFF);
-					const int best = min(min((int)Lp[j], min(lm, lq)+P.P1), far);
-					Ln[j] = j < nval ? (unsigned)((int)cb[j]+best-(int)minLp) : 0xFFFFu;
-				}
-			}
-			if (active) {
-				#pragma unroll
-				for (int j = 0; j < NPL; ++j) ab[j] = (uint16_t)(ab[j]+(j < nval ? Ln[j] : 0u));
-				const unsigned long long idx = (unsigned long long)rec.x | ((unsigned long long)rec.y<<32);
-				uint2* dst = (uint2*)(P.accums + idx) + lane*(NPL/4);
-				uint2 w0; memcpy(&w0, ab, 8); dst[0] = w0;
-				if (NPL == 8 && nval > 4) { uint2 w1; memcpy(&w1, ab+4, 8); dst[1] = w1; }
-			}
-			unsigned mn = Ln[0];
-			#pragma unroll
-			for (int j = 0; j < NPL; ++j) { Lp[j] = Ln[j]; mn = min(mn, Ln[j]); }
-			minLp = __reduce_min_sync(0xFFFFFFFFu, mn);
-			havePrev = true;
-		}
+		if (rec.w & 1u)
+			path.step(P, __uint_as_float(rec.z), c, a, P.accums + ((unsigned long long)rec.x | ((unsigned long long)rec.y<<32)));
 		rec = recN; c = cN; a = aN;
 	}
 }
@@ -689,7 +653,7 @@ __global__ void sgm_stats_init_kernel(SGMMapStats* out) {
 
 template <int NPL, int E>
 static cudaError_t configure_ring() {
-	return cudaFuncSetAttribute(sgm_aggregate_uniform_ring_kernel<NPL, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2*E*AGG_WARPS*(3*(NPL*32)+24));
+	return cudaFuncSetAttribute(sgm_aggregate_uniform_ring_kernel<NPL, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, AGG_WARPS*ring_warp_bytes(E, NPL*32));
 }
 // dynamic shared memory opt-in of the SGM kernels on the current device (called by b200mvs_create; idempotent)
 cudaError_t sgm_configure_device() {
@@ -713,8 +677,7 @@ static int aggregate_grid(const SGMParams& P, int dir) { return (front_path_coun
 // ring: slices are 16-byte aligned (num % 16 == 0, idx % 16 == 0, aligned base pointers) -> bulk-copy ring kernel
 template <int NPL, int E>
 static cudaError_t launch_ring(const SGMParams& P, int dir, int dmin, int num, int grid, cudaStream_t s) {
-	const size_t smem = (size_t)AGG_WARPS*2*E*(3*(size_t)num+24);
-	sgm_aggregate_uniform_ring_kernel<NPL, E><<<grid, AGG_WARPS*32, smem, s>>>(P, dir, dmin, num);
+	sgm_aggregate_uniform_ring_kernel<NPL, E><<<grid, AGG_WARPS*32, AGG_WARPS*ring_warp_bytes(E, num), s>>>(P, dir, dmin, num);
 	return cudaGetLastError();
 }
 cudaError_t sgm_launch_aggregate_uniform(const SGMParams& P, int dir, int dmin, int num, bool ring, cudaStream_t s) {

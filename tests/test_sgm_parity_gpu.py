@@ -164,11 +164,15 @@ def test_cross_check_and_subpixel_refinement_parity(sgm):
 	assert np.abs(want[valid]/4.0-disp_in[valid]).max() <= 0.5+1e-6  # the offset stays within half a pixel
 
 
-@pytest.mark.parametrize("num", [4, 36, 48, 128, 132, 144, 256])
-def test_uniform_range_fast_path_bit_exact(sgm, num):
+_UNIFORM_CASES = [(num, 0) for num in (4, 36, 48, 128, 132, 144, 192, 256)] + [(num, 2) for num in (48, 128, 144, 192, 256)]
+
+
+@pytest.mark.parametrize("num,mode", _UNIFORM_CASES, ids=[str(n) if mode == 0 else "%d-register" % n for n, mode in _UNIFORM_CASES])
+def test_uniform_range_fast_path_bit_exact(sgm, num, mode):
 	"""One global disparity range (the non-tSGM branch) against the oracle, with some invalid pixels: the packed
 	register-pipelined aggregation kernel (4, 36, 132: slices not 16-byte aligned) and the bulk-copy ring kernel
-	(48, 128: 4 disparities per lane; 144, 256: 8 per lane)."""
+	(48, 128: 4 disparities per lane; 144, 192, 256: 8 per lane), and the register-pipelined kernel forced
+	(sgmAggregation = 2) on the 16-byte aligned widths, so that both kernels run the shared packed step at 4 and 8 per lane."""
 	m, O = sgm
 	w, h = 150, 90
 	rng = np.random.RandomState(num)
@@ -177,7 +181,11 @@ def test_uniform_range_fast_path_bit_exact(sgm, num):
 	costs = rng.randint(0, 256, n).astype(np.uint8)
 	c, a, disp, cost = O.sgm_match(lg, lc, rg, px, n, costs=costs)
 	accums = torch.zeros(n, dtype=torch.int16, device="cuda")
-	gd, gc = m.MatchDevice(_dev(lg), _dev(lc), _dev(rg), _px_dev(px), n, stages=6, costs=_dev(costs), accums=accums)
+	try:
+		m.SetDebug(sgmAggregation=mode)
+		gd, gc = m.MatchDevice(_dev(lg), _dev(lc), _dev(rg), _px_dev(px), n, stages=6, costs=_dev(costs), accums=accums)
+	finally:
+		m.SetDebug()
 	assert np.array_equal(accums.cpu().numpy().view(np.uint16), a)
 	assert np.array_equal(gd.cpu().numpy(), disp) and np.array_equal(gc.cpu().numpy().view(np.uint16), cost)
 
