@@ -524,6 +524,23 @@ int b200mvs_estimate_point_normals_device(b200mvs_ctx* ctx, const float* points,
 /* The exact neighbour search of the normals: per point the min(numNeighbors, nPoints) nearest points, ascending by (squared distance
  * in double, index), into indices (nPoints x min(numNeighbors, nPoints), DEVICE).  points: DEVICE, finite. */
 int b200mvs_point_knn_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, int numNeighbors, uint32_t* indices, void* stream);
+/* The visibility counts of Scene::PointCloudFilter (libs/MVS/SceneDensify.cpp:2226-2360) into visibility (one int32 per point).
+ * For every point X and every view v of X, the cone with apex Cast<float>(C of v), axis through X, half-angle
+ * float(ComputeFOV(0)/width) of v and height 1.02 |X - C| classifies every point P of the cloud (TConeIntersect::Classify); a
+ * VISIBLE P whose distance along the axis differs from |X - C| by 1 % or more gains the size of its own view list when it lies
+ * beyond X and loses the size of X's view list otherwise.  Every point is tested (the reference's octree only skips cells that
+ * cannot intersect), so the counts are those of the single-threaded reference exactly (DESIGN.md §5.7).  Same buffers as the
+ * colour calls; of images only the size and the camera (K, R, C) are read, and the result depends on width, K(0,0) and C alone
+ * (R, height and the rest of K decide which points are searched, never what is counted).  The view lists need not be non-empty:
+ * a point without a view issues no cone but can still be counted.  Every coordinate must be finite; at most 2^31 - 1 points. */
+int b200mvs_point_cloud_visibility(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
+	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int32_t* visibility, b200mvs_stats* stats);
+int b200mvs_point_cloud_visibility_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
+	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int32_t* visibility, void* stream);
+/* The points PointCloudFilter keeps, in the order its removal loop leaves them: RFOREACH(i) if (remove[i]) RemovePoint(i), where
+ * RemovePoint moves the last point into slot i (cList::RemoveAt).  order[k] (n entries of room) is the original index of the point
+ * in slot k afterwards, for k < *nKept.  Host code. */
+int b200mvs_pointcloud_remove_order(const uint8_t* remove, uint64_t n, uint32_t* order, uint64_t* nKept);
 
 #ifdef __cplusplus
 }

@@ -1,6 +1,7 @@
 // cloud_common.cuh — the interface between the point-cloud kernels (cloud_kernels.cu) and their host driver (cloud_host.cu):
-// DepthMapsData::MergeDepthMaps, EstimatePointColors and EstimatePointNormals.  The arithmetic they share with the fusion
-// (compose, image_to_world, normal_to_world, project_row and the correctly rounded helpers) is fuse_common.cuh's.
+// DepthMapsData::MergeDepthMaps, EstimatePointColors, EstimatePointNormals and the visibility counts of Scene::PointCloudFilter.
+// The arithmetic they share with the fusion (compose, image_to_world, normal_to_world, project_row, depth_similar and the
+// correctly rounded helpers) is fuse_common.cuh's.
 #pragma once
 #include <string.h>
 #include "fuse_common.cuh"
@@ -44,6 +45,22 @@ struct CloudGrid {
 	int dim[3];
 };
 
+// Scene::PointCloudFilter (DESIGN.md §5.7): one view v as the visibility kernels see it.  The cones of v share the apex o and
+// cosSq; o, R and K also define the pixel cells its points are binned into (a pinhole at o, so that every point of a cone
+// projects near the projection of the cone's axis).  binned = false: the view is not binned and all its queries test every point.
+constexpr int VIS_CELL = 2;               // pixels per side of a cell
+constexpr int VIS_MARGIN = 16;            // pixels the binned rectangle reaches beyond the image on every side
+struct VisView {
+	float o[3];                   // Cast<float>(C): the apex of the cones
+	float cosSq;                  // SQUARE(COS(angle)), angle = float(ComputeFOV(0)/width), on the host
+	double cosB, sinB;            // a conservative bound beta on the angle between a VISIBLE point and the axis (cloud_host.cu)
+	double R[9];                  // rotation (checked orthonormal when binned)
+	double fx, skew, cx, fy, cy;  // K = [fx skew cx; 0 fy cy; 0 0 1]
+	int w, h, ncx, ncy;           // image size; cells per row and per column of the binned rectangle
+	uint32_t nCells;              // ncx * ncy: the key of a point outside the rectangle
+	bool binned;
+};
+
 cudaError_t cloud_launch_merge_flags(const float* depth, size_t n, uint8_t* flags, unsigned long long* count, cudaStream_t s);
 cudaError_t cloud_launch_merge_bases(const unsigned long long* counts, int nImages, unsigned long long* bases, unsigned long long* total,
 	cudaStream_t s);
@@ -65,3 +82,18 @@ cudaError_t cloud_launch_knn(const float4* sorted, uint32_t n, const uint32_t* c
 	int k, uint32_t* indices, cudaStream_t s);
 cudaError_t cloud_launch_pca(const float* points, uint32_t n, const uint32_t* indices, int k, const uint32_t* offsets,
 	const uint32_t* views, const CloudImage* images, float* normals, cudaStream_t s);
+// the entries of the view lists: entryPoint[j] = the point whose list holds entry j
+cudaError_t cloud_launch_vis_entries(const uint32_t* offsets, uint32_t n, uint32_t* entryPoint, cudaStream_t s);
+// start[k] (k <= nKeys) = the first i with min(keys[i], nKeys) >= k, over n keys sorted ascending (n >= 1)
+cudaError_t cloud_launch_vis_starts(const uint32_t* keys, uint32_t n, uint32_t nKeys, uint32_t* start, cudaStream_t s);
+// the cell of every point in view V (V.nCells when it is not binned) and the identity permutation
+cudaError_t cloud_launch_vis_keys(const VisView& V, const float* points, uint32_t n, uint32_t* keys, uint32_t* idx, cudaStream_t s);
+// the binned points in cell order: (x, y, z, original index) for i < cellStart[V.nCells]
+cudaError_t cloud_launch_vis_gather(const float* points, const uint32_t* idxSorted, uint32_t n, const uint32_t* binnedCount, float4* sorted,
+	cudaStream_t s);
+// The nq queries of view V (query q: point qPoint[q]) over the bins, atomically into visibility; the queries the bins cannot
+// answer are appended to flagged (*nFlagged counts them), then cloud_launch_vis_exhaustive tests every point for them.
+cudaError_t cloud_launch_vis_query(const VisView& V, const uint32_t* qPoint, uint32_t nq, const float* points, const uint32_t* offsets,
+	const float4* sorted, const uint32_t* cellStart, int* visibility, uint32_t* flagged, uint32_t* nFlagged, cudaStream_t s);
+cudaError_t cloud_launch_vis_exhaustive(const VisView& V, const uint32_t* flagged, const uint32_t* nFlagged, uint32_t maxFlagged,
+	const float* points, uint32_t n, const uint32_t* offsets, int* visibility, cudaStream_t s);

@@ -5,7 +5,10 @@
 //  - EstimatePointColors (libs/MVS/DepthMap.cpp:1429-1465): the colour of the closest view, sampled bilinearly.
 //  - EstimatePointNormals (libs/MVS/DepthMap.cpp:1469-1519): PCA over the k nearest points, turned towards the first view.  The
 //    neighbour search is exact (DESIGN.md §5.6): a uniform grid in Morton order and a shell-by-shell search per point.
-// The CPU restatements used by the tests are in oracle/point_cloud_oracle.py.
+//  - Scene::PointCloudFilter (libs/MVS/SceneDensify.cpp:2226-2360): the visibility counts of every (point, view) cone, exactly
+//    those of the single-threaded reference (DESIGN.md §5.7), and the order its removal loop leaves the kept points in.
+// The CPU restatements used by the tests are in oracle/point_cloud_oracle.py and tests/cpp/visibility_oracle.cpp.
+#include <float.h>
 #include <stdint.h>
 #include <string.h>
 #include <math.h>
@@ -208,6 +211,109 @@ int normals_device(b200mvs_ctx* ctx, const float* points, uint32_t n, const uint
 	if (int rc = grid_knn(ctx, G, points, n, g, kk, nbr, cubBytes, s)) return rc;
 	CK(cloud_launch_pca(points, n, nbr, kk, off, views, dImages, normals, s));
 	++ctx->launches;
+	CK(cudaStreamSynchronize(s));
+	return B200MVS_OK;
+}
+
+// The cone parameters of image I and its bins (DESIGN.md §5.7).  angle and cosSq are the reference's expressions in its types
+// (SceneDensify.cpp:2295, Ray.h:209-212): ComputeFOV(0) = 2*atan(width/(2 K(0,0))) in double (Image.cpp:209-216), over width, cast
+// to float; COS is std::cos of that float.
+//
+// beta bounds the angle phi between the axis dir and D = P - o of a point P the kernel classifies VISIBLE.  With u = 2^-24 and the
+// float rounding of each step: |t - dir.D| <= 2u |dir| |D| (the dot product), fl(|D|^2) >= (1 - 2u) |D|^2, and VISIBLE means
+// fl(t^2) > fl(cosSq fl(|D|^2)), so t > sqrt(cosSq) |D| (1 - 2.1u).  The kernel's binned path also requires | |dir|^2 - 1 | <= 16u,
+// so |dir| <= 1 + 8u, and then cos(phi) = dir.D / (|dir| |D|) >= sqrt(cosSq) - 12.1u.  beta = acos(sqrt(cosSq) - 16u), plus 1e-6
+// rad for the rounding of D itself against the exact P - o (at most ~2u) and of the double arithmetic.  The bins need a rotation
+// (angles are kept), K = [fx skew cx; 0 fy cy; 0 0 1], beta below 80 degrees and at most 2^28 cells; otherwise the view is not
+// binned and each of its queries tests every point.
+VisView vis_view(const b200mvs_fuse_view& I) {
+	VisView V;
+	memset(&V, 0, sizeof(V));
+	for (int a = 0; a < 3; ++a) V.o[a] = (float)I.C[a];
+	const float angle = (float)(2*atan((double)I.width/(I.K[0]*2))/I.width);
+	const float c = cosf(angle);
+	V.cosSq = c*c;
+	const double cb = sqrt((double)V.cosSq) - 16.0*FLT_EPSILON/2;
+	const double beta = (cb > -1 ? acos(cb) : M_PI) + 1e-6;
+	V.cosB = cos(beta); V.sinB = sin(beta);
+	memcpy(V.R, I.R, sizeof(V.R));
+	V.fx = I.K[0]; V.skew = I.K[1]; V.cx = I.K[2]; V.fy = I.K[4]; V.cy = I.K[5];
+	V.w = I.width; V.h = I.height;
+	double err = 0;
+	for (int r = 0; r < 3; ++r)
+		for (int s = 0; s < 3; ++s)
+			err = std::max(err, fabs(I.R[r]*I.R[s] + I.R[3+r]*I.R[3+s] + I.R[6+r]*I.R[6+s] - (r == s)));
+	const double ncx = ceil((I.width + 2.0*VIS_MARGIN)/VIS_CELL), ncy = ceil((I.height + 2.0*VIS_MARGIN)/VIS_CELL);
+	bool finite = true;
+	for (int a = 0; a < 9; ++a) finite &= std::isfinite(I.K[a]);
+	V.binned = err <= 1e-9 && finite && I.K[3] == 0 && I.K[6] == 0 && I.K[7] == 0 && I.K[8] == 1 && beta < 80*M_PI/180 &&
+		ncx*ncy <= (double)(1u << 28);
+	if (V.binned) { V.ncx = (int)ncx; V.ncy = (int)ncy; V.nCells = (uint32_t)(ncx*ncy); }
+	return V;
+}
+
+// the number of key bits of a radix sort of keys up to maxKey
+int key_bits(uint32_t maxKey) {
+	int b = 1;
+	while (b < 32 && (maxKey >> b)) ++b;
+	return b;
+}
+
+// PointCloudFilter's visibility counts on device buffers: the queries (the entries of the view lists) sorted by view, then per
+// view with queries: bin every point by its cell, sort the bins, answer the queries from the bins and the flagged ones by testing
+// every point.  One carve of the call's scratch, one read-back of the per-view query ranges.
+int visibility_device(b200mvs_ctx* ctx, const float* points, uint32_t n, const uint32_t* off, const uint32_t* views,
+	const b200mvs_fuse_view* images, int nImages, int32_t* visibility, cudaStream_t s)
+{
+	for (int i = 0; i < nImages; ++i)
+		if (images[i].width <= 0 || images[i].height <= 0) return fail(ctx, B200MVS_ERR_ARG, "point visibility: image size out of range");
+	float box[6];
+	if (int rc = cloud_check(ctx, points, n, off, views, nImages, false, box, nullptr, s)) return rc;
+	uint32_t nEntries = 0;
+	CK(cudaMemcpyAsync(&nEntries, off + n, sizeof(nEntries), cudaMemcpyDeviceToHost, s));
+	CK(cudaMemsetAsync(visibility, 0, sizeof(int32_t)*n, s));
+	CK(cudaStreamSynchronize(s));
+	if (nEntries == 0) return B200MVS_OK;
+	std::vector<VisView> V(nImages);
+	uint32_t maxCells = 0;
+	for (int i = 0; i < nImages; ++i) { V[i] = vis_view(images[i]); maxCells = std::max(maxCells, V[i].nCells); }
+	// CUB's temporary storage for both sorts, reserved before the first launch of the call's work
+	const int viewBits = key_bits((uint32_t)std::max(nImages-1, 0)), cellBits = key_bits(maxCells);
+	size_t bytesViews = 0, bytesCells = 0;
+	CK(fuse_sort(nullptr, bytesViews, nullptr, nullptr, nullptr, nullptr, nEntries, viewBits, nullptr));
+	CK(fuse_sort(nullptr, bytesCells, nullptr, nullptr, nullptr, nullptr, n, cellBits, nullptr));
+	CK(ctx->pcCub.reserve(std::max<size_t>(std::max(bytesViews, bytesCells), 1)));
+	size_t cubBytes = ctx->pcCub.cap;
+	Carve scratch(ctx->pcScratch);
+	uint32_t *entryPoint, *viewSorted, *qPoint, *viewStart, *keys, *keysSorted, *idx, *idxSorted, *cellStart, *flagged, *nFlagged;
+	float4* sorted;
+	scratch.take(entryPoint, nEntries); scratch.take(viewSorted, nEntries); scratch.take(qPoint, nEntries);
+	scratch.take(viewStart, nImages+1); scratch.take(flagged, nEntries); scratch.take(nFlagged, 1);
+	scratch.take(keys, n); scratch.take(keysSorted, n); scratch.take(idx, n); scratch.take(idxSorted, n); scratch.take(sorted, n);
+	scratch.take(cellStart, (size_t)maxCells+1);
+	CK(scratch.commit());
+	CK(cloud_launch_vis_entries(off, n, entryPoint, s));
+	CK(fuse_sort(ctx->pcCub.p, cubBytes, views, viewSorted, entryPoint, qPoint, nEntries, viewBits, s));
+	CK(cloud_launch_vis_starts(viewSorted, nEntries, (uint32_t)nImages, viewStart, s));
+	ctx->launches += 3;
+	std::vector<uint32_t> start(nImages+1);
+	CK(cudaMemcpyAsync(start.data(), viewStart, sizeof(uint32_t)*(nImages+1), cudaMemcpyDeviceToHost, s));
+	CK(cudaStreamSynchronize(s));
+	for (int v = 0; v < nImages; ++v) {
+		const uint32_t nq = start[v+1] - start[v];
+		if (!nq) continue;
+		CK(cudaMemsetAsync(nFlagged, 0, sizeof(uint32_t), s));
+		if (V[v].binned) {
+			CK(cloud_launch_vis_keys(V[v], points, n, keys, idx, s));
+			CK(fuse_sort(ctx->pcCub.p, cubBytes, keys, keysSorted, idx, idxSorted, n, cellBits, s));
+			CK(cloud_launch_vis_starts(keysSorted, n, V[v].nCells, cellStart, s));
+			CK(cloud_launch_vis_gather(points, idxSorted, n, cellStart + V[v].nCells, sorted, s));
+			ctx->launches += 4;
+		}
+		CK(cloud_launch_vis_query(V[v], qPoint + start[v], nq, points, off, sorted, cellStart, visibility, flagged, nFlagged, s));
+		CK(cloud_launch_vis_exhaustive(V[v], flagged, nFlagged, nq, points, n, off, visibility, s));
+		ctx->launches += 2;
+	}
 	CK(cudaStreamSynchronize(s));
 	return B200MVS_OK;
 }
@@ -421,6 +527,48 @@ int b200mvs_estimate_point_normals(b200mvs_ctx* ctx, const float* points, uint64
 	return call.run([&](cudaStream_t s) {
 		return normals_device(ctx, dPoints, (uint32_t)nPoints, dOff, dViews, images, nImages, numNeighbors, dNormals, s);
 	}, stats);
+}
+
+int b200mvs_point_cloud_visibility_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
+	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int32_t* visibility, void* stream)
+{
+	if (int rc = cloud_args(ctx, points, nPoints, viewOffsets, views, images, nImages, visibility)) return rc;
+	if (nPoints == 0) return B200MVS_OK;
+	CK(cudaSetDevice(ctx->device));
+	if (!on_device(ctx, points) || !on_device(ctx, viewOffsets) || !on_device(ctx, views) || !on_device(ctx, visibility))
+		return fail(ctx, B200MVS_ERR_ARG, "point visibility: a buffer is not in device memory of the context's device");
+	ctx->launches = 0;
+	return visibility_device(ctx, points, (uint32_t)nPoints, viewOffsets, views, images, nImages, visibility, stream_of(ctx, stream));
+}
+
+int b200mvs_point_cloud_visibility(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
+	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int32_t* visibility, b200mvs_stats* stats)
+{
+	if (int rc = cloud_args(ctx, points, nPoints, viewOffsets, views, images, nImages, visibility)) return rc;
+	if (nPoints == 0) return stats ? (memset(stats, 0, sizeof(*stats)), B200MVS_OK) : B200MVS_OK;
+	if (int rc = check_views_host(ctx, viewOffsets, views, nPoints, nImages, false)) return rc;
+	CK(cudaSetDevice(ctx->device));
+	ctx->launches = 0;
+	HostCall call(ctx);
+	const float* dPoints; const uint32_t *dOff, *dViews; int32_t* dVis;
+	call.in(dPoints, points, 12*nPoints); call.in(dOff, viewOffsets, 4*(nPoints+1)); call.in(dViews, views, 4*(size_t)viewOffsets[nPoints]);
+	call.out(dVis, visibility, 4*nPoints);
+	if (int rc = call.stage()) return rc;
+	return call.run([&](cudaStream_t s) {
+		return visibility_device(ctx, dPoints, (uint32_t)nPoints, dOff, dViews, images, nImages, dVis, s);
+	}, stats);
+}
+
+int b200mvs_pointcloud_remove_order(const uint8_t* remove, uint64_t n, uint32_t* order, uint64_t* nKept) {
+	if (!nKept || n > 0xFFFFFFFFull || (n && (!remove || !order))) return B200MVS_ERR_ARG;
+	// RFOREACH(i, points) if (remove[i]) RemovePoint(i): slot i still holds point i when the loop reaches it, and RemoveAt moves
+	// the last point into it
+	uint64_t size = n;
+	for (uint64_t i = 0; i < n; ++i) order[i] = (uint32_t)i;
+	for (uint64_t i = n; i-- > 0; )
+		if (remove[i]) order[i] = order[--size];
+	*nKept = size;
+	return B200MVS_OK;
 }
 
 int b200mvs_point_knn_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, int numNeighbors, uint32_t* indices, void* stream) {

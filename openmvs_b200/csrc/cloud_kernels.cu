@@ -1,5 +1,6 @@
 // cloud_kernels.cu — the point-cloud tail of the densification on the device (host driver: cloud_host.cu): MergeDepthMaps,
-// EstimatePointColors, and the exact k-nearest-neighbour search and PCA of EstimatePointNormals (DESIGN.md §5.6).
+// EstimatePointColors, the exact k-nearest-neighbour search and PCA of EstimatePointNormals (DESIGN.md §5.6), and the visibility
+// counts of PointCloudFilter (§5.7).
 #include <cfloat>
 #include <cub/cub.cuh>
 #include "cloud_common.cuh"
@@ -321,6 +322,151 @@ __global__ void __launch_bounds__(TPB) k_pca(const float* __restrict__ pts, uint
 	for (int a = 0; a < 3; ++a) normals[3*(size_t)i+a] = nf[a];
 }
 
+// ---- PointCloudFilter (libs/MVS/SceneDensify.cpp:2226-2360): the visibility counts ----
+
+// Eigen's sum of three terms (Redux.h, redux_novec_unroller halves the range): a0 + (a1 + a2), as in VECTOR::dot and squaredNorm
+__device__ __forceinline__ float sum3(float a0, float a1, float a2) { return fuse::add_f(a0, fuse::add_f(a1, a2)); }
+
+// One cone: Collector::Init (SceneDensify.cpp:2258-2266) for point X and its view list of `weight` entries
+struct VisCone {
+	float dir[3], distance, maxHeight;
+	int weight;
+};
+
+__device__ __forceinline__ void vis_cone(const VisView& V, const float* __restrict__ X, int weight, VisCone& c) {
+	const float D0 = fuse::sub_f(X[0], V.o[0]), D1 = fuse::sub_f(X[1], V.o[1]), D2 = fuse::sub_f(X[2], V.o[2]);
+	c.distance = fuse::sqrt_f(sum3(fuse::mul_f(D0, D0), fuse::mul_f(D1, D1), fuse::mul_f(D2, D2)));
+	c.dir[0] = fuse::div_f(D0, c.distance); c.dir[1] = fuse::div_f(D1, c.distance); c.dir[2] = fuse::div_f(D2, c.distance);
+	c.maxHeight = fuse::mul_f(c.distance, 1.02f);   // MaxDepthDifference (libs/Common/Util.inl:790)
+	c.weight = weight;
+}
+
+// Collector::operator() on point P (index idx): TConeIntersect::Classify (libs/Common/Ray.inl:905-920), then IsDepthSimilar with
+// 0.01; a VISIBLE point that is not similar gains the size of its own view list beyond X and loses the weight of X before it
+__device__ __forceinline__ void vis_count(const VisView& V, const VisCone& c, float px, float py, float pz, uint32_t idx,
+	const uint32_t* __restrict__ off, int* __restrict__ vis)
+{
+	const float D0 = fuse::sub_f(px, V.o[0]), D1 = fuse::sub_f(py, V.o[1]), D2 = fuse::sub_f(pz, V.o[2]);
+	const float t = sum3(fuse::mul_f(c.dir[0], D0), fuse::mul_f(c.dir[1], D1), fuse::mul_f(c.dir[2], D2));
+	if (fabsf(t) < 0.0001f || t < 0.f || t > c.maxHeight) return;   // PLANAR (ISZERO), BACK, FRONT
+	const float tSq = fuse::mul_f(t, t);
+	const float dSq = fuse::mul_f(V.cosSq, sum3(fuse::mul_f(D0, D0), fuse::mul_f(D1, D1), fuse::mul_f(D2, D2)));
+	if (!(tSq > dSq)) return;                                         // CULLED or PLANAR
+	if (fuse::depth_similar(c.distance, t, 0.01f)) return;
+	atomicAdd(vis + idx, t > c.distance ? (int)(off[idx+1] - off[idx]) : -c.weight);
+}
+
+// The pixel of P in the binning camera of V (a pinhole at the apex o): false when P is behind it or outside the binned rectangle
+__device__ __forceinline__ bool vis_pixel(const VisView& V, const float* p, double& u, double& v) {
+	const double d0 = (double)p[0] - V.o[0], d1 = (double)p[1] - V.o[1], d2 = (double)p[2] - V.o[2];
+	const double x = V.R[0]*d0 + V.R[1]*d1 + V.R[2]*d2, y = V.R[3]*d0 + V.R[4]*d1 + V.R[5]*d2, z = V.R[6]*d0 + V.R[7]*d1 + V.R[8]*d2;
+	if (!(z > 0)) return false;
+	const double nx = x/z, ny = y/z;
+	u = V.fx*nx + V.skew*ny + V.cx; v = V.fy*ny + V.cy;
+	return u >= -VIS_MARGIN && u < V.w + VIS_MARGIN && v >= -VIS_MARGIN && v < V.h + VIS_MARGIN;
+}
+
+__device__ __forceinline__ int vis_cell(double u) { return (int)floor((u + VIS_MARGIN)*(1.0/VIS_CELL)); }
+
+// The cells a cone's VISIBLE points can lie in: columns [cx0, cx1] of rows [cy0, cy1]; false when the bins cannot answer the cone.
+//
+// Bound.  Let d be the unit axis in camera space, at angle theta to the optical axis e, and u the unit direction of a VISIBLE point
+// P from the apex, at angle phi <= beta to d (beta: the host's bound on phi, cloud_host.cu vis_view).  If theta + beta < 90 deg,
+// the normalised image points p(u) = u_xy/u_z and p(d) = d_xy/d_z satisfy
+//     |p(u) - p(d)| = |u_xy d_z - d_xy u_z| / (u_z d_z) <= |u x d| / (u_z d_z) <= sin(beta) / (cos(theta) cos(theta + beta))
+// because (u_xy d_z - d_xy u_z) is, up to sign and order, the xy part of u x d, |u x d| = sin(phi) <= sin(beta), d_z = cos(theta)
+// and u_z = cos(angle(u, e)) >= cos(theta + beta) by the triangle inequality of angles.  (It equals tan(theta + beta) - tan(theta).)
+// The pixel offset is K's upper-left 2x2 block times p(u) - p(d): at most (|fx| + |skew|) rho across and |fy| rho down.  One pixel
+// more absorbs the double rounding of both projections (relative 1e-16).  A cone with theta + beta near 90 deg, a degenerate
+// cone (distance 0 or infinite: then nothing is VISIBLE anyway) or one whose rectangle leaves the binned rectangle is flagged.
+__device__ __forceinline__ bool vis_cells(const VisView& V, const VisCone& c, int& cx0, int& cx1, int& cy0, int& cy1) {
+	if (!V.binned) return false;
+	const double d0 = c.dir[0], d1 = c.dir[1], d2 = c.dir[2], n2 = d0*d0 + d1*d1 + d2*d2;
+	if (!(fabs(n2 - 1.0) <= 8.0*FLT_EPSILON)) return false;    // |dir|^2 within 16 u of 1, as the bound on beta assumes
+	const double ax = V.R[0]*d0 + V.R[1]*d1 + V.R[2]*d2, ay = V.R[3]*d0 + V.R[4]*d1 + V.R[5]*d2, az = V.R[6]*d0 + V.R[7]*d1 + V.R[8]*d2;
+	const double cosT = az/sqrt(n2), sinT = sqrt(fmax(0.0, 1.0 - cosT*cosT));
+	const double cosTB = cosT*V.cosB - sinT*V.sinB;             // cos(theta + beta)
+	if (!(cosT > 0.1 && cosTB > 0.1)) return false;              // theta + beta beyond 84 deg
+	const double rho = V.sinB/(cosT*cosTB);
+	const double u = V.fx*(ax/az) + V.skew*(ay/az) + V.cx, v = V.fy*(ay/az) + V.cy;
+	const double rx = (fabs(V.fx) + fabs(V.skew))*rho + 1.0, ry = fabs(V.fy)*rho + 1.0;
+	if (!(u - rx >= -VIS_MARGIN && u + rx < V.w + VIS_MARGIN && v - ry >= -VIS_MARGIN && v + ry < V.h + VIS_MARGIN)) return false;
+	cx0 = max(vis_cell(u - rx), 0); cx1 = min(vis_cell(u + rx), V.ncx - 1);
+	cy0 = max(vis_cell(v - ry), 0); cy1 = min(vis_cell(v + ry), V.ncy - 1);
+	return true;
+}
+
+__global__ void k_vis_entries(const uint32_t* __restrict__ off, uint32_t n, uint32_t* __restrict__ entryPoint) {
+	const uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	for (uint32_t j = off[i], e = off[i+1]; j < e; ++j) entryPoint[j] = i;
+}
+
+// every thread fills the starts of the keys from its predecessor's (exclusive) to its own (inclusive); the last one the rest
+__global__ void k_vis_starts(const uint32_t* __restrict__ keys, uint32_t n, uint32_t nKeys, uint32_t* __restrict__ start) {
+	const uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const uint32_t k = min(keys[i], nKeys);
+	for (uint32_t j = i ? min(keys[i-1], nKeys) + 1 : 0; j <= k; ++j) start[j] = i;
+	if (i == n-1) for (uint32_t j = k + 1; j <= nKeys; ++j) start[j] = n;
+}
+
+__global__ void k_vis_keys(const VisView V, const float* __restrict__ pts, uint32_t n, uint32_t* __restrict__ keys, uint32_t* __restrict__ idx) {
+	const uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	double u, v;
+	const bool in = vis_pixel(V, pts + 3*(size_t)i, u, v);
+	keys[i] = in ? (uint32_t)min(vis_cell(v), V.ncy - 1)*V.ncx + min(vis_cell(u), V.ncx - 1) : V.nCells;
+	idx[i] = i;
+}
+
+__global__ void k_vis_gather(const float* __restrict__ pts, const uint32_t* __restrict__ idxSorted, uint32_t n, const uint32_t* binned,
+	float4* __restrict__ sorted)
+{
+	const uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
+	if (i >= n || i >= *binned) return;
+	const uint32_t o = idxSorted[i];
+	sorted[i] = make_float4(pts[3*(size_t)o], pts[3*(size_t)o+1], pts[3*(size_t)o+2], __uint_as_float(o));
+}
+
+// One warp per query: the lanes stride over the binned points of each cell row of the cone's rectangle (one contiguous range per
+// row, since the keys are row-major), so a warp's loads are coalesced and all its lanes run the same trip count.
+__global__ void __launch_bounds__(TPB) k_vis_query(const VisView V, const uint32_t* __restrict__ qPoint, uint32_t nq,
+	const float* __restrict__ pts, const uint32_t* __restrict__ off, const float4* __restrict__ sorted,
+	const uint32_t* __restrict__ cellStart, int* __restrict__ vis, uint32_t* __restrict__ flagged, uint32_t* nFlagged)
+{
+	const uint32_t q = (blockIdx.x*blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+	if (q >= nq) return;
+	const uint32_t i = qPoint[q];
+	VisCone c;
+	vis_cone(V, pts + 3*(size_t)i, (int)(off[i+1] - off[i]), c);
+	int cx0, cx1, cy0, cy1;
+	if (!vis_cells(V, c, cx0, cx1, cy0, cy1)) {
+		if (lane == 0) flagged[atomicAdd(nFlagged, 1u)] = i;
+		return;
+	}
+	for (int cy = cy0; cy <= cy1; ++cy) {
+		const uint32_t row = (uint32_t)cy*V.ncx;
+		for (uint32_t s = cellStart[row + cx0] + lane, e = cellStart[row + cx1 + 1]; s < e; s += 32) {
+			const float4 p = sorted[s];
+			vis_count(V, c, p.x, p.y, p.z, __float_as_uint(p.w), off, vis);
+		}
+	}
+}
+
+// One block per flagged query (grid-stride over the list): its threads test every point of the cloud
+__global__ void __launch_bounds__(TPB) k_vis_exhaustive(const VisView V, const uint32_t* __restrict__ flagged, const uint32_t* nFlagged,
+	const float* __restrict__ pts, uint32_t n, const uint32_t* __restrict__ off, int* __restrict__ vis)
+{
+	for (uint32_t f = blockIdx.x; f < *nFlagged; f += gridDim.x) {
+		const uint32_t i = flagged[f];
+		VisCone c;
+		vis_cone(V, pts + 3*(size_t)i, (int)(off[i+1] - off[i]), c);
+		for (uint32_t j = threadIdx.x; j < n; j += blockDim.x)
+			vis_count(V, c, pts[3*(size_t)j], pts[3*(size_t)j+1], pts[3*(size_t)j+2], j, off, vis);
+	}
+}
+
 } // namespace
 
 cudaError_t cloud_launch_merge_flags(const float* depth, size_t n, uint8_t* flags, unsigned long long* count, cudaStream_t s) {
@@ -392,5 +538,42 @@ cudaError_t cloud_launch_pca(const float* points, uint32_t n, const uint32_t* in
 	const uint32_t* views, const CloudImage* images, float* normals, cudaStream_t s)
 {
 	k_pca<<<blocks(n), TPB, 0, s>>>(points, n, indices, k, offsets, views, images, normals);
+	return cudaGetLastError();
+}
+
+cudaError_t cloud_launch_vis_entries(const uint32_t* offsets, uint32_t n, uint32_t* entryPoint, cudaStream_t s) {
+	k_vis_entries<<<blocks(n), TPB, 0, s>>>(offsets, n, entryPoint);
+	return cudaGetLastError();
+}
+
+cudaError_t cloud_launch_vis_starts(const uint32_t* keys, uint32_t n, uint32_t nKeys, uint32_t* start, cudaStream_t s) {
+	k_vis_starts<<<blocks(n), TPB, 0, s>>>(keys, n, nKeys, start);
+	return cudaGetLastError();
+}
+
+cudaError_t cloud_launch_vis_keys(const VisView& V, const float* points, uint32_t n, uint32_t* keys, uint32_t* idx, cudaStream_t s) {
+	k_vis_keys<<<blocks(n), TPB, 0, s>>>(V, points, n, keys, idx);
+	return cudaGetLastError();
+}
+
+cudaError_t cloud_launch_vis_gather(const float* points, const uint32_t* idxSorted, uint32_t n, const uint32_t* binnedCount, float4* sorted,
+	cudaStream_t s)
+{
+	k_vis_gather<<<blocks(n), TPB, 0, s>>>(points, idxSorted, n, binnedCount, sorted);
+	return cudaGetLastError();
+}
+
+cudaError_t cloud_launch_vis_query(const VisView& V, const uint32_t* qPoint, uint32_t nq, const float* points, const uint32_t* offsets,
+	const float4* sorted, const uint32_t* cellStart, int* visibility, uint32_t* flagged, uint32_t* nFlagged, cudaStream_t s)
+{
+	k_vis_query<<<blocks(32*(size_t)nq), TPB, 0, s>>>(V, qPoint, nq, points, offsets, sorted, cellStart, visibility, flagged, nFlagged);
+	return cudaGetLastError();
+}
+
+cudaError_t cloud_launch_vis_exhaustive(const VisView& V, const uint32_t* flagged, const uint32_t* nFlagged, uint32_t maxFlagged,
+	const float* points, uint32_t n, const uint32_t* offsets, int* visibility, cudaStream_t s)
+{
+	// the count stays on the device: enough blocks for every SM, each taking flagged queries in turn
+	k_vis_exhaustive<<<std::max(std::min(maxFlagged, 4096u), 1u), TPB, 0, s>>>(V, flagged, nFlagged, points, n, offsets, visibility);
 	return cudaGetLastError();
 }

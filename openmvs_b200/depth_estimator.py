@@ -946,7 +946,8 @@ def FuseRoundStats():
 
 # The point-cloud calls after the fusion live in point_cloud.py, which builds on this module; they are re-exported here on first
 # use, so that either module can be imported first.
-_POINT_CLOUD_CALLS = ("MergeDepthMaps", "EstimatePointColors", "EstimatePointNormals", "PointKNN")
+_POINT_CLOUD_CALLS = ("MergeDepthMaps", "EstimatePointColors", "EstimatePointNormals", "PointKNN", "PointCloudVisibility",
+	"PointCloudFilter")
 
 
 def __getattr__(name):

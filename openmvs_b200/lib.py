@@ -172,6 +172,9 @@ PROTOTYPES = {
 	"b200mvs_estimate_point_normals": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, I, P, PStats]),
 	"b200mvs_estimate_point_normals_device": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, I, P, P]),
 	"b200mvs_point_knn_device": (I, [P, P, U64, I, P, P]),
+	"b200mvs_point_cloud_visibility": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, P, PStats]),
+	"b200mvs_point_cloud_visibility_device": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, P, P]),
+	"b200mvs_pointcloud_remove_order": (I, [P, U64, P, C.POINTER(U64)]),
 }
 SYMBOLS = list(PROTOTYPES)
 

@@ -1,10 +1,12 @@
 """The point cloud after the fusion: DepthMapsData::MergeDepthMaps (libs/MVS/SceneDensify.cpp:1305-1366), EstimatePointColors
-(libs/MVS/DepthMap.cpp:1429-1465) and EstimatePointNormals (libs/MVS/DepthMap.cpp:1469-1519), and the exact k-NN search of the
-normals, above the C-ABI (include/b200mvs.h); the kernels are openmvs_b200/csrc/cloud_kernels.cu.  Re-exported by
-depth_estimator.  numpy inputs take the host forms, CUDA tensors the device forms on the context kept per device."""
+(libs/MVS/DepthMap.cpp:1429-1465), EstimatePointNormals (libs/MVS/DepthMap.cpp:1469-1519) with the exact k-NN search of the
+normals, and Scene::PointCloudFilter (libs/MVS/SceneDensify.cpp:2226-2360), above the C-ABI (include/b200mvs.h); the kernels are
+openmvs_b200/csrc/cloud_kernels.cu.  Re-exported by depth_estimator.  numpy inputs take the host forms, CUDA tensors the device
+forms on the context kept per device."""
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 
 import numpy as np
 
@@ -138,3 +140,76 @@ def PointKNN(points, numNeighbors: int = 16):
 	out = torch.empty((n, max(min(int(numNeighbors), n), 0)), dtype=torch.int32, device=points.device)
 	ctx._call("point_knn_device", ptr, n, int(numNeighbors), out.data_ptr() if n else None, _stream_handle(ctx.device))
 	return out
+
+
+def PointCloudVisibility(views, pointcloud: PointCloud):
+	"""The visibility counts of Scene::PointCloudFilter (libs/MVS/SceneDensify.cpp:2226-2360): for every point and every view of
+	it, the cone from the view's camera centre through the point with a half-angle of one pixel classifies every point of the
+	cloud, and each VISIBLE point at least 1 % farther (nearer) along the axis than the apex-to-point distance gains the size of
+	its own view list (loses the size of the point's view list).  Exactly the counts of the single-threaded reference
+	(DESIGN.md §5.7).  views: the scene images as dicts with K, R, C and their size, given as width and height or by a depth or
+	colour map (only the size and the camera are read).  -> (n,) int32: a numpy array for numpy points (host-buffer form), a
+	tensor on the points' device for CUDA points (device form)."""
+	return _visibility("PointCloudVisibility", views, pointcloud)
+
+
+def _visibility(where: str, views, pointcloud: PointCloud):
+	rows = len(pointcloud.points) if hasattr(pointcloud.points, "__len__") else None
+	if rows is not None and rows != len(pointcloud.pointViews):
+		raise ValueError("%s: pointcloud.points must have one row per view list; got %d rows and %d lists" % (where, rows,
+			len(pointcloud.pointViews)))
+	device, ctx, args, keep = _cloud_args(where, views, pointcloud, ())
+	table = args[4]
+	for i, v in enumerate(views):
+		if v.get("width") is not None and v.get("height") is not None:
+			size = (v["height"], v["width"])
+		else:
+			m = next((v[k] for k in ("depth", "color") if v.get(k) is not None), None)
+			if m is None:
+				raise ValueError("%s: views[%d] needs width and height, or a depth or colour map to take them from" % (where, i))
+			size = tuple(m.shape[:2])
+		if not all(isinstance(s, (int, np.integer)) and 0 < int(s) < 2**31 for s in size):
+			raise ValueError("%s: views[%d] width and height must be positive integers; got %r" % (where, i, size[::-1]))
+		table[i].height, table[i].width = int(size[0]), int(size[1])
+	n = args[1]
+	if device is None:
+		vis = np.zeros(n, np.int32)
+		ctx = _device_context(0)
+		ctx._call("point_cloud_visibility", *args, vis.ctypes.data, C.byref(ctx.stats))
+	else:
+		import torch
+		vis = torch.empty(n, dtype=torch.int32, device=pointcloud.points.device)
+		ctx._call("point_cloud_visibility_device", *args, vis.data_ptr(), _stream_handle(ctx.device))
+	return vis
+
+
+def PointCloudFilter(views, pointcloud: PointCloud, thRemove: int = 0) -> PointCloud:
+	"""Scene::PointCloudFilter(thRemove) (libs/MVS/SceneDensify.cpp:2226-2360): the cloud without the points whose visibility
+	count (PointCloudVisibility) is <= thRemove, in the order the reference's removal loop leaves them (from the last point down,
+	each removed point replaced by the current last one: b200mvs_pointcloud_remove_order).  points, pointViews, pointWeights,
+	colors, normals and projs are reordered alike, where present; a CUDA cloud stays on its device.  -> a new PointCloud."""
+	if isinstance(thRemove, bool) or not isinstance(thRemove, (int, np.integer)) or not -2**31 <= int(thRemove) < 2**31:
+		raise ValueError("PointCloudFilter: thRemove must be an int32 integer; got %r" % (thRemove,))
+	vis = _visibility("PointCloudFilter", views, pointcloud)
+	remove = vis <= int(thRemove)
+	remove = np.ascontiguousarray(remove.cpu().numpy() if _is_torch(remove) else remove, np.uint8)
+	n = len(remove)
+	order = np.zeros(max(n, 1), np.uint32)
+	kept = C.c_uint64()
+	rc = _lib.load().b200mvs_pointcloud_remove_order(remove.ctypes.data, n, order.ctypes.data, C.byref(kept))
+	if rc:
+		raise _lib.B200MVSError("b200mvs_pointcloud_remove_order failed with status %d" % rc)
+	order = order[:kept.value].astype(np.int64)
+
+	def take(a):
+		if a is None:
+			return None
+		if isinstance(a, list):
+			return [a[k] for k in order]
+		if _is_torch(a):
+			import torch
+			return a[torch.from_numpy(order).to(a.device)]
+		return np.asarray(a)[order]
+	return dataclasses.replace(pointcloud, points=take(pointcloud.points), pointViews=take(pointcloud.pointViews),
+		pointWeights=take(pointcloud.pointWeights), colors=take(pointcloud.colors), normals=take(pointcloud.normals),
+		projs=take(pointcloud.projs))

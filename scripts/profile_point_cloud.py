@@ -1,5 +1,5 @@
-"""The point-cloud tail on 12 views at 1920x1080 with 9 neighbours each: MergeDepthMaps (device form), EstimatePointColors and
-EstimatePointNormals (k = 16) on the fused and on the merged cloud.
+"""The point-cloud tail on 12 views at 1920x1080 with 9 neighbours each: MergeDepthMaps (device form), EstimatePointColors,
+EstimatePointNormals (k = 16) and the visibility counts of PointCloudFilter on the fused and on the merged cloud.
 
   python scripts/profile_point_cloud.py [--width W] [--height H] [--iters N] [--subset M] [--out FILE]
 
@@ -8,8 +8,10 @@ time of the merge (its events, without the read-back of the cloud), of the colou
 call on device buffers, which includes its checks' read-back), best of --iters runs after one warm-up, on the fused cloud, the
 merged cloud and the fused cloud with 16 far outliers; the normals split into grid build (checks, bounding box, sample, keys,
 sort, cells), k-NN and PCA from the kernel times under torch.profiler, each the best of --iters profiled runs after a warm-up;
-the numpy ORACLE's time for the normals of --subset points (brute-force k-NN and PCA, scaled per point), which is not the
-reference (CGAL); and the card name and power limit (read-only nvidia-smi query)."""
+the visibility counts' device time (CUDA events around the call on device buffers), best of --iters runs after one warm-up, with
+its split into checks, binning (query sort, per-view keys, sorts, cell starts, gather) and queries (binned and exhaustive) from
+the kernel times under torch.profiler, and the queries (entries of the view lists) per second; the numpy ORACLE's time for the
+normals of --subset points (brute-force k-NN and PCA, scaled per point), which is not the reference (CGAL); and the card name and power limit (read-only nvidia-smi query)."""
 import argparse
 import ctypes as C
 import json
@@ -116,6 +118,30 @@ def split(fn, iters):
 	return {k: round(v, 3) for k, v in best.items()}
 
 
+def split_visibility(fn, iters):
+	"""device ms of the visibility call's checks, binning and query kernels, each the best of iters profiled runs after a warm-up"""
+	from torch.profiler import ProfilerActivity, profile
+	fn(); torch.cuda.synchronize()
+	keys = ("checks", "binning", "queries", "exhaustive")
+	best = dict.fromkeys(keys, float("inf"))
+	for _ in range(iters):
+		with profile(activities=[ProfilerActivity.CUDA]) as prof:
+			fn(); torch.cuda.synchronize()
+		out = dict.fromkeys(keys, 0.0)
+		for e in prof.key_averages():
+			name, ms = e.key, e.device_time_total/1000.0 if hasattr(e, "device_time_total") else e.cuda_time_total/1000.0
+			if "k_vis_query" in name:
+				out["queries"] += ms
+			elif "k_vis_exhaustive" in name:
+				out["exhaustive"] += ms
+			elif any(s in name for s in ("k_vis_entries", "k_vis_starts", "k_vis_keys", "k_vis_gather", "RadixSort", "Onesweep")):
+				out["binning"] += ms
+			elif any(s in name for s in ("k_check_views", "k_bbox", "Memset", "memset")):
+				out["checks"] += ms
+		best = {k: min(best[k], out[k]) for k in keys}
+	return {k: round(v, 3) for k, v in best.items()}
+
+
 def main():
 	ap = argparse.ArgumentParser()
 	ap.add_argument("--width", type=int, default=1920)
@@ -156,6 +182,16 @@ def main():
 		run = lambda: ctx._call("estimate_point_normals_device", *args, 16, normals.data_ptr(), stream)
 		row["ms_normals_"+label] = timed(run, a.iters)
 		row["normals_split_ms_"+label] = split(run, a.iters)
+		if label == "fused_outliers":
+			continue
+		vis = torch.empty(n, dtype=torch.int32, device="cuda")
+		run = lambda: ctx._call("point_cloud_visibility_device", *args, vis.data_ptr(), stream)
+		row["ms_visibility_"+label] = timed(run, a.iters)
+		row["visibility_split_ms_"+label] = split_visibility(run, a.iters)
+		row["visibility_queries_"+label] = int(off[-1])
+		row["visibility_queries_per_s_"+label] = int(off[-1])/(row["ms_visibility_"+label]/1000.0)
+		v = vis.cpu().numpy()
+		row["visibility_removed_at_0_"+label] = int((v <= 0).sum())
 	# the numpy oracle on a subset: brute force over the whole fused cloud for --subset queries, then PCA
 	X = fused[0]
 	rng = np.random.RandomState(0)

@@ -1,6 +1,6 @@
 """Small PatchMatch (photometric, multi-scale, geometric) + SGM + post-processing runs for compute-sanitizer.
 SANITIZE_ONLY=post runs the post-processing part alone."""
-import os, sys
+import copy, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 from openmvs_b200 import synth
@@ -62,3 +62,14 @@ EstimatePointColors(pv, pc); EstimatePointNormals(pv, pc)
 pc.points = torch.from_numpy(pc.points).cuda()
 EstimatePointColors([dict(v, color=torch.from_numpy(v["color"]).cuda()) for v in pv], pc); EstimatePointNormals(pv, pc, 32)
 print("point cloud", len(pc.points), "knn", tuple(PointKNN(pc.points, 16).shape))
+# PointCloudFilter: the visibility counts (host-buffer and device forms, binned and exhaustive paths) and the filter
+from openmvs_b200.depth_estimator import FuseDepthMaps, PointCloudFilter, PointCloudVisibility
+fv = [dict(v, conf=None, neighbors=[j for j in range(3) if j != i], n_scene_neighbors=2) for i, v in enumerate(copy.deepcopy(pv))]
+fc = FuseDepthMaps(fv)
+vh = PointCloudVisibility(pv, fc)
+fc.points = torch.from_numpy(fc.points).cuda()
+vd = PointCloudVisibility(pv, fc).cpu().numpy()
+away = [dict(v, R=-np.asarray(v["R"])) for v in pv]   # every query of every view takes the exhaustive path
+ve = PointCloudVisibility(away, fc).cpu().numpy()
+print("visibility", len(vh), "host == device", bool((vh == vd).all()), "exhaustive == binned", bool((ve == vd).all()),
+	"kept", len(PointCloudFilter(pv, fc, 0).points))
