@@ -7,7 +7,7 @@
 //    neighbour search is exact (DESIGN.md §5.6): a uniform grid in Morton order and a shell-by-shell search per point.
 //  - Scene::PointCloudFilter (libs/MVS/SceneDensify.cpp:2226-2360): the visibility counts of every (point, view) cone, exactly
 //    those of the single-threaded reference (DESIGN.md §5.7), and the order its removal loop leaves the kept points in.
-// The CPU restatements used by the tests are in oracle/point_cloud_oracle.py and tests/cpp/visibility_oracle.cpp.
+// The CPU restatements used by the tests are in oracle/point_cloud_oracle.py and oracle/visibility_oracle.cpp.
 #include <float.h>
 #include <stdint.h>
 #include <string.h>
@@ -56,29 +56,52 @@ int cloud_bad(b200mvs_ctx* ctx, int bad) {
 	return B200MVS_OK;
 }
 
-// the arguments every cloud call shares
+// What sets the per-point cloud calls apart at their entry: the prefix of their messages, whether every point needs a view, whether
+// they read the images' colour maps, and the bytes of one point's output
+struct CloudCall { const char* what; bool needView, colorMaps; size_t outBytes; };
+const CloudCall COLORS{"point colors: ", false, true, 3}, NORMALS{"point normals: ", true, false, 12},
+	VISIBILITY{"point visibility: ", false, false, 4};
+
+int refuse(b200mvs_ctx* ctx, const CloudCall& c, const char* why) {
+	return fail(ctx, B200MVS_ERR_ARG, (std::string(c.what) + why).c_str());
+}
+
+// A per-point call's buffers where its device form reads them (the caller's, or staged by the host form): the n points with their
+// view lists, image i's colour map color[i] (null: empty, or not read), and the output
+struct CloudBufs {
+	const float* points; uint32_t n; const uint32_t *off, *views;
+	std::vector<const uint8_t*> color;
+	void* out;
+};
+
+// the arguments every per-point call shares; refused: the call's own refusal of one of its other arguments, if any
 int cloud_args(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* offsets, const uint32_t* views,
-	const b200mvs_fuse_view* images, int nImages, const void* out)
+	const b200mvs_fuse_view* images, int nImages, const void* out, const char* refused)
 {
 	if (!ctx) return B200MVS_ERR_ARG;
 	if (nPoints > 0x7FFFFFFFull) return fail(ctx, B200MVS_ERR_ARG, "point cloud: more than 2^31 - 1 points");
 	// every point reads views unless the offsets are bad (refused then anyway)
 	if (nPoints > 0 && (!points || !offsets || !views || !out)) return fail(ctx, B200MVS_ERR_ARG, "point cloud: null pointer");
 	if (nImages < 0 || (nImages > 0 && !images)) return fail(ctx, B200MVS_ERR_ARG, "point cloud: bad image table");
-	return B200MVS_OK;
+	return refused ? fail(ctx, B200MVS_ERR_ARG, refused) : B200MVS_OK;
 }
 
-// the scene images as the kernels see them; color[i] is image i's colour map where the kernels read it (staged or the caller's)
-std::vector<CloudImage> cloud_images(const b200mvs_fuse_view* images, int nImages, const std::vector<const uint8_t*>& color) {
-	std::vector<CloudImage> t(nImages);
+// The scene images as the kernels see them, copied to dImages on s; color[i] is image i's colour map where the kernels read it.
+// The copy reads `table`, which the caller keeps until it synchronises s.
+int upload_images(b200mvs_ctx* ctx, CloudImage* dImages, std::vector<CloudImage>& table, const b200mvs_fuse_view* images,
+	int nImages, const std::vector<const uint8_t*>& color, cudaStream_t s)
+{
+	table.resize(nImages);
 	for (int i = 0; i < nImages; ++i) {
 		Cam cam;
 		fuse::compose(images[i].K, images[i].R, images[i].C, cam);
-		t[i].color = color[i]; t[i].w = images[i].width; t[i].h = images[i].height;
-		memcpy(t[i].P, cam.P, sizeof(cam.P));
-		for (int a = 0; a < 3; ++a) t[i].C[a] = (float)images[i].C[a];
+		CloudImage& t = table[i];
+		t.color = color[i]; t.w = images[i].width; t.h = images[i].height;
+		memcpy(t.P, cam.P, sizeof(cam.P));
+		for (int a = 0; a < 3; ++a) t.C[a] = (float)images[i].C[a];
 	}
-	return t;
+	if (nImages) CK(cudaMemcpyAsync(dImages, table.data(), sizeof(CloudImage)*nImages, cudaMemcpyHostToDevice, s));
+	return B200MVS_OK;
 }
 
 // Run the view checks (and with a box, the bounding box, the finite check and the sample of make_grid) of a device cloud, with
@@ -138,78 +161,61 @@ CloudGrid make_grid(const float box[6], const std::vector<float>& sample, uint32
 	return g;
 }
 
-// the grid's scratch, declared in the caller's carve
-struct GridScratch {
+// The exact k nearest neighbours (k <= n) of n points into nbr (n x k), with the checks of the cloud (and of its view lists when off
+// is given, each point with a view) and the grid's scratch joining the caller's slices in `scratch`, which this commits before its
+// first launch.  nbr may be one of those slices: it is read after the commit.
+int grid_knn(b200mvs_ctx* ctx, Carve& scratch, const float* points, uint32_t n, const uint32_t* off, const uint32_t* views,
+	int nImages, int k, uint32_t* const& nbr, cudaStream_t s)
+{
+	size_t cubBytes;
+	CK(cub_reserve(ctx->pcCub, cubBytes, [&](void* tmp, size_t& bytes) {
+		return fuse_sort(tmp, bytes, nullptr, nullptr, nullptr, nullptr, n, 30, nullptr);
+	}));
+	float box[6]; std::vector<float> sample;
+	if (int rc = cloud_check(ctx, points, n, off, views, nImages, true, box, &sample, s)) return rc;
+	const CloudGrid g = make_grid(box, sample, n, k);
+	// the grid: keys, the sort by key, the cells
+	const size_t nCells = (size_t)g.dim[0]*g.dim[1]*g.dim[2];
 	uint32_t *keys, *keysSorted, *idx, *idxSorted, *cellStart, *cellEnd;
 	float4* sorted;
-	size_t nCells;
-	void take(Carve& c, uint32_t n, const CloudGrid& g) {
-		nCells = (size_t)g.dim[0]*g.dim[1]*g.dim[2];
-		c.take(keys, n); c.take(keysSorted, n); c.take(idx, n); c.take(idxSorted, n); c.take(sorted, n);
-		c.take(cellStart, nCells); c.take(cellEnd, nCells);
-	}
-};
-
-// CUB's temporary storage of the key sort of n points, reserved before the call's first launch
-int reserve_sort(b200mvs_ctx* ctx, uint32_t n, size_t& bytes) {
-	bytes = 0;
-	CK(fuse_sort(nullptr, bytes, nullptr, nullptr, nullptr, nullptr, n, 30, nullptr));
-	CK(ctx->pcCub.reserve(std::max<size_t>(bytes, 1)));
-	bytes = ctx->pcCub.cap;
-	return B200MVS_OK;
-}
-
-// the grid (keys, the sort by key, the cells) and the k-NN search into indices (n x k, k <= n)
-int grid_knn(b200mvs_ctx* ctx, const GridScratch& G, const float* points, uint32_t n, const CloudGrid& g, int k, uint32_t* indices,
-	size_t cubBytes, cudaStream_t s)
-{
-	CK(cloud_launch_keys(points, n, g, G.keys, G.idx, s));
-	CK(fuse_sort(ctx->pcCub.p, cubBytes, G.keys, G.keysSorted, G.idx, G.idxSorted, n, 30, s));
-	CK(cudaMemsetAsync(G.cellStart, 0, G.nCells*4, s));
-	CK(cudaMemsetAsync(G.cellEnd, 0, G.nCells*4, s));
-	CK(cloud_launch_cells(points, G.keysSorted, G.idxSorted, n, g, G.sorted, G.cellStart, G.cellEnd, s));
-	CK(cloud_launch_knn(G.sorted, n, G.cellStart, G.cellEnd, g, k, indices, s));
+	scratch.take(keys, n); scratch.take(keysSorted, n); scratch.take(idx, n); scratch.take(idxSorted, n); scratch.take(sorted, n);
+	scratch.take(cellStart, nCells); scratch.take(cellEnd, nCells);
+	CK(scratch.commit());
+	CK(cloud_launch_keys(points, n, g, keys, idx, s));
+	CK(fuse_sort(ctx->pcCub.p, cubBytes, keys, keysSorted, idx, idxSorted, n, 30, s));
+	CK(cudaMemsetAsync(cellStart, 0, nCells*4, s));
+	CK(cudaMemsetAsync(cellEnd, 0, nCells*4, s));
+	CK(cloud_launch_cells(points, keysSorted, idxSorted, n, g, sorted, cellStart, cellEnd, s));
+	CK(cloud_launch_knn(sorted, n, cellStart, cellEnd, g, k, nbr, s));
 	ctx->launches += 4;
 	return B200MVS_OK;
 }
 
-// EstimatePointColors on device buffers; color[i] is image i's colour map on the device (null: empty)
-int colors_device(b200mvs_ctx* ctx, const float* points, uint32_t n, const uint32_t* off, const uint32_t* views,
-	const b200mvs_fuse_view* images, int nImages, const std::vector<const uint8_t*>& color, uint8_t* colors, cudaStream_t s)
-{
-	if (int rc = cloud_check(ctx, points, n, off, views, nImages, false, nullptr, nullptr, s)) return rc;
-	const std::vector<CloudImage> table = cloud_images(images, nImages, color);
+// EstimatePointColors on device buffers
+int colors_device(b200mvs_ctx* ctx, const CloudBufs& b, const b200mvs_fuse_view* images, int nImages, cudaStream_t s) {
+	if (int rc = cloud_check(ctx, b.points, b.n, b.off, b.views, nImages, false, nullptr, nullptr, s)) return rc;
 	Carve scratch(ctx->pcScratch);
 	CloudImage* dImages;
 	scratch.take(dImages, std::max(nImages, 1));
 	CK(scratch.commit());
-	if (nImages) CK(cudaMemcpyAsync(dImages, table.data(), sizeof(CloudImage)*nImages, cudaMemcpyHostToDevice, s));
-	CK(cloud_launch_colors(points, n, off, views, dImages, colors, s));
+	std::vector<CloudImage> table;
+	if (int rc = upload_images(ctx, dImages, table, images, nImages, b.color, s)) return rc;
+	CK(cloud_launch_colors(b.points, b.n, b.off, b.views, dImages, (uint8_t*)b.out, s));
 	++ctx->launches;
 	CK(cudaStreamSynchronize(s));   // the table is read from host memory that ends with this call
 	return B200MVS_OK;
 }
 
 // EstimatePointNormals on device buffers
-int normals_device(b200mvs_ctx* ctx, const float* points, uint32_t n, const uint32_t* off, const uint32_t* views,
-	const b200mvs_fuse_view* images, int nImages, int k, float* normals, cudaStream_t s)
-{
-	size_t cubBytes;
-	if (int rc = reserve_sort(ctx, n, cubBytes)) return rc;
-	float box[6]; std::vector<float> sample;
-	if (int rc = cloud_check(ctx, points, n, off, views, nImages, true, box, &sample, s)) return rc;
-	const int kk = (int)std::min<uint64_t>(k, n);
-	const CloudGrid g = make_grid(box, sample, n, kk);
-	const std::vector<CloudImage> table = cloud_images(images, nImages, std::vector<const uint8_t*>(nImages, nullptr));
+int normals_device(b200mvs_ctx* ctx, const CloudBufs& b, const b200mvs_fuse_view* images, int nImages, int k, cudaStream_t s) {
+	const int kk = (int)std::min<uint64_t>(k, b.n);
 	Carve scratch(ctx->pcScratch);
-	GridScratch G;
-	G.take(scratch, n, g);
 	uint32_t* nbr; CloudImage* dImages;
-	scratch.take(nbr, (size_t)n*kk); scratch.take(dImages, std::max(nImages, 1));
-	CK(scratch.commit());
-	CK(cudaMemcpyAsync(dImages, table.data(), sizeof(CloudImage)*nImages, cudaMemcpyHostToDevice, s));
-	if (int rc = grid_knn(ctx, G, points, n, g, kk, nbr, cubBytes, s)) return rc;
-	CK(cloud_launch_pca(points, n, nbr, kk, off, views, dImages, normals, s));
+	scratch.take(nbr, (size_t)b.n*kk); scratch.take(dImages, std::max(nImages, 1));
+	if (int rc = grid_knn(ctx, scratch, b.points, b.n, b.off, b.views, nImages, kk, nbr, s)) return rc;
+	std::vector<CloudImage> table;
+	if (int rc = upload_images(ctx, dImages, table, images, nImages, b.color, s)) return rc;
+	CK(cloud_launch_pca(b.points, b.n, nbr, kk, b.off, b.views, dImages, (float*)b.out, s));
 	++ctx->launches;
 	CK(cudaStreamSynchronize(s));
 	return B200MVS_OK;
@@ -262,9 +268,9 @@ int key_bits(uint32_t maxKey) {
 // PointCloudFilter's visibility counts on device buffers: the queries (the entries of the view lists) sorted by view, then per
 // view with queries: bin every point by its cell, sort the bins, answer the queries from the bins and the flagged ones by testing
 // every point.  One carve of the call's scratch, one read-back of the per-view query ranges.
-int visibility_device(b200mvs_ctx* ctx, const float* points, uint32_t n, const uint32_t* off, const uint32_t* views,
-	const b200mvs_fuse_view* images, int nImages, int32_t* visibility, cudaStream_t s)
-{
+int visibility_device(b200mvs_ctx* ctx, const CloudBufs& b, const b200mvs_fuse_view* images, int nImages, cudaStream_t s) {
+	const float* points = b.points; const uint32_t *off = b.off, *views = b.views; const uint32_t n = b.n;
+	int32_t* visibility = (int32_t*)b.out;
 	for (int i = 0; i < nImages; ++i)
 		if (images[i].width <= 0 || images[i].height <= 0) return fail(ctx, B200MVS_ERR_ARG, "point visibility: image size out of range");
 	float box[6];
@@ -279,11 +285,10 @@ int visibility_device(b200mvs_ctx* ctx, const float* points, uint32_t n, const u
 	for (int i = 0; i < nImages; ++i) { V[i] = vis_view(images[i]); maxCells = std::max(maxCells, V[i].nCells); }
 	// CUB's temporary storage for both sorts, reserved before the first launch of the call's work
 	const int viewBits = key_bits((uint32_t)std::max(nImages-1, 0)), cellBits = key_bits(maxCells);
-	size_t bytesViews = 0, bytesCells = 0;
-	CK(fuse_sort(nullptr, bytesViews, nullptr, nullptr, nullptr, nullptr, nEntries, viewBits, nullptr));
-	CK(fuse_sort(nullptr, bytesCells, nullptr, nullptr, nullptr, nullptr, n, cellBits, nullptr));
-	CK(ctx->pcCub.reserve(std::max<size_t>(std::max(bytesViews, bytesCells), 1)));
-	size_t cubBytes = ctx->pcCub.cap;
+	size_t cubBytes;
+	CK(cub_reserve(ctx->pcCub, cubBytes,
+		[&](void* tmp, size_t& bytes) { return fuse_sort(tmp, bytes, nullptr, nullptr, nullptr, nullptr, nEntries, viewBits, nullptr); },
+		[&](void* tmp, size_t& bytes) { return fuse_sort(tmp, bytes, nullptr, nullptr, nullptr, nullptr, n, cellBits, nullptr); }));
 	Carve scratch(ctx->pcScratch);
 	uint32_t *entryPoint, *viewSorted, *qPoint, *viewStart, *keys, *keysSorted, *idx, *idxSorted, *cellStart, *flagged, *nFlagged;
 	float4* sorted;
@@ -316,6 +321,56 @@ int visibility_device(b200mvs_ctx* ctx, const float* points, uint32_t n, const u
 	}
 	CK(cudaStreamSynchronize(s));
 	return B200MVS_OK;
+}
+
+// The device form of a per-point call: the shared checks, then form(buffers, stream) on the caller's buffers
+template <typename F>
+int cloud_device(b200mvs_ctx* ctx, const CloudCall& c, const char* refused, const float* points, uint64_t nPoints,
+	const uint32_t* off, const uint32_t* views, const b200mvs_fuse_view* images, int nImages, void* out, void* stream, F&& form)
+{
+	if (int rc = cloud_args(ctx, points, nPoints, off, views, images, nImages, out, refused)) return rc;
+	if (nPoints == 0) return B200MVS_OK;
+	CK(cudaSetDevice(ctx->device));
+	CloudBufs b{points, (uint32_t)nPoints, off, views, std::vector<const uint8_t*>(nImages, nullptr), out};
+	for (int i = 0; c.colorMaps && i < nImages; ++i) {
+		b.color[i] = images[i].color;
+		if (b.color[i] && (images[i].width <= 0 || images[i].height <= 0)) return refuse(ctx, c, "image size out of range");
+		if (!on_device(ctx, b.color[i])) return refuse(ctx, c, "an image is not in device memory of the context's device");
+	}
+	if (!on_device(ctx, points) || !on_device(ctx, off) || !on_device(ctx, views) || !on_device(ctx, out))
+		return refuse(ctx, c, "a buffer is not in device memory of the context's device");
+	ctx->launches = 0;
+	return form(b, stream_of(ctx, stream));
+}
+
+// The host-buffer form of a per-point call: the shared checks, then the caller's buffers staged for form(buffers, stream) and its
+// output copied back (HostCall)
+template <typename F>
+int cloud_host(b200mvs_ctx* ctx, const CloudCall& c, const char* refused, const float* points, uint64_t nPoints,
+	const uint32_t* off, const uint32_t* views, const b200mvs_fuse_view* images, int nImages, void* out, b200mvs_stats* stats,
+	F&& form)
+{
+	if (int rc = cloud_args(ctx, points, nPoints, off, views, images, nImages, out, refused)) return rc;
+	if (nPoints == 0) return stats ? (memset(stats, 0, sizeof(*stats)), B200MVS_OK) : B200MVS_OK;
+	if (int rc = check_views_host(ctx, off, views, nPoints, nImages, c.needView)) return rc;
+	CK(cudaSetDevice(ctx->device));
+	ctx->launches = 0;
+	HostCall call(ctx);
+	CloudBufs b{nullptr, (uint32_t)nPoints, nullptr, nullptr, std::vector<const uint8_t*>(nImages, nullptr), nullptr};
+	call.in(b.points, points, 12*nPoints); call.in(b.off, off, 4*(nPoints+1)); call.in(b.views, views, 4*(size_t)off[nPoints]);
+	for (int i = 0; c.colorMaps && i < nImages; ++i) {
+		if (!images[i].color) continue;
+		if (images[i].width <= 0 || images[i].height <= 0) return refuse(ctx, c, "image size out of range");
+		call.in(b.color[i], images[i].color, 3*(size_t)images[i].width*images[i].height);
+	}
+	call.out(b.out, out, c.outBytes*nPoints);
+	if (int rc = call.stage()) return rc;
+	return call.run([&](cudaStream_t s) { return form(b, s); }, stats);
+}
+
+// EstimatePointNormals' own refusal
+const char* normals_refused(int numNeighbors) {
+	return numNeighbors < 1 || numNeighbors > B200MVS_MAX_POINT_NEIGHBORS ? "point normals: numNeighbors out of [1, 32]" : nullptr;
 }
 
 } // namespace
@@ -388,10 +443,10 @@ int b200mvs_merge_depth_maps_device(b200mvs_ctx* ctx, const b200mvs_fuse_view* v
 			const size_t np = (size_t)views[i].width*views[i].height;
 			flagOff[i] = flagBytes; flagBytes += np; maxNp = std::max(maxNp, np);
 		}
-	size_t cubBytes = 0;
-	CK(fuse_select(nullptr, cubBytes, nullptr, nullptr, nullptr, std::max<size_t>(maxNp, 1), nullptr));
-	CK(ctx->pcCub.reserve(std::max<size_t>(cubBytes, 1)));
-	cubBytes = ctx->pcCub.cap;
+	size_t cubBytes;
+	CK(cub_reserve(ctx->pcCub, cubBytes, [&](void* tmp, size_t& bytes) {
+		return fuse_select(tmp, bytes, nullptr, nullptr, nullptr, std::max<size_t>(maxNp, 1), nullptr);
+	}));
 	Carve scratch(ctx->pcScratch);
 	unsigned long long *counts, *bases; uint8_t* flags; uint32_t *idx, *nSel;
 	scratch.take(counts, nViews); scratch.take(bases, nViews); scratch.take(flags, std::max<size_t>(flagBytes, 1));
@@ -432,131 +487,52 @@ int b200mvs_merge_depth_maps_device(b200mvs_ctx* ctx, const b200mvs_fuse_view* v
 		ctx->launches += 2;
 	}
 	CK(cudaEventRecord(ctx->ev1, s));
-	// one read-back of the whole point cloud
-	b200mvs_pointcloud* pc = new (std::nothrow) b200mvs_pointcloud;
-	if (!pc) return fail(ctx, B200MVS_ERR_CUDA, "merge: out of host memory");
-	struct Owner { b200mvs_pointcloud* p; ~Owner() { delete p; } } own{pc};
-	pc->points.resize(3*total); pc->projs.resize(2*total); pc->views.resize(total);
-	pc->colors.resize(bColor ? 3*total : 0); pc->normals.resize(bNormal ? 3*total : 0);
-	auto get = [&](void* dst, const void* src, size_t bytes) {
-		d2h += bytes;
-		return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
-	};
-	CK(get(pc->points.data(), points, pc->points.size()*4)); CK(get(pc->projs.data(), projs, pc->projs.size()*2));
-	CK(get(pc->views.data(), pviews, pc->views.size()*4)); CK(get(pc->colors.data(), colors, pc->colors.size()));
-	CK(get(pc->normals.data(), normals, pc->normals.size()*4));
-	pc->offsets.resize(total+1);
-	for (size_t i = 0; i <= total; ++i) pc->offsets[i] = (uint32_t)i;   // one view per point
-	CK(cudaStreamSynchronize(s));
-	pc->nDepths = total;
-	if (stats) { const int rc = fill_stats(ctx, stats, t0, 1, 0, d2h); if (rc) return rc; }
-	*out = pc;
-	own.p = nullptr;
-	return B200MVS_OK;
+	const DeviceCloud cloud{total, total, bColor ? total : 0, points, normals, nullptr, colors, nullptr, pviews, projs, nullptr};
+	return read_cloud(ctx, "merge: out of host memory", cloud, s, t0, d2h, stats, out);
 }
 
 int b200mvs_estimate_point_colors_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
 	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, uint8_t* colors, void* stream)
 {
-	if (int rc = cloud_args(ctx, points, nPoints, viewOffsets, views, images, nImages, colors)) return rc;
-	if (nPoints == 0) return B200MVS_OK;
-	CK(cudaSetDevice(ctx->device));
-	std::vector<const uint8_t*> color(nImages);
-	for (int i = 0; i < nImages; ++i) {
-		color[i] = images[i].color;
-		if (color[i] && (images[i].width <= 0 || images[i].height <= 0)) return fail(ctx, B200MVS_ERR_ARG, "point colors: image size out of range");
-		if (!on_device(ctx, color[i])) return fail(ctx, B200MVS_ERR_ARG, "point colors: an image is not in device memory of the context's device");
-	}
-	if (!on_device(ctx, points) || !on_device(ctx, viewOffsets) || !on_device(ctx, views) || !on_device(ctx, colors))
-		return fail(ctx, B200MVS_ERR_ARG, "point colors: a buffer is not in device memory of the context's device");
-	ctx->launches = 0;
-	return colors_device(ctx, points, (uint32_t)nPoints, viewOffsets, views, images, nImages, color, colors, stream_of(ctx, stream));
+	return cloud_device(ctx, COLORS, nullptr, points, nPoints, viewOffsets, views, images, nImages, colors, stream,
+		[&](const CloudBufs& b, cudaStream_t s) { return colors_device(ctx, b, images, nImages, s); });
 }
 
 int b200mvs_estimate_point_colors(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
 	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, uint8_t* colors, b200mvs_stats* stats)
 {
-	if (int rc = cloud_args(ctx, points, nPoints, viewOffsets, views, images, nImages, colors)) return rc;
-	if (nPoints == 0) return stats ? (memset(stats, 0, sizeof(*stats)), B200MVS_OK) : B200MVS_OK;
-	if (int rc = check_views_host(ctx, viewOffsets, views, nPoints, nImages, false)) return rc;
-	CK(cudaSetDevice(ctx->device));
-	ctx->launches = 0;
-	HostCall call(ctx);
-	const float* dPoints; const uint32_t *dOff, *dViews; uint8_t* dColors;
-	std::vector<const uint8_t*> color(nImages, nullptr);
-	call.in(dPoints, points, 12*nPoints); call.in(dOff, viewOffsets, 4*(nPoints+1)); call.in(dViews, views, 4*(size_t)viewOffsets[nPoints]);
-	for (int i = 0; i < nImages; ++i) {
-		if (!images[i].color) continue;
-		if (images[i].width <= 0 || images[i].height <= 0) return fail(ctx, B200MVS_ERR_ARG, "point colors: image size out of range");
-		call.in(color[i], images[i].color, 3*(size_t)images[i].width*images[i].height);
-	}
-	call.out(dColors, colors, 3*nPoints);
-	if (int rc = call.stage()) return rc;
-	return call.run([&](cudaStream_t s) {
-		return colors_device(ctx, dPoints, (uint32_t)nPoints, dOff, dViews, images, nImages, color, dColors, s);
-	}, stats);
+	return cloud_host(ctx, COLORS, nullptr, points, nPoints, viewOffsets, views, images, nImages, colors, stats,
+		[&](const CloudBufs& b, cudaStream_t s) { return colors_device(ctx, b, images, nImages, s); });
 }
 
 int b200mvs_estimate_point_normals_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
 	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int numNeighbors, float* normals, void* stream)
 {
-	if (int rc = cloud_args(ctx, points, nPoints, viewOffsets, views, images, nImages, normals)) return rc;
-	if (numNeighbors < 1 || numNeighbors > B200MVS_MAX_POINT_NEIGHBORS) return fail(ctx, B200MVS_ERR_ARG, "point normals: numNeighbors out of [1, 32]");
-	if (nPoints == 0) return B200MVS_OK;
-	CK(cudaSetDevice(ctx->device));
-	if (!on_device(ctx, points) || !on_device(ctx, viewOffsets) || !on_device(ctx, views) || !on_device(ctx, normals))
-		return fail(ctx, B200MVS_ERR_ARG, "point normals: a buffer is not in device memory of the context's device");
-	ctx->launches = 0;
-	return normals_device(ctx, points, (uint32_t)nPoints, viewOffsets, views, images, nImages, numNeighbors, normals, stream_of(ctx, stream));
+	return cloud_device(ctx, NORMALS, normals_refused(numNeighbors), points, nPoints, viewOffsets, views, images, nImages,
+		normals, stream,
+		[&](const CloudBufs& b, cudaStream_t s) { return normals_device(ctx, b, images, nImages, numNeighbors, s); });
 }
 
 int b200mvs_estimate_point_normals(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
 	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int numNeighbors, float* normals, b200mvs_stats* stats)
 {
-	if (int rc = cloud_args(ctx, points, nPoints, viewOffsets, views, images, nImages, normals)) return rc;
-	if (numNeighbors < 1 || numNeighbors > B200MVS_MAX_POINT_NEIGHBORS) return fail(ctx, B200MVS_ERR_ARG, "point normals: numNeighbors out of [1, 32]");
-	if (nPoints == 0) return stats ? (memset(stats, 0, sizeof(*stats)), B200MVS_OK) : B200MVS_OK;
-	if (int rc = check_views_host(ctx, viewOffsets, views, nPoints, nImages, true)) return rc;
-	CK(cudaSetDevice(ctx->device));
-	ctx->launches = 0;
-	HostCall call(ctx);
-	const float* dPoints; const uint32_t *dOff, *dViews; float* dNormals;
-	call.in(dPoints, points, 12*nPoints); call.in(dOff, viewOffsets, 4*(nPoints+1)); call.in(dViews, views, 4*(size_t)viewOffsets[nPoints]);
-	call.out(dNormals, normals, 12*nPoints);
-	if (int rc = call.stage()) return rc;
-	return call.run([&](cudaStream_t s) {
-		return normals_device(ctx, dPoints, (uint32_t)nPoints, dOff, dViews, images, nImages, numNeighbors, dNormals, s);
-	}, stats);
+	return cloud_host(ctx, NORMALS, normals_refused(numNeighbors), points, nPoints, viewOffsets, views, images, nImages,
+		normals, stats,
+		[&](const CloudBufs& b, cudaStream_t s) { return normals_device(ctx, b, images, nImages, numNeighbors, s); });
 }
 
 int b200mvs_point_cloud_visibility_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
 	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int32_t* visibility, void* stream)
 {
-	if (int rc = cloud_args(ctx, points, nPoints, viewOffsets, views, images, nImages, visibility)) return rc;
-	if (nPoints == 0) return B200MVS_OK;
-	CK(cudaSetDevice(ctx->device));
-	if (!on_device(ctx, points) || !on_device(ctx, viewOffsets) || !on_device(ctx, views) || !on_device(ctx, visibility))
-		return fail(ctx, B200MVS_ERR_ARG, "point visibility: a buffer is not in device memory of the context's device");
-	ctx->launches = 0;
-	return visibility_device(ctx, points, (uint32_t)nPoints, viewOffsets, views, images, nImages, visibility, stream_of(ctx, stream));
+	return cloud_device(ctx, VISIBILITY, nullptr, points, nPoints, viewOffsets, views, images, nImages, visibility, stream,
+		[&](const CloudBufs& b, cudaStream_t s) { return visibility_device(ctx, b, images, nImages, s); });
 }
 
 int b200mvs_point_cloud_visibility(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets,
 	const uint32_t* views, const b200mvs_fuse_view* images, int nImages, int32_t* visibility, b200mvs_stats* stats)
 {
-	if (int rc = cloud_args(ctx, points, nPoints, viewOffsets, views, images, nImages, visibility)) return rc;
-	if (nPoints == 0) return stats ? (memset(stats, 0, sizeof(*stats)), B200MVS_OK) : B200MVS_OK;
-	if (int rc = check_views_host(ctx, viewOffsets, views, nPoints, nImages, false)) return rc;
-	CK(cudaSetDevice(ctx->device));
-	ctx->launches = 0;
-	HostCall call(ctx);
-	const float* dPoints; const uint32_t *dOff, *dViews; int32_t* dVis;
-	call.in(dPoints, points, 12*nPoints); call.in(dOff, viewOffsets, 4*(nPoints+1)); call.in(dViews, views, 4*(size_t)viewOffsets[nPoints]);
-	call.out(dVis, visibility, 4*nPoints);
-	if (int rc = call.stage()) return rc;
-	return call.run([&](cudaStream_t s) {
-		return visibility_device(ctx, dPoints, (uint32_t)nPoints, dOff, dViews, images, nImages, dVis, s);
-	}, stats);
+	return cloud_host(ctx, VISIBILITY, nullptr, points, nPoints, viewOffsets, views, images, nImages, visibility, stats,
+		[&](const CloudBufs& b, cudaStream_t s) { return visibility_device(ctx, b, images, nImages, s); });
 }
 
 int b200mvs_pointcloud_remove_order(const uint8_t* remove, uint64_t n, uint32_t* order, uint64_t* nKept) {
@@ -581,19 +557,10 @@ int b200mvs_point_knn_device(b200mvs_ctx* ctx, const float* points, uint64_t nPo
 	if (!on_device(ctx, points) || !on_device(ctx, indices))
 		return fail(ctx, B200MVS_ERR_ARG, "k-NN: a buffer is not in device memory of the context's device");
 	ctx->launches = 0;
-	const uint32_t n = (uint32_t)nPoints;
 	cudaStream_t s = stream_of(ctx, stream);
-	size_t cubBytes;
-	if (int rc = reserve_sort(ctx, n, cubBytes)) return rc;
-	float box[6]; std::vector<float> sample;
-	if (int rc = cloud_check(ctx, points, n, nullptr, nullptr, 0, false, box, &sample, s)) return rc;
-	const int kk = (int)std::min<uint64_t>(numNeighbors, n);
-	const CloudGrid g = make_grid(box, sample, n, kk);
 	Carve scratch(ctx->pcScratch);
-	GridScratch G;
-	G.take(scratch, n, g);
-	CK(scratch.commit());
-	if (int rc = grid_knn(ctx, G, points, n, g, kk, indices, cubBytes, s)) return rc;
+	if (int rc = grid_knn(ctx, scratch, points, (uint32_t)nPoints, nullptr, nullptr, 0, (int)std::min<uint64_t>(numNeighbors, nPoints),
+		indices, s)) return rc;
 	CK(cudaStreamSynchronize(s));
 	return B200MVS_OK;
 }

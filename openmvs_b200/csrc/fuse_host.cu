@@ -300,10 +300,6 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 	DevBuf* O = ctx->fsOut;
 	const size_t perPoint[4] = {12, 12, 3, 4}, perView[3] = {4, 4, 4};
 	uint64_t nPts = 0, nVw = 0, nCol = 0, shared = 0;
-	size_t need = 0;
-	// a CUB call: query its temporary storage, then run it
-#define FUSE_CUB(call) do { need = 0; { void* tmp = nullptr; CK(call); } \
-		CK(ctx->fsCub.reserve(std::max<size_t>(need, 1))); { void* tmp = ctx->fsCub.p; CK(call); } } while (0)
 	for (const int a: plan.order) {
 		const b200mvs_fuse_view& A = views[a];
 		const size_t np = (size_t)A.width*A.height;
@@ -316,7 +312,7 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 		CK(cudaEventRecord(ev.b, s));
 		// the candidates: pixels with a depth and no claim, in raster order
 		CK(fuse_launch_candidates(A.depth, dv[a].claim, np, flags, &cnt->nDepths, s));
-		FUSE_CUB(fuse_select(tmp, need, flags, cand, &cnt->nCand, np, s));
+		CK(cub_run(ctx->fsCub, [&](void* tmp, size_t& bytes) { return fuse_select(tmp, bytes, flags, cand, &cnt->nCand, np, s); }));
 		ctx->launches += 2;
 		uint32_t nCand = 0, nEdges = 0;
 		CK(cudaMemcpyAsync(&nCand, &cnt->nCand, 4, cudaMemcpyDeviceToHost, s));
@@ -339,7 +335,7 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 				// the edges: type and target from the maps at the start of the round; the claim and zero edges, grouped by target in
 				// raster order of their owners (the radix sort is stable and its input is in edge order)
 				CK(fuse_launch_classify(R, cand, nCand, typ, tgt, s));
-				FUSE_CUB(fuse_select(tmp, need, typ, e1, &cnt->nEdges, ne, s));
+				CK(cub_run(ctx->fsCub, [&](void* tmp, size_t& bytes) { return fuse_select(tmp, bytes, typ, e1, &cnt->nEdges, ne, s); }));
 				ctx->launches += 2;
 				CK(cudaMemcpyAsync(&nEdges, &cnt->nEdges, 4, cudaMemcpyDeviceToHost, s));
 				CK(cudaStreamSynchronize(s));
@@ -349,7 +345,7 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 					while (endBit < 32 && (1ull << endBit) < (uint64_t)nbBase[nbOff[a]+nNb-1] + (uint64_t)dv[nbIds[nbOff[a]+nNb-1]].w*dv[nbIds[nbOff[a]+nNb-1]].h)
 						++endBit;
 					CK(fuse_launch_gather_keys(tgt, e1, nEdges, k1, s));
-					FUSE_CUB(fuse_sort(tmp, need, k1, keys, e1, edges, nEdges, endBit, s));
+					CK(cub_run(ctx->fsCub, [&](void* tmp, size_t& bytes) { return fuse_sort(tmp, bytes, k1, keys, e1, edges, nEdges, endBit, s); }));
 					CK(fuse_launch_shared(keys, nEdges, &cnt->shared, s));
 					ctx->launches += 3;
 				}
@@ -372,8 +368,8 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 			if (nEdges > 0) { CK(fuse_launch_walk(keys, edges, nEdges, nNb, acc, status, s)); ++ctx->launches; }
 			// point IDs and view offsets in raster order, then the points
 			CK(fuse_launch_count(R, nCand, typ, status, acc, isPt, nv, s));
-			FUSE_CUB(fuse_scan(tmp, need, isPt, ptId, nCand, s));
-			FUSE_CUB(fuse_scan(tmp, need, nv, vOff, nCand, s));
+			CK(cub_run(ctx->fsCub, [&](void* tmp, size_t& bytes) { return fuse_scan(tmp, bytes, isPt, ptId, nCand, s); }));
+			CK(cub_run(ctx->fsCub, [&](void* tmp, size_t& bytes) { return fuse_scan(tmp, bytes, nv, vOff, nCand, s); }));
 			CK(fuse_launch_totals(isPt, ptId, nv, vOff, nCand, cnt->totals, s));
 			ctx->launches += 4;
 			FuseCounters hc;
@@ -406,31 +402,10 @@ int b200mvs_fuse_depth_maps_device(b200mvs_ctx* ctx, b200mvs_fuse_view* views, i
 		CK(cudaEventElapsedTime(&st.ms, ev.b, ev.e));
 		ctx->fsRounds.push_back(st);
 	}
-#undef FUSE_CUB
 	CK(cudaEventRecord(ctx->ev1, s));
-	// one read-back of the whole point cloud
-	b200mvs_pointcloud* pc = new (std::nothrow) b200mvs_pointcloud;
-	if (!pc) return fail(ctx, B200MVS_ERR_CUDA, "fuse: out of host memory");
-	struct Owner { b200mvs_pointcloud* p; ~Owner() { delete p; } } own{pc};
-	FuseCounters hc;
-	CK(cudaMemcpyAsync(&hc, cnt, sizeof(hc), cudaMemcpyDeviceToHost, s));
-	pc->points.resize(3*nPts); pc->normals.resize(plan.bNormal ? 3*nPts : 0); pc->colors.resize(3*nCol);
-	pc->offsets.resize(nPts+1); pc->views.resize(nVw); pc->weights.resize(nVw); pc->projs.resize(2*nVw);
-	auto get = [&](void* dst, const DevBuf& src, size_t bytes) {
-		d2h += bytes;
-		return bytes ? cudaMemcpyAsync(dst, src.p, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
-	};
-	CK(get(pc->points.data(), O[0], pc->points.size()*4)); CK(get(pc->normals.data(), O[1], pc->normals.size()*4));
-	CK(get(pc->colors.data(), O[2], pc->colors.size())); CK(get(pc->offsets.data(), O[3], nPts*4));
-	CK(get(pc->views.data(), O[4], nVw*4)); CK(get(pc->weights.data(), O[5], nVw*4)); CK(get(pc->projs.data(), O[6], nVw*4));
-	CK(cudaStreamSynchronize(s));
-	d2h += sizeof(hc);
-	pc->offsets[nPts] = (uint32_t)nVw;
-	pc->nDepths = hc.nDepths;
-	if (stats) { const int rc = fill_stats(ctx, stats, t0, 1, 0, d2h); if (rc) return rc; }
-	*out = pc;
-	own.p = nullptr;
-	return B200MVS_OK;
+	const DeviceCloud cloud{nPts, nVw, nCol, O[0].as<float>(), plan.bNormal ? O[1].as<float>() : nullptr, O[5].as<float>(),
+		O[2].as<uint8_t>(), O[3].as<uint32_t>(), O[4].as<uint32_t>(), O[6].as<uint16_t>(), cnt};
+	return read_cloud(ctx, "fuse: out of host memory", cloud, s, t0, d2h, stats, out);
 }
 
 int b200mvs_fuse_round_stats(b200mvs_ctx* ctx, int maxRounds, int* nRounds, int* image, int* iterations, uint64_t* candidates,

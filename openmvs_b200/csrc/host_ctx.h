@@ -1,6 +1,6 @@
 // host_ctx.h — the engine context behind the C-ABI (b200mvs_ctx) and the helpers shared by its host files: capi.cu (lifecycle
 // and settings), pm_host.cu (PatchMatch), sgm_host.cu (SGM), post_host.cu (post-processing and image preparation), fuse_host.cu
-// (FuseDepthMaps), cloud_host.cu (MergeDepthMaps, point colours and normals).
+// (FuseDepthMaps), cloud_host.cu (MergeDepthMaps and the point-cloud calls).
 // Internal to the library; include/b200mvs.h is the interface.
 //
 // Device scratch is owned by subsystem: the context keeps one arena per subsystem, and each entry point carves all of its
@@ -17,6 +17,7 @@
 #include <chrono>
 #include <cmath>
 #include <cstring>
+#include <new>
 #include <string>
 #include <vector>
 
@@ -172,6 +173,73 @@ inline int fill_stats(b200mvs_ctx* ctx, b200mvs_stats* stats, std::chrono::stead
 	stats->ms_total = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now()-t0).count();
 	stats->kernel_launches = ctx->launches; stats->levels = levels;
 	stats->bytes_h2d = h2d; stats->bytes_d2h = d2h;
+	return B200MVS_OK;
+}
+
+// CUB's temporary storage in the arena `cub` for the CUB calls given as call(tmp, bytes), each of which only queries its bytes
+// when tmp is null: the arena grows to the largest query, and every one of them may then run on cub.p with `bytes`
+template <typename... F> cudaError_t cub_reserve(DevBuf& cub, size_t& bytes, F&&... calls) {
+	size_t need = 1;
+	cudaError_t e = cudaSuccess;
+	auto query = [&](auto& call) {
+		size_t b = 0;
+		if (e == cudaSuccess) e = call(nullptr, b);
+		need = std::max(need, b);
+	};
+	(query(calls), ...);
+	if (e == cudaSuccess) e = cub.reserve(need);
+	bytes = cub.cap;
+	return e;
+}
+// one CUB call, on the arena grown for it
+template <typename F> cudaError_t cub_run(DevBuf& cub, F&& call) {
+	size_t bytes;
+	if (cudaError_t e = cub_reserve(cub, bytes, call)) return e;
+	return call(cub.p, bytes);
+}
+
+// A point cloud that a device form (FuseDepthMaps, MergeDepthMaps) built on the device: nPoints points with nViews views in all.
+// normals, weights: null when the cloud has none; colors: the first nColors points'; offsets: the first nPoints view offsets, or
+// null for one view per point; counters: FuseDepthMaps' counters, which give nDepths (null: nDepths = nPoints).
+struct DeviceCloud {
+	uint64_t nPoints, nViews, nColors;
+	const float *points, *normals, *weights;
+	const uint8_t* colors;
+	const uint32_t *offsets, *views;
+	const uint16_t* projs;
+	const FuseCounters* counters;
+};
+
+// The read-back of a device form's cloud into *out, with one synchronisation of s: the copies' bytes are added to d2h, the
+// statistics (stats may be null) are filled, and the cloud is handed over only when all of it succeeded.  oom: the error text
+// when the host allocation fails.
+inline int read_cloud(b200mvs_ctx* ctx, const char* oom, const DeviceCloud& c, cudaStream_t s,
+	std::chrono::steady_clock::time_point t0, uint64_t d2h, b200mvs_stats* stats, b200mvs_pointcloud** out)
+{
+	b200mvs_pointcloud* pc = new (std::nothrow) b200mvs_pointcloud;
+	if (!pc) return fail(ctx, B200MVS_ERR_CUDA, oom);
+	struct Owner { b200mvs_pointcloud* p; ~Owner() { delete p; } } own{pc};
+	const uint64_t n = c.nPoints, nv = c.nViews;
+	pc->points.resize(3*n); pc->normals.resize(c.normals ? 3*n : 0); pc->colors.resize(3*c.nColors);
+	pc->offsets.resize(n+1); pc->views.resize(nv); pc->weights.resize(c.weights ? nv : 0); pc->projs.resize(2*nv);
+	auto get = [&](void* dst, const void* src, size_t bytes) {
+		d2h += bytes;
+		return bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+	};
+	FuseCounters counters;
+	if (c.counters) CK(get(&counters, c.counters, sizeof(counters)));
+	CK(get(pc->points.data(), c.points, pc->points.size()*4)); CK(get(pc->normals.data(), c.normals, pc->normals.size()*4));
+	CK(get(pc->colors.data(), c.colors, pc->colors.size()));
+	CK(get(pc->views.data(), c.views, nv*4)); CK(get(pc->weights.data(), c.weights, pc->weights.size()*4));
+	CK(get(pc->projs.data(), c.projs, nv*4));
+	if (c.offsets) CK(get(pc->offsets.data(), c.offsets, n*4));
+	else for (uint64_t i = 0; i < n; ++i) pc->offsets[i] = (uint32_t)i;
+	CK(cudaStreamSynchronize(s));
+	pc->offsets[n] = (uint32_t)nv;
+	pc->nDepths = c.counters ? counters.nDepths : n;
+	if (stats) { const int rc = fill_stats(ctx, stats, t0, 1, 0, d2h); if (rc) return rc; }
+	*out = pc;
+	own.p = nullptr;
 	return B200MVS_OK;
 }
 

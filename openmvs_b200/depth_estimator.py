@@ -866,43 +866,66 @@ def FuseDepthMaps(views, nMinViewsFuse: int = 2, fDepthDiffThreshold: float = 0.
 	numpy maps take b200mvs_fuse_depth_maps (host code: the sequential loop).  CUDA tensors (every map on one device, depth
 	contiguous) take b200mvs_fuse_depth_maps_device on a context kept per device: the same point cloud, bit for bit, with the
 	pixels of each image resolved in parallel; a neighbour list must not repeat an image ID there."""
-	lib = _lib.load()
-	first = next((v["depth"] for v in views if _is_torch(v.get("depth"))), None)
-	device = None if first is None else _cuda_index(first)
-	n = len(views)
-	arr = (_lib.FuseView*n)()
+	maps = (("depth", "float32", ()), ("normal", "float32", (3,)), ("conf", "float32", ()), ("color", "uint8", (3,)))
+	return _cloud_call("FuseDepthMaps", "fuse_depth_maps", views, maps,
+		(nMinViewsFuse, fDepthDiffThreshold, fNormalDiffThreshold, bEstimateColor, bEstimateNormal), fuse=True)
+
+
+def _image_table(where: str, views, device, maps, fuse: bool = False):
+	"""the b200mvs_fuse_view table of FuseDepthMaps, MergeDepthMaps and the point-cloud calls -> (table, keepalive).  maps: (key,
+	dtype, channels) of the maps the call reads; a map's size is the size of the first map given.  fuse (FuseDepthMaps): depth
+	comes first and is modified in place, so it is passed as given and a host depth-map must be writeable; a view without one has
+	no other map; and the neighbour fields are set."""
+	arr = (_lib.FuseView*len(views))()
 	keep = []
 	for i, v in enumerate(views):
 		o = arr[i]
-		d = v.get("depth")
-		if d is not None:
-			o.depth = _arg("FuseDepthMaps", "views[%d].depth" % i, d, "float32", (None, None), device)
-			if device is None and not d.flags.writeable:
-				raise ValueError("FuseDepthMaps: views[%d].depth must be writeable (it is modified in place)" % i)
-			o.height, o.width = d.shape
-			for key, dt, ch in (("normal", "float32", (3,)), ("conf", "float32", ()), ("color", "uint8", (3,))):
-				a = v.get(key)
+		size = None
+		for key, dt, ch in maps:
+			a = v.get(key)
+			in_place = fuse and key == "depth"
+			if not in_place:
 				a = a.contiguous() if _is_torch(a) and a.is_cuda else _host(a, dt, device)
-				keep.append(a)
-				setattr(o, key, _arg("FuseDepthMaps", "views[%d].%s" % (i, key), a, dt, tuple(d.shape)+ch, device))
+			keep.append(a)
+			shape = (None, None)+ch if size is None else size+ch
+			setattr(o, key, _arg(where, "views[%d].%s" % (i, key), a, dt, shape, device))
+			if in_place and device is None and a is not None and not a.flags.writeable:
+				raise ValueError("%s: views[%d].depth must be writeable (it is modified in place)" % (where, i))
+			if a is not None and size is None:
+				size = tuple(a.shape[:2])
+				o.height, o.width = size
+			if fuse and size is None:
+				break
 		for name in ("K", "R", "C"):
 			getattr(o, name)[:] = list(np.asarray(v[name], np.float64).ravel())
-		nb = np.ascontiguousarray(v.get("neighbors", []), np.uint32)
-		keep.append(nb)
-		o.neighbors = nb.ctypes.data if nb.size else None
-		o.nNeighbors = int(nb.size)
-		o.nSceneNeighbors = int(v.get("n_scene_neighbors", nb.size))
-	prm = _lib.FuseParams(int(nMinViewsFuse), float(fDepthDiffThreshold), float(fNormalDiffThreshold), int(bool(bEstimateColor)), int(bool(bEstimateNormal)))
+		if fuse:
+			nb = np.ascontiguousarray(v.get("neighbors", []), np.uint32)
+			keep.append(nb)
+			o.neighbors = nb.ctypes.data if nb.size else None
+			o.nNeighbors = int(nb.size)
+			o.nSceneNeighbors = int(v.get("n_scene_neighbors", nb.size))
+	return arr, keep
+
+
+def _cloud_call(where: str, name: str, views, maps, params, fuse: bool = False) -> PointCloud:
+	"""FuseDepthMaps (fuse) or MergeDepthMaps -> PointCloud: b200mvs_<name> for numpy maps, or b200mvs_<name>_device on the context
+	of the device of the first tensor depth-map.  params: the fields of b200mvs_fuse_params."""
+	lib = _lib.load()
+	first = next((v["depth"] for v in views if _is_torch(v.get("depth"))), None)
+	device = None if first is None else _cuda_index(first)
+	arr, keep = _image_table(where, views, device, maps, fuse)
+	n, md, mn, color, normal = params
+	prm = _lib.FuseParams(int(n), float(md), float(mn), int(bool(color)), int(bool(normal)))
 	cloud = C.c_void_p()
 	if device is not None:
 		ctx = _device_context(first.device)
-		ctx._call("fuse_depth_maps_device", arr, n, C.byref(prm), C.byref(cloud), _stream_handle(ctx.device), C.byref(ctx.stats))
+		ctx._call(name + "_device", arr, len(views), C.byref(prm), C.byref(cloud), _stream_handle(ctx.device), C.byref(ctx.stats))
 	else:
-		rc = lib.b200mvs_fuse_depth_maps(arr, n, C.byref(prm), C.byref(cloud))
+		rc = getattr(lib, "b200mvs_" + name)(arr, len(views), C.byref(prm), C.byref(cloud))
 		if rc:
-			raise _lib.B200MVSError("b200mvs_fuse_depth_maps failed with status %d (bad view description)" % rc)
+			raise _lib.B200MVSError("b200mvs_%s failed with status %d (bad view description)" % (name, rc))
 	try:
-		return _point_cloud(lib, cloud)
+		return _point_cloud(lib, cloud, weights=fuse)
 	finally:
 		lib.b200mvs_pointcloud_free(cloud)
 

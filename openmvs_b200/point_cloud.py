@@ -11,29 +11,8 @@ import dataclasses
 import numpy as np
 
 from . import lib as _lib
-from .depth_estimator import PointCloud, _arg, _cuda_index, _device_context, _host, _is_torch, _point_cloud, _stream_handle
-
-
-def _image_table(where: str, views, device, maps):
-	"""the b200mvs_fuse_view table of the merge and point-cloud calls -> (table, keepalive).  maps: (key, dtype, channels) of the
-	maps the call reads; a map's size is the size of the first map given (depth, else color)."""
-	arr = (_lib.FuseView*len(views))()
-	keep = []
-	for i, v in enumerate(views):
-		o = arr[i]
-		size = None
-		for key, dt, ch in maps:
-			a = v.get(key)
-			a = a.contiguous() if _is_torch(a) and a.is_cuda else _host(a, dt, device)
-			keep.append(a)
-			shape = (None, None)+ch if size is None else size+ch
-			setattr(o, key, _arg(where, "views[%d].%s" % (i, key), a, dt, shape, device))
-			if a is not None and size is None:
-				size = tuple(a.shape[:2])
-				o.height, o.width = size
-		for name in ("K", "R", "C"):
-			getattr(o, name)[:] = list(np.asarray(v[name], np.float64).ravel())
-	return arr, keep
+from .depth_estimator import (PointCloud, _arg, _cloud_call, _cuda_index, _device_context, _host, _image_table, _is_torch,
+	_stream_handle)
 
 
 def MergeDepthMaps(views, bEstimateColor: bool = True, bEstimateNormal: bool = True) -> PointCloud:
@@ -43,30 +22,15 @@ def MergeDepthMaps(views, bEstimateColor: bool = True, bEstimateNormal: bool = T
 	on one device) b200mvs_merge_depth_maps_device on a context kept per device: the same cloud, bit for bit.  pointWeights is
 	None (the reference leaves them empty); an image with a depth-map needs a colour map with bEstimateColor and a normal map
 	with bEstimateNormal."""
-	lib = _lib.load()
-	first = next((v["depth"] for v in views if _is_torch(v.get("depth"))), None)
-	device = None if first is None else _cuda_index(first)
 	maps = (("depth", "float32", ()), ("normal", "float32", (3,)), ("color", "uint8", (3,)))
-	arr, keep = _image_table("MergeDepthMaps", views, device, maps)
-	prm = _lib.FuseParams(1, 0.01, 25.0, int(bool(bEstimateColor)), int(bool(bEstimateNormal)))
-	cloud = C.c_void_p()
-	if device is not None:
-		ctx = _device_context(first.device)
-		ctx._call("merge_depth_maps_device", arr, len(views), C.byref(prm), C.byref(cloud), _stream_handle(ctx.device), C.byref(ctx.stats))
-	else:
-		rc = lib.b200mvs_merge_depth_maps(arr, len(views), C.byref(prm), C.byref(cloud))
-		if rc:
-			raise _lib.B200MVSError("b200mvs_merge_depth_maps failed with status %d (bad view description)" % rc)
-	try:
-		return _point_cloud(lib, cloud, weights=False)
-	finally:
-		lib.b200mvs_pointcloud_free(cloud)
+	return _cloud_call("MergeDepthMaps", "merge_depth_maps", views, maps, (1, 0.01, 25.0, bEstimateColor, bEstimateNormal))
 
 
-def _cloud_args(where: str, views, pointcloud, maps):
-	"""the cloud and image arguments of EstimatePointColors / EstimatePointNormals -> (device index or None, context or None,
-	points, offsets, ids, image table, keepalive).  CUDA points take the device form: the view lists are flattened and copied to
-	the points' device."""
+def _per_point(where: str, name: str, views, pointcloud, maps, cols, dtype: str, extra=(), view_size=None):
+	"""b200mvs_<name> of the points of pointcloud -> the (n,)+cols output of dtype: the host-buffer form on device 0's context for
+	numpy points, a numpy array; the device form on the context of the points' device for CUDA points (the view lists are flattened
+	and copied there), a tensor on that device.  extra: the int arguments between the image count and the output; view_size(where,
+	i, view) -> (height, width) of each image in the table, where the call takes them from elsewhere than its maps."""
 	pts = pointcloud.points
 	device = _cuda_index(pts) if _is_torch(pts) and pts.is_cuda else None
 	pv = pointcloud.pointViews
@@ -85,8 +49,20 @@ def _cloud_args(where: str, views, pointcloud, maps):
 	po = _arg(where, "pointcloud view offsets", off, ("uint32", "int32"), (len(pv)+1,), device)
 	pi = _arg(where, "pointcloud view IDs", ids, ("uint32", "int32"), None, device)
 	arr, keep = _image_table(where, views, device, maps)
-	ctx = None if device is None else _device_context(pts.device)
-	return device, ctx, (p, len(pv), po, pi, arr, len(views)), [pts, off, ids, keep]
+	for i, v in enumerate(views if view_size else ()):
+		arr[i].height, arr[i].width = view_size(where, i, v)
+	n = len(pv)
+	args = (p, n, po, pi, arr, len(views)) + tuple(int(e) for e in extra)
+	if device is None:
+		out = np.zeros((n,)+cols, dtype)
+		ctx = _device_context(0)
+		ctx._call(name, *args, out.ctypes.data, C.byref(ctx.stats))
+	else:
+		import torch
+		out = torch.empty((n,)+cols, dtype=getattr(torch, dtype), device=pts.device)
+		ctx = _device_context(pts.device)
+		ctx._call(name + "_device", *args, out.data_ptr(), _stream_handle(ctx.device))
+	return out
 
 
 def EstimatePointColors(views, pointcloud: PointCloud) -> PointCloud:
@@ -94,18 +70,8 @@ def EstimatePointColors(views, pointcloud: PointCloud) -> PointCloud:
 	point's view of least depth, sampled bilinearly as the reference does (white without a view or outside the border).  views:
 	the scene images as dicts with color ((h, w, 3) uint8, None: empty image), K, R, C.  numpy points take the host-buffer form;
 	CUDA points (and colour maps on the same device) the device form, and colors is then a tensor."""
-	lib = _lib.load()
-	device, ctx, args, keep = _cloud_args("EstimatePointColors", views, pointcloud, (("color", "uint8", (3,)),))
-	n = args[1]
-	if device is None:
-		colors = np.zeros((n, 3), np.uint8)
-		ctx = _device_context(0)
-		ctx._call("estimate_point_colors", *args, colors.ctypes.data, C.byref(ctx.stats))
-	else:
-		import torch
-		colors = torch.empty((n, 3), dtype=torch.uint8, device=pointcloud.points.device)
-		ctx._call("estimate_point_colors_device", *args, colors.data_ptr(), _stream_handle(ctx.device))
-	pointcloud.colors = colors
+	pointcloud.colors = _per_point("EstimatePointColors", "estimate_point_colors", views, pointcloud, (("color", "uint8", (3,)),),
+		(3,), "uint8")
 	return pointcloud
 
 
@@ -114,18 +80,8 @@ def EstimatePointNormals(views, pointcloud: PointCloud, numNeighbors: int = 16) 
 	of each point's numNeighbors nearest points (exact search, ties to the lower index; DESIGN.md §5.6), turned towards the
 	camera of its first view.  views: the scene images as dicts with K, R, C.  numpy points take the host-buffer form, CUDA
 	points the device form (normals is then a tensor)."""
-	lib = _lib.load()
-	device, ctx, args, keep = _cloud_args("EstimatePointNormals", views, pointcloud, ())
-	n = args[1]
-	if device is None:
-		normals = np.zeros((n, 3), np.float32)
-		ctx = _device_context(0)
-		ctx._call("estimate_point_normals", *args, int(numNeighbors), normals.ctypes.data, C.byref(ctx.stats))
-	else:
-		import torch
-		normals = torch.empty((n, 3), dtype=torch.float32, device=pointcloud.points.device)
-		ctx._call("estimate_point_normals_device", *args, int(numNeighbors), normals.data_ptr(), _stream_handle(ctx.device))
-	pointcloud.normals = normals
+	pointcloud.normals = _per_point("EstimatePointNormals", "estimate_point_normals", views, pointcloud, (), (3,), "float32",
+		(numNeighbors,))
 	return pointcloud
 
 
@@ -153,34 +109,26 @@ def PointCloudVisibility(views, pointcloud: PointCloud):
 	return _visibility("PointCloudVisibility", views, pointcloud)
 
 
+def _view_size(where: str, i: int, v):
+	"""the size of a view of the visibility counts: width and height, or the shape of a depth or colour map"""
+	if v.get("width") is not None and v.get("height") is not None:
+		size = (v["height"], v["width"])
+	else:
+		m = next((v[k] for k in ("depth", "color") if v.get(k) is not None), None)
+		if m is None:
+			raise ValueError("%s: views[%d] needs width and height, or a depth or colour map to take them from" % (where, i))
+		size = tuple(m.shape[:2])
+	if not all(isinstance(s, (int, np.integer)) and 0 < int(s) < 2**31 for s in size):
+		raise ValueError("%s: views[%d] width and height must be positive integers; got %r" % (where, i, size[::-1]))
+	return int(size[0]), int(size[1])
+
+
 def _visibility(where: str, views, pointcloud: PointCloud):
 	rows = len(pointcloud.points) if hasattr(pointcloud.points, "__len__") else None
 	if rows is not None and rows != len(pointcloud.pointViews):
 		raise ValueError("%s: pointcloud.points must have one row per view list; got %d rows and %d lists" % (where, rows,
 			len(pointcloud.pointViews)))
-	device, ctx, args, keep = _cloud_args(where, views, pointcloud, ())
-	table = args[4]
-	for i, v in enumerate(views):
-		if v.get("width") is not None and v.get("height") is not None:
-			size = (v["height"], v["width"])
-		else:
-			m = next((v[k] for k in ("depth", "color") if v.get(k) is not None), None)
-			if m is None:
-				raise ValueError("%s: views[%d] needs width and height, or a depth or colour map to take them from" % (where, i))
-			size = tuple(m.shape[:2])
-		if not all(isinstance(s, (int, np.integer)) and 0 < int(s) < 2**31 for s in size):
-			raise ValueError("%s: views[%d] width and height must be positive integers; got %r" % (where, i, size[::-1]))
-		table[i].height, table[i].width = int(size[0]), int(size[1])
-	n = args[1]
-	if device is None:
-		vis = np.zeros(n, np.int32)
-		ctx = _device_context(0)
-		ctx._call("point_cloud_visibility", *args, vis.ctypes.data, C.byref(ctx.stats))
-	else:
-		import torch
-		vis = torch.empty(n, dtype=torch.int32, device=pointcloud.points.device)
-		ctx._call("point_cloud_visibility_device", *args, vis.data_ptr(), _stream_handle(ctx.device))
-	return vis
+	return _per_point(where, "point_cloud_visibility", views, pointcloud, (), (), "int32", view_size=_view_size)
 
 
 def PointCloudFilter(views, pointcloud: PointCloud, thRemove: int = 0) -> PointCloud:

@@ -183,6 +183,16 @@ void oracle_gap_interpolation(float* depth, float* normal, float* conf, int widt
 /* TImage<Pixel8U>::toGray(..., bNormalize = true) (libs/Common/Types.inl:2377-2431); stride in bytes */
 void oracle_to_gray(const uint8_t* src, int width, int height, int stride, int channels, int bgr, float* dst);
 
+/* ---- Scene::PointCloudFilter (libs/MVS/SceneDensify.cpp:2226-2360; visibility_oracle.cpp) ---- */
+/* the visibility counts of every (point, view) cone over every point.  pts: 3 floats per point; off: n + 1 view offsets, views:
+ * the image IDs; K: 9 doubles per image (row-major), C: 3 doubles per image, width: per image.  visibility: n ints, overwritten */
+int oracle_visibility(const float* pts, uint64_t n, const uint32_t* off, const uint32_t* views, int nImages, const double* K,
+	const double* C, const int* width, int threads, int32_t* visibility);
+/* The reference's removal loop, literally: RFOREACH(idxPoint, points) if (visibility[idxPoint] <= thRemove) RemovePoint(idxPoint),
+ * on an array of original indices; RemovePoint is cList::RemoveAt (libs/Common/List.h:1129-1136).  -> the number kept; order
+ * holds the kept original indices in their final slots */
+uint64_t oracle_visibility_filter(const int32_t* visibility, uint64_t n, int thRemove, uint32_t* order);
+
 #ifdef __cplusplus
 }
 #endif

@@ -89,6 +89,8 @@ PROTOTYPES = {
 	"oracle_count_asymmetric_edges": (I, [P, I, I, F]),
 	"oracle_gap_interpolation": (None, [P, P, P, I, I, F, U]),
 	"oracle_to_gray": (None, [P, I, I, I, I, I, P]),
+	"oracle_visibility": (I, [P, U64, P, P, I, P, P, P, I, P]),
+	"oracle_visibility_filter": (U64, [P, U64, I, P]),
 }
 
 

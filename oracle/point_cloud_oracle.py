@@ -4,16 +4,24 @@
   estimate_point_colors  EstimatePointColors               libs/MVS/DepthMap.cpp:1429-1465
   knn                    the neighbourhoods of EstimatePointNormals, brute force (DESIGN.md §5.6)
   estimate_point_normals EstimatePointNormals              libs/MVS/DepthMap.cpp:1469-1519
+  visibility             Scene::PointCloudFilter's counts  libs/MVS/SceneDensify.cpp:2226-2360
+  filter_order           its removal loop                  libs/MVS/SceneDensify.cpp:2226-2360
 
 Plain numpy, with the float32 / float64 operations in the reference's order, one elementwise operation at a time (numpy does
-not contract them), so the merge and the colours are bit-exact restatements.  Only tests/ and scripts/ may import this module;
-the product path is b200mvs_merge_depth_maps / b200mvs_estimate_point_* (openmvs_b200/csrc/cloud_host.cu).
+not contract them), so the merge and the colours are bit-exact restatements.  The visibility counts are exhaustive over every
+point, so they come from C++ (oracle/visibility_oracle.cpp in the parity build of the oracle library).  Only tests/ and
+scripts/ may import this module; the product path is b200mvs_merge_depth_maps / b200mvs_estimate_point_* /
+b200mvs_point_cloud_visibility (openmvs_b200/csrc/cloud_host.cu).
 parity unpinned: the reference has no golden vectors for these functions, and the normals come from CGAL, which is not in the
 reference tree (DESIGN.md §3, §8).
 """
 from __future__ import annotations
 
+import os
+
 import numpy as np
+
+from . import oracle as O
 
 F32 = np.float32
 
@@ -182,3 +190,34 @@ def estimate_point_normals(points, offsets, ids, Cs, nbr):
 	dot = ((nf[:, 0]*dv[:, 0]).astype(F32) + (nf[:, 1]*dv[:, 1]).astype(F32)).astype(F32) + (nf[:, 2]*dv[:, 2]).astype(F32)
 	nf[dot < 0] = -nf[dot < 0]
 	return nf, w
+
+
+def flat(pointViews):
+	"""per-point view lists -> (offsets (n+1,) uint32, IDs uint32)"""
+	off = np.zeros(len(pointViews)+1, np.uint32)
+	off[1:] = np.cumsum([len(v) for v in pointViews])
+	ids = np.concatenate([np.asarray(v, np.uint32).ravel() for v in pointViews]) if off[-1] else np.zeros(1, np.uint32)
+	return off, np.ascontiguousarray(ids, np.uint32)
+
+
+def visibility(points, pointViews, views, threads=None):
+	"""the counts of the single-threaded reference: points (n, 3) float32, pointViews per-point image IDs, views dicts with K, C
+	and width (or a depth / colour map) -> (n,) int32"""
+	pts = np.ascontiguousarray(points, np.float32)
+	off, ids = flat(pointViews)
+	K = np.ascontiguousarray([np.asarray(v["K"], np.float64).ravel() for v in views], np.float64)
+	Cs = np.ascontiguousarray([np.asarray(v["C"], np.float64).ravel() for v in views], np.float64)
+	W = np.array([v["width"] if v.get("width") is not None else (v["depth"] if v.get("depth") is not None else v["color"]).shape[1]
+		for v in views], np.int32)
+	out = np.zeros(len(pts), np.int32)
+	O.lib().oracle_visibility(pts.ctypes.data, len(pts), off.ctypes.data, ids.ctypes.data, len(views), K.ctypes.data, Cs.ctypes.data,
+		W.ctypes.data, int(threads or os.cpu_count() or 1), out.ctypes.data)
+	return out
+
+
+def filter_order(vis, thRemove):
+	"""the original indices of the kept points in the slots the reference's removal loop leaves them in"""
+	vis = np.ascontiguousarray(vis, np.int32)
+	order = np.zeros(max(len(vis), 1), np.uint32)
+	k = O.lib().oracle_visibility_filter(vis.ctypes.data, len(vis), int(thRemove), order.ctypes.data)
+	return order[:k].copy()

@@ -29,10 +29,10 @@ _CONVERT_MS = []
 _point_cloud = DE._point_cloud
 
 
-def _timed_point_cloud(lib, cloud):
+def _timed_point_cloud(lib, cloud, **kw):
 	t = time.perf_counter()
 	try:
-		return _point_cloud(lib, cloud)
+		return _point_cloud(lib, cloud, **kw)
 	finally:
 		_CONVERT_MS.append((time.perf_counter()-t)*1000.0)
 

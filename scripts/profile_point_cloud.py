@@ -59,13 +59,6 @@ def to_device(views):
 	return [dict(v, **{k: torch.from_numpy(np.ascontiguousarray(v[k])).cuda() for k in ("depth", "normal", "conf", "color")}) for v in views]
 
 
-def flat(pointViews):
-	"""per-point view lists -> (offsets, IDs)"""
-	off = np.zeros(len(pointViews)+1, np.int64)
-	off[1:] = np.cumsum(np.fromiter((len(v) for v in pointViews), np.int64, len(pointViews)))
-	return off, np.concatenate(pointViews)
-
-
 def merge_raw(ctx, dev):
 	"""b200mvs_merge_depth_maps_device without the per-point lists of MergeDepthMaps -> (points, offsets, IDs)"""
 	lib = ctx._lib
@@ -161,7 +154,7 @@ def main():
 		merged = merge_raw(ctx, dev)
 		ms.append(ctx.stats.ms_device)
 	row["ms_merge_device"] = min(ms[1:])
-	fused = (fused.points, *flat(fused.pointViews))
+	fused = (fused.points, *PO.flat(fused.pointViews))
 	arr, keep = _image_table("profile", dev, 0, (("color", "uint8", (3,)),))
 	stream = _stream_handle(ctx.device)
 	# the fused cloud with 16 far outliers (1000 times the scene's extent away), one view each

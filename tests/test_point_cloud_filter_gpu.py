@@ -1,5 +1,5 @@
 """Scene::PointCloudFilter on the device: the visibility counts of the host-buffer and device forms equal the exhaustive CPU
-restatement (tests/cpp/visibility_oracle.cpp) exactly, on the fused and the merged cloud of a synthetic scene and on adversarial
+restatement (oracle/visibility_oracle.cpp) exactly, on the fused and the merged cloud of a synthetic scene and on adversarial
 clouds; PointCloudFilter keeps the oracle's points in the reference's order; two runs are identical; and a 12 x 1080p fused cloud
 runs through both forms to the same counts."""
 import copy
@@ -11,9 +11,9 @@ pytestmark = pytest.mark.gpu
 
 torch = pytest.importorskip("torch")
 
-import visibility_oracle as VO  # noqa: E402
 from openmvs_b200 import synth  # noqa: E402
 from openmvs_b200.depth_estimator import FuseDepthMaps, MergeDepthMaps, PointCloud, PointCloudFilter, PointCloudVisibility  # noqa: E402
+from oracle import point_cloud_oracle as VO  # noqa: E402
 
 
 def _scene_views(w, h, n, noise, seed, drop=0.1, n_nb=4):

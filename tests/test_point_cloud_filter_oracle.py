@@ -1,11 +1,11 @@
 """Scene::PointCloudFilter without a GPU: hand-computed counts of the exhaustive CPU restatement
-(tests/cpp/visibility_oracle.cpp) for points on and around one ray, the library's removal order
+(oracle/visibility_oracle.cpp) for points on and around one ray, the library's removal order
 (b200mvs_pointcloud_remove_order) against the reference's literal loop, and the argument checks of the binding."""
 import numpy as np
 import pytest
 
-import visibility_oracle as VO
 from openmvs_b200.depth_estimator import PointCloud, PointCloudFilter, PointCloudVisibility
+from oracle import point_cloud_oracle as VO
 
 K = np.array([[500.0, 0, 320], [0, 500, 240], [0, 0, 1]])
 # camera 0 at the origin looking down +z; camera 1 at (0, 10, 10) looking down -y at the first point, so that its cone (and that
