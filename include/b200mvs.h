@@ -542,6 +542,53 @@ int b200mvs_point_cloud_visibility_device(b200mvs_ctx* ctx, const float* points,
  * in slot k afterwards, for k < *nKept.  Host code. */
 int b200mvs_pointcloud_remove_order(const uint8_t* remove, uint64_t n, uint32_t* order, uint64_t* nKept);
 
+/* ---- removals from the point cloud on the device (DESIGN.md §5.8) ------------------------------------------------------
+ * The same order on the device: remove (n bytes, nonzero = remove) and order (room for n entries) are DEVICE buffers; order[k]
+ * is written for k < *nKept only.  The chains of moved points are resolved by pointer jumping in ceil(log2 n) rounds.  *nKept
+ * is a HOST word, written after one synchronisation of `stream`.  At most 2^31 - 2 points. */
+int b200mvs_pointcloud_remove_order_device(b200mvs_ctx* ctx, const uint8_t* remove, uint64_t n, uint32_t* order, uint64_t* nKept,
+	void* stream);
+/* The cloud of nPoints points in the layout of the b200mvs_pointcloud accessors, gathered by order (nKept entries below nPoints)
+ * into the out* buffers, all DEVICE: points, normals (3 floats per point) and colors (3 bytes) each when given (NULL: skipped);
+ * with viewOffsets, the view lists: outViewOffsets (nKept + 1 entries from 0) and outViews, and outWeights / outProjs where
+ * weights / projs are given.  The view outputs need room for the input's viewOffsets[nPoints] entries, of which the first
+ * *nViewsKept (a HOST word, written after one synchronisation of `stream`) are written.  An order entry not below nPoints is
+ * refused (B200MVS_ERR_ARG). */
+int b200mvs_pointcloud_compact_device(b200mvs_ctx* ctx, const uint32_t* order, uint64_t nKept, uint64_t nPoints, const float* points,
+	const float* normals, const uint8_t* colors, const uint32_t* viewOffsets, const uint32_t* views, const float* weights,
+	const uint16_t* projs, float* outPoints, float* outNormals, uint8_t* outColors, uint32_t* outViewOffsets, uint32_t* outViews,
+	float* outWeights, uint16_t* outProjs, uint64_t* nViewsKept, void* stream);
+/* The remove mask of PointCloud::RemovePointsOutside(ROI) (libs/MVS/PointCloud.cpp:82-87) into remove (one byte per point, 1 =
+ * outside): !OBB3f::Intersects(X) of the box given as OBB3f holds it, rot (9 floats, world to box, row-major), pos (3, the centre) and
+ * ext (3, the half extents): |rot (X - pos)| <= ext per axis in float, each row summed r0 + (r1 + r2) with no FMA.  The
+ * ROI is obb with DenseReconstruction's fBorderROI applied (SceneDensify.cpp:1728): > 0 multiplies ext by it, < 0 adds
+ * -fBorderROI to ext, 0 keeps obb.  The host form is host code over HOST buffers; the _device form takes DEVICE points / remove,
+ * runs on `stream` and does not wait for it. */
+int b200mvs_point_cloud_outside_obb(const float* points, uint64_t nPoints, const float* rot, const float* pos, const float* ext,
+	float fBorderROI, uint8_t* remove);
+int b200mvs_point_cloud_outside_obb_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const float* rot, const float* pos,
+	const float* ext, float fBorderROI, uint8_t* remove, void* stream);
+/* The remove mask of PointCloud::RemoveMinViews(thMinViews) (libs/MVS/PointCloud.cpp:88-93): 1 where the point's view list
+ * (viewOffsets, nPoints + 1 entries) is shorter than thMinViews.  Forms as for the OBB mask. */
+int b200mvs_point_cloud_min_views(const uint32_t* viewOffsets, uint64_t nPoints, uint32_t thMinViews, uint8_t* remove);
+int b200mvs_point_cloud_min_views_device(b200mvs_ctx* ctx, const uint32_t* viewOffsets, uint64_t nPoints, uint32_t thMinViews,
+	uint8_t* remove, void* stream);
+/* Scene::EstimateROI(nEstimateROI, scale) (libs/MVS/Scene.cpp:1652-1740) of the cloud (the layout of the colour calls) seen from
+ * the scene images: an image is valid (Image::IsValid) when its width and height are positive; of images only the size and
+ * the camera (K, R, C) are read.  *bounded = 1 and rot / pos / ext (HOST, 9 / 3 / 3 floats, as the OBB mask takes them) are the
+ * ROI, an axis-aligned box (rot = I) of the core points' bounds enlarged by scale; or *bounded = 0 and they are untouched when the scene stays unbounded: nEstimateROI 0, no point, fewer than 3 valid
+ * images, no core point, or with nEstimateROI 2 an unbalanced mean viewing direction or a camera not facing the scene centre.
+ * The cameras are reduced on the host in the reference's types and order; a core point has a valid view that sees it at a depth
+ * below twice the scene radius; a zero bound is -0 when a core point has -0 there (the reference keeps the first zero it
+ * meets).  0 <= nEstimateROI <= 2, scale > 0, at most 2^31 - 1 points, view IDs below nImages (B200MVS_ERR_ARG otherwise).  The
+ * host form is host code (ctx nullable: it only receives the error text); the _device form takes DEVICE points / viewOffsets /
+ * views and a host `images` table, runs on `stream` and waits for it. */
+int b200mvs_estimate_roi(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets, const uint32_t* views,
+	const b200mvs_fuse_view* images, int nImages, int nEstimateROI, float scale, float* rot, float* pos, float* ext, int* bounded);
+int b200mvs_estimate_roi_device(b200mvs_ctx* ctx, const float* points, uint64_t nPoints, const uint32_t* viewOffsets, const uint32_t* views,
+	const b200mvs_fuse_view* images, int nImages, int nEstimateROI, float scale, float* rot, float* pos, float* ext, int* bounded,
+	void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -970,7 +970,7 @@ def FuseRoundStats():
 # The point-cloud calls after the fusion live in point_cloud.py, which builds on this module; they are re-exported here on first
 # use, so that either module can be imported first.
 _POINT_CLOUD_CALLS = ("MergeDepthMaps", "EstimatePointColors", "EstimatePointNormals", "PointKNN", "PointCloudVisibility",
-	"PointCloudFilter")
+	"PointCloudFilter", "OBB", "EstimateROI", "RemovePointsOutside", "RemoveMinViews")
 
 
 def __getattr__(name):

@@ -175,6 +175,14 @@ PROTOTYPES = {
 	"b200mvs_point_cloud_visibility": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, P, PStats]),
 	"b200mvs_point_cloud_visibility_device": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, P, P]),
 	"b200mvs_pointcloud_remove_order": (I, [P, U64, P, C.POINTER(U64)]),
+	"b200mvs_pointcloud_remove_order_device": (I, [P, P, U64, P, C.POINTER(U64), P]),
+	"b200mvs_pointcloud_compact_device": (I, [P, P, U64, U64, P, P, P, P, P, P, P, P, P, P, P, P, P, P, C.POINTER(U64), P]),
+	"b200mvs_point_cloud_outside_obb": (I, [P, U64, P, P, P, F, P]),
+	"b200mvs_point_cloud_outside_obb_device": (I, [P, P, U64, P, P, P, F, P, P]),
+	"b200mvs_point_cloud_min_views": (I, [P, U64, C.c_uint32, P]),
+	"b200mvs_point_cloud_min_views_device": (I, [P, P, U64, C.c_uint32, P, P]),
+	"b200mvs_estimate_roi": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, I, F, P, P, P, IP]),
+	"b200mvs_estimate_roi_device": (I, [P, P, U64, P, P, C.POINTER(FuseView), I, I, F, P, P, P, IP, P]),
 }
 SYMBOLS = list(PROTOTYPES)
 
